@@ -191,8 +191,10 @@ LHB200_API int32_t lhb200_shuffle_list(const uint64_t* input, uint64_t n, uint8_
  * *ok = 1 iff  prod_i e(r_i apk_i, H(m_i)) == e(g1, sum_i r_i sig_i)  and every set passed its checks
  * (non-empty, subgroup-checked signature; >= 1 key; aggregate key not at infinity).  n_sets == 0 -> *ok = 0
  * (blst.rs:42-44).  set_status (optional, n bytes): 0 fine, 1 empty sig, 2 sig decode, 3 sig not in subgroup,
- * 4 no keys, 5 aggregate key at infinity, 6 key decode.  fast_aggregate_verify / Signature::verify
- * (blst.rs:196-200, :250-261) are the n_sets == 1 case. */
+ * 4 no keys, 5 aggregate key at infinity, 6 key decode.  A set that fails several checks reports one code, in the
+ * order blst.rs:73-106 checks them: a signature failure (1, 2, 3) first, then no keys (4), then key decode (6), then
+ * the aggregate key at infinity (5).  fast_aggregate_verify / Signature::verify (blst.rs:196-200, :250-261) are the
+ * n_sets == 1 case. */
 LHB200_API int32_t lhb200_verify_signature_sets(const uint8_t* sigs, const uint8_t* msgs, const uint8_t* pks,
                                                 const uint32_t* pk_offsets, const uint64_t* rands, uint32_t n_sets,
                                                 uint8_t* ok, uint8_t* set_status);
@@ -234,6 +236,47 @@ LHB200_API int32_t lhb200_bls_batch_upload_indexed(lhb200_bls_batch* b, const lh
 /* Test hook: final-exponentiated product of the last verify as 12 x 48-byte big-endian Fp (tower order
  * c0.c0.c0 .. c1.c2.c1).  NOTE: this is the cube of the canonical GT element (3 is coprime to r). */
 LHB200_API int32_t lhb200_bls_batch_gt(lhb200_bls_batch* b, uint8_t out576[576]);
+/* Test hook: which kernels the last lhb200_bls_batch_verify_enqueue on `b` launched, so a test can tell which path a
+ * batch size exercised.  Writes min(n_words, LHB200_PLAN_WORDS) words, indexed by LHB200_PLAN_*; the stage words
+ * hold LHB200_K_* ids, 0 where the stage did not run (the sum tree of a single set). */
+#define LHB200_PLAN_WORDS 20
+#define LHB200_PLAN_N_SETS 0
+#define LHB200_PLAN_N_SM 1                    /* SM count the launch shapes were derived from */
+#define LHB200_PLAN_SIG 2
+#define LHB200_PLAN_SUM 3                     /* sum of r_i sig_i */
+#define LHB200_PLAN_SUM_LEVELS 4
+#define LHB200_PLAN_HASH 5
+#define LHB200_PLAN_KEY 6
+#define LHB200_PLAN_KEY_CHUNKS 7              /* streamed upload: chunks of whole sets; 0 = one launch */
+#define LHB200_PLAN_MILLER 8
+#define LHB200_PLAN_MILLER_WPB 9              /* warps per block (k_miller_warp, k_miller_coop) */
+#define LHB200_PLAN_MILLER_SPW 10             /* sets per warp (k_miller_warp: 1, k_miller_coop) or per thread (multi) */
+#define LHB200_PLAN_MILLER_GRID 11
+#define LHB200_PLAN_MILLER_ROUNDS_CAP 12      /* k_miller_coop: rounds of 30 sets per lane */
+#define LHB200_PLAN_MILLER_FEW_WARPS 13       /* k_miller_coop: 1 on the few-warps branch (small batches) */
+#define LHB200_PLAN_FP12_REDUCE_LEVELS 14
+#define LHB200_PLAN_N_TAIL 15                 /* Miller products the final kernel folds itself */
+#define LHB200_PLAN_FINAL 16
+#define LHB200_PLAN_LANE_GRID 17              /* blocks of the one-thread-per-set kernels */
+#define LHB200_PLAN_LANE_SETS_PER_THREAD 18   /* > 1 once the CTA cap makes them grid-stride */
+#define LHB200_PLAN_LAST_MILLER 19            /* 1 if k_last_miller ran (the pair -g1, sum r sig on its own) */
+#define LHB200_K_SIG_PREPARE 1
+#define LHB200_K_SIG_PREPARE_WARP 2
+#define LHB200_K_G2_REDUCE 3
+#define LHB200_K_G2_SUM_WARP 4
+#define LHB200_K_HASH_TO_G2 5
+#define LHB200_K_HASH_TO_G2_PAIR 6
+#define LHB200_K_HASH_TO_G2_WARP 7
+#define LHB200_K_PK_AGGREGATE 8
+#define LHB200_K_PK_PARTIAL_COMBINE 9
+#define LHB200_K_PK_AGGREGATE_TMA 10
+#define LHB200_K_PK_AGGREGATE_INDEXED 11
+#define LHB200_K_MILLER_MULTI 12
+#define LHB200_K_MILLER_COOP 13
+#define LHB200_K_MILLER_WARP 14
+#define LHB200_K_FINAL_COOP 15
+#define LHB200_K_FINAL_WARP 16
+LHB200_API int32_t lhb200_bls_batch_plan(const lhb200_bls_batch* b, uint32_t* out, uint32_t n_words);
 LHB200_API uint64_t lhb200_bls_batch_launches(const lhb200_bls_batch* b);
 /* Device time (ms) of the dominant kernel (k_miller) in the last completed enqueue, from CUDA events recorded on
  * the launching stream; < 0 if unavailable. */

@@ -95,6 +95,7 @@ _sig("lhb200_bls_batch_verify_enqueue", C.c_int32, vp, vp)
 _sig("lhb200_bls_batch_result", C.c_int32, vp, vp, vp, vp)
 _sig("lhb200_bls_batch_gt", C.c_int32, vp, vp)
 _sig("lhb200_bls_batch_launches", C.c_uint64, vp)
+_sig("lhb200_bls_batch_plan", C.c_int32, vp, vp, C.c_uint32)
 _sig("lhb200_sk_to_pk", C.c_int32, vp, C.c_uint32, vp, vp)
 _sig("lhb200_sign", C.c_int32, vp, vp, C.c_uint32, vp)
 _sig("lhb200_g1_decompress_validate", C.c_int32, vp, C.c_uint32, vp, vp)

@@ -401,6 +401,17 @@ class PubkeyTable:
             pass
 
 
+# word layout of lhb200_bls_batch_plan (LHB200_PLAN_* in include/lhb200.h) and its kernel ids (LHB200_K_*)
+PLAN_FIELDS = ("n_sets", "n_sm", "sig", "sum", "sum_levels", "hash", "key", "key_chunks", "miller", "miller_wpb",
+               "miller_spw", "miller_grid", "miller_rounds_cap", "miller_few_warps", "fp12_reduce_levels", "n_tail",
+               "final", "lane_grid", "lane_sets_per_thread", "last_miller")
+_PLAN_KERNEL_FIELDS = ("sig", "sum", "hash", "key", "miller", "final")
+PLAN_KERNELS = ("", "k_sig_prepare", "k_sig_prepare_warp", "k_g2_reduce", "k_g2_sum_warp", "k_hash_to_g2",
+                "k_hash_to_g2_pair", "k_hash_to_g2_warp", "k_pk_aggregate", "k_pk_partial+k_pk_combine",
+                "k_pk_aggregate_tma", "k_pk_aggregate_indexed", "k_miller_multi", "k_miller_coop", "k_miller_warp",
+                "k_final_coop", "k_final_warp")
+
+
 class Batch:
     """Staged verify (lhb200_bls_batch_*): device-resident inputs, enqueue on a stream, read the verdict."""
 
@@ -462,6 +473,13 @@ class Batch:
     @property
     def launches(self):
         return lib.lhb200_bls_batch_launches(self._h)
+
+    def plan(self):
+        """Kernels the last enqueue() launched (lhb200_bls_batch_plan test hook): a dict of the PLAN_FIELDS, with
+        kernel names for the stage fields ("" where a stage did not run)."""
+        w = np.zeros(len(PLAN_FIELDS), dtype=np.uint32)
+        check(lib.lhb200_bls_batch_plan(self._h, w.ctypes.data, len(w)), "lhb200_bls_batch_plan")
+        return {f: (PLAN_KERNELS[int(v)] if f in _PLAN_KERNEL_FIELDS else int(v)) for f, v in zip(PLAN_FIELDS, w)}
 
     @property
     def dominant_kernel_ms(self):

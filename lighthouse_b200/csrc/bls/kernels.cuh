@@ -19,6 +19,10 @@
 namespace lhb200 {
 namespace bls {
 
+// Per-set statuses.  The signature stage and the key stage run concurrently, so each writes an array of its own: the
+// signature kernels store failures (1-3) into `status` (zeroed before the launch), the key kernels store every set's
+// code (0, 4-6) into `pk_status`.  The Miller kernels skip a set unless both are 0, and lhb200_bls_batch_result merges
+// them with the signature code first, the order of the oracle's checks (blst.rs:73-106).
 enum SetStatus : uint8_t {
     SET_OK = 0,
     SET_EMPTY_SIG = 1,      // all-zero "empty" signature (generic_signature.rs:26) -> batch false (blst.rs:79-82)
@@ -88,7 +92,7 @@ __global__ void __launch_bounds__(BLS_BLOCK) k_sig_prepare(const uint8_t* __rest
 __global__ void __launch_bounds__(BLS_BLOCK) k_pk_aggregate(const uint8_t* __restrict__ pks,
                                                              const uint32_t* __restrict__ offsets,
                                                              const uint64_t* __restrict__ rands, uint32_t n,
-                                                             G1Proj3* __restrict__ out_p, uint8_t* __restrict__ status,
+                                                             G1Proj3* __restrict__ out_p, uint8_t* __restrict__ pk_status,
                                                              uint32_t* __restrict__ fail) {
     // grid-stride: the host caps resident CTAs per SM so the per-thread stacks stay cache-resident
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -114,7 +118,8 @@ __global__ void __launch_bounds__(BLS_BLOCK) k_pk_aggregate(const uint8_t* __res
             P.px = FP_ONE; P.py = FP_ONE; P.pz = FP_ONE;
         }
         out_p[i] = P;
-        if (st != SET_OK) { status[i] = st; atomicOr(fail, 1u); }
+        pk_status[i] = st;
+        if (st != SET_OK) atomicOr(fail, 1u);
     }
 }
 
@@ -151,7 +156,7 @@ __global__ void __launch_bounds__(BLS_BLOCK) k_pk_combine(const G1Jac* __restric
                                                            const uint8_t* __restrict__ part_bad,
                                                            const uint32_t* __restrict__ offsets,
                                                            const uint64_t* __restrict__ rands, uint32_t n,
-                                                           G1Proj3* __restrict__ out_p, uint8_t* __restrict__ status,
+                                                           G1Proj3* __restrict__ out_p, uint8_t* __restrict__ pk_status,
                                                            uint32_t* __restrict__ fail) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -175,7 +180,8 @@ __global__ void __launch_bounds__(BLS_BLOCK) k_pk_combine(const G1Jac* __restric
         P.px = FP_ONE; P.py = FP_ONE; P.pz = FP_ONE;
     }
     out_p[i] = P;
-    if (st != SET_OK) { status[i] = st; atomicOr(fail, 1u); }
+    pk_status[i] = st;
+    if (st != SET_OK) atomicOr(fail, 1u);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -248,7 +254,7 @@ __device__ __forceinline__ int32_t g1_from_uncompressed_words(G1Affine& r, const
 __global__ void __launch_bounds__(BLS_BLOCK) k_pk_aggregate_tma(const uint8_t* __restrict__ pks,
                                                                  const uint32_t* __restrict__ offsets,
                                                                  const uint64_t* __restrict__ rands, uint32_t n,
-                                                                 G1Proj3* __restrict__ out_p, uint8_t* __restrict__ status,
+                                                                 G1Proj3* __restrict__ out_p, uint8_t* __restrict__ pk_status,
                                                                  uint32_t* __restrict__ fail) {
     __shared__ __align__(128) uint8_t ring[PK_TMA_STAGES][BLS_BLOCK][PK_TMA_SLOT];
     __shared__ __align__(8) uint64_t bars[PK_TMA_STAGES];
@@ -312,7 +318,8 @@ __global__ void __launch_bounds__(BLS_BLOCK) k_pk_aggregate_tma(const uint8_t* _
         P.px = FP_ONE; P.py = FP_ONE; P.pz = FP_ONE;
     }
     out_p[i] = P;
-    if (st != SET_OK) { status[i] = st; atomicOr(fail, 1u); }
+    pk_status[i] = st;
+    if (st != SET_OK) atomicOr(fail, 1u);
 }
 
 // Device-resident pubkey table (mirror of ValidatorPubkeyCache, beacon_chain/src/validator_pubkey_cache.rs:20-25):
@@ -342,7 +349,7 @@ __global__ void __launch_bounds__(BLS_BLOCK) k_pk_aggregate_indexed(const G1Mont
                                                                      const uint32_t* __restrict__ offsets,
                                                                      const uint64_t* __restrict__ rands, uint32_t n,
                                                                      G1Proj3* __restrict__ out_p,
-                                                                     uint8_t* __restrict__ status,
+                                                                     uint8_t* __restrict__ pk_status,
                                                                      uint32_t* __restrict__ fail) {
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const uint32_t lo = offsets[i], hi = offsets[i + 1];
@@ -368,7 +375,8 @@ __global__ void __launch_bounds__(BLS_BLOCK) k_pk_aggregate_indexed(const G1Mont
             P.px = FP_ONE; P.py = FP_ONE; P.pz = FP_ONE;
         }
         out_p[i] = P;
-        if (st != SET_OK) { status[i] = st; atomicOr(fail, 1u); }
+        pk_status[i] = st;
+        if (st != SET_OK) atomicOr(fail, 1u);
     }
 }
 
@@ -421,14 +429,15 @@ __global__ void __launch_bounds__(BLS_BLOCK) k_hash_to_g2_pair(const uint8_t* __
 // Group g = sets [g*k, (g+1)*k): one thread runs their Miller loops with shared squarings; out_f[g] = the product.
 // The host picks k = ceil(n / resident threads) so that every resident thread gets one group (no partial last wave).
 __global__ void __launch_bounds__(MILLER_BLOCK) k_miller_multi(const G1Proj3* __restrict__ P, const G2Jac* __restrict__ H,
-                                                             const uint8_t* __restrict__ status, uint32_t n, uint32_t k,
+                                                             const uint8_t* __restrict__ status,
+                                                             const uint8_t* __restrict__ pk_status, uint32_t n, uint32_t k,
                                                              uint32_t n_groups, Fp12* __restrict__ out_f) {
     for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < n_groups; g += gridDim.x * blockDim.x) {
         uint32_t idx[MILLER_KMAX];
         int m = 0;
         for (uint32_t j = 0; j < k; j++) {
             const uint32_t i = g * k + j;
-            if (i < n && status[i] == SET_OK && !jac_is_inf(H[i])) idx[m++] = i;
+            if (i < n && (status[i] | pk_status[i]) == SET_OK && !jac_is_inf(H[i])) idx[m++] = i;
         }
         Fp12 f;
         if (m == 0) fp12_set_one(f);

@@ -90,8 +90,9 @@ constexpr int lanes_used() { return Geom<NT>::LANES_USED; }
 struct Args {
     const G1Proj3* P;
     const G2Jac* H;
-    const uint8_t* status;
-    uint32_t n;                // sets in P / H / status
+    const uint8_t* status;     // signature stage
+    const uint8_t* pk_status = nullptr;   // key stage; null: only `status` marks the sets to skip
+    uint32_t n;                // sets in P / H / status / pk_status
     const G2Jac* extra_q;      // nullable: the pair (*extra_p, *extra_q) = (-g1, sum r sig) is appended as set n
     const G1Proj3* extra_p;
     uint32_t lo, hi;           // this warp's sets [lo, hi)
@@ -132,7 +133,7 @@ LHB_HD LHB_INLINE void lane_select(Lane<NT>& L, const Args& a, uint32_t r) {
     bool act = L.set < a.hi && L.set < n_total;
     if (act) {
         if (L.set >= a.n) { L.extra = true; act = !jac_is_inf(*a.extra_q); }
-        else act = a.status[L.set] == 0 && !jac_is_inf(a.H[L.set]);
+        else act = (a.status[L.set] | (a.pk_status ? a.pk_status[L.set] : 0)) == 0 && !jac_is_inf(a.H[L.set]);
     }
     L.active = act;
     L.act[L.lane] = act ? 1 : 0;
@@ -416,7 +417,8 @@ constexpr size_t mc_smem_bytes() { return Geom<32>::REGION_WORDS * 4 * MC_WARPS;
 // cooperative w-basis product), so the kernel emits ONE Miller value per block: out_f[blockIdx.x].  scratch: per warp
 // sets_per_warp rounded up to whole rounds of 30, 2 * TWORDS words per lane and round.
 __global__ void __launch_bounds__(32 * MC_WARPS, 1) k_miller_coop(const G1Proj3* __restrict__ P, const G2Jac* __restrict__ H,
-                                                                   const uint8_t* __restrict__ status, uint32_t n,
+                                                                   const uint8_t* __restrict__ status,
+                                                                   const uint8_t* __restrict__ pk_status, uint32_t n,
                                                                    const G2Jac* __restrict__ extra_q,
                                                                    const G1Proj3* __restrict__ extra_p,
                                                                    uint32_t sets_per_warp, uint32_t* __restrict__ scratch,
@@ -434,7 +436,7 @@ __global__ void __launch_bounds__(32 * MC_WARPS, 1) k_miller_coop(const G1Proj3*
     L.active = false; L.extra = false; L.set = 0;
     const uint32_t n_total = n + (extra_q ? 1u : 0u);
     Args a;
-    a.P = P; a.H = H; a.status = status; a.n = n; a.extra_q = extra_q; a.extra_p = extra_p;
+    a.P = P; a.H = H; a.status = status; a.pk_status = pk_status; a.n = n; a.extra_q = extra_q; a.extra_p = extra_p;
     a.lo = min(n_total, gw * sets_per_warp);
     a.hi = min(n_total, a.lo + sets_per_warp);
     const uint32_t rounds_cap = (sets_per_warp + Geom<NT>::LANES_USED - 1) / Geom<NT>::LANES_USED;

@@ -176,10 +176,11 @@ LHB_HD LHB_INLINE void set_one_words(uint32_t* R, int word) {   // word < 24 * S
 constexpr size_t smem_bytes(int warps) { return ((size_t)warps * REGION_WORDS + table_words(MW_N_MUL, MW_N_LIN, MW_N_PHASES)) * 4; }
 #if !defined(LHB_HOSTSIM)
 // One warp per pair (P_i, H_i), i < n, plus the pair (extra_p, extra_q) = (-g1, sum r sig) as pair n.  Invalid sets
-// (status != 0, H at infinity) contribute f = 1, like k_miller_coop.  The warps of a block multiply their values
+// (status or pk_status != 0, H at infinity) contribute f = 1, like k_miller_coop.  The warps of a block multiply their values
 // (dense section) and the block writes ONE Fp12.  Dynamic shared memory: smem_bytes(warps_per_block).
 __global__ void __launch_bounds__(256, 1) k_miller_warp(const G1Proj3* __restrict__ P, const G2Jac* __restrict__ H,
-                                                        const uint8_t* __restrict__ status, uint32_t n,
+                                                        const uint8_t* __restrict__ status,
+                                                        const uint8_t* __restrict__ pk_status, uint32_t n,
                                                         const G2Jac* __restrict__ extra_q, const G1Proj3* __restrict__ extra_p,
                                                         Fp12* __restrict__ out_f) {
     const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
@@ -193,7 +194,7 @@ __global__ void __launch_bounds__(256, 1) k_miller_warp(const G1Proj3* __restric
     const G1Proj3* p = nullptr;
     if (active) {
         if (set >= n) { q = extra_q; p = extra_p; }
-        else { q = H + set; p = P + set; active = status[set] == 0; }
+        else { q = H + set; p = P + set; active = (status[set] | pk_status[set]) == 0; }
         if (active) active = !jac_is_inf(*q);
     }
     if (active) {   // warp-uniform

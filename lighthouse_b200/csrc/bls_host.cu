@@ -61,10 +61,11 @@ struct lhb200_bls_batch {
     Fp12* d_f_tmp[2] = {nullptr, nullptr};
     Fp12* d_flast = nullptr;
     Fp12* d_gt = nullptr;
-    uint8_t* d_status = nullptr;
+    uint8_t* d_status = nullptr;     // signature-stage codes (1-3), zeroed per verify
+    uint8_t* d_pk_status = nullptr;  // key-stage codes (0, 4-6), written for every set by the key kernels
     uint32_t* d_fail = nullptr;
     uint8_t* d_ok = nullptr;
-    uint8_t* h_res = nullptr;     // pinned: ok + status
+    uint8_t* h_res = nullptr;     // pinned: ok, status (at 64), pk_status (at 64 + cap_sets)
     cudaStream_t s_main = nullptr;   // the stream lhb200_verify_signature_sets drives this handle on (one per handle)
     cudaStream_t s2 = nullptr, s3 = nullptr;
     cudaEvent_t e_h2c = nullptr, e_sig = nullptr;
@@ -92,6 +93,7 @@ struct lhb200_bls_batch {
     const uint8_t* h_pks = nullptr;          // caller's host keys (valid until result)
     int n_chunks = 0;                        // 0: inputs already complete on the device
     std::vector<uint64_t> rbuf;              // scalars drawn by the library (must outlive the async copy)
+    uint32_t plan[LHB200_PLAN_WORDS] = {};   // kernels the last verify_enqueue chose (lhb200_bls_batch_plan)
 };
 
 static void batch_free(lhb200_bls_batch* b) {
@@ -99,7 +101,8 @@ static void batch_free(lhb200_bls_batch* b) {
     if (b->d_indices) cudaFree(b->d_indices);
     void* ptrs[] = {b->d_sigs, b->d_msgs, b->d_pks, b->d_offsets, b->d_rands, b->d_sigr, b->d_sig_tmp[0],
                     b->d_sig_tmp[1], b->d_p, b->d_h, b->d_f, b->d_f_tmp[0], b->d_f_tmp[1], b->d_flast, b->d_gt,
-                    b->d_status, b->d_fail, b->d_ok, b->d_mc_scratch, b->d_neg_g1, b->d_pk_part, b->d_pk_part_bad};
+                    b->d_status, b->d_pk_status, b->d_fail, b->d_ok, b->d_mc_scratch, b->d_neg_g1, b->d_pk_part,
+                    b->d_pk_part_bad};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     if (b->h_res) cudaFreeHost(b->h_res);
@@ -309,13 +312,14 @@ int32_t lhb200_bls_batch_create(uint32_t max_sets, uint64_t max_keys, lhb200_bls
     ALLOC(b->d_flast, sizeof(Fp12));
     ALLOC(b->d_gt, sizeof(Fp12));
     ALLOC(b->d_status, n);
+    ALLOC(b->d_pk_status, n);
     ALLOC(b->d_fail, 4);
     ALLOC(b->d_ok, 4);
     ALLOC(b->d_neg_g1, sizeof(G1Proj3));
     ALLOC(b->d_pk_part, std::min<uint64_t>(n, PK_SPLIT_MAX_SETS) * PK_SLICES * sizeof(G1Jac));
     ALLOC(b->d_pk_part_bad, std::min<uint64_t>(n, PK_SPLIT_MAX_SETS) * PK_SLICES);
 #undef ALLOC
-    cudaError_t e = cudaHostAlloc(reinterpret_cast<void**>(&b->h_res), n + 64 + sizeof(Fp12), cudaHostAllocDefault);
+    cudaError_t e = cudaHostAlloc(reinterpret_cast<void**>(&b->h_res), 2 * n + 64 + sizeof(Fp12), cudaHostAllocDefault);
     if (e != cudaSuccess) { batch_free(b); return cuda_fail(e, "cudaHostAlloc(result)"); }
     if ((e = cudaStreamCreateWithFlags(&b->s_main, cudaStreamNonBlocking)) != cudaSuccess ||
         (e = cudaStreamCreateWithFlags(&b->s2, cudaStreamNonBlocking)) != cudaSuccess ||
@@ -643,6 +647,12 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
         grid = cdiv(n, (uint64_t)per_thread * BLS_BLOCK);
     }
     uint64_t launches = 0;
+    uint32_t* plan = b->plan;
+    memset(plan, 0, sizeof b->plan);
+    plan[LHB200_PLAN_N_SETS] = n;
+    plan[LHB200_PLAN_N_SM] = (uint32_t)n_sm;
+    plan[LHB200_PLAN_LANE_GRID] = grid;
+    plan[LHB200_PLAN_LANE_SETS_PER_THREAD] = cdiv(n, (uint64_t)grid * BLS_BLOCK);
     // key ingest through the TMA unit (bulk async copies into a shared-memory ring); needs 16-byte aligned keys.
     // Opt-in (LHB_PK_TMA=1): on the H100 the plain kernel is faster at every size measured (100 000 sets x 128 keys:
     // 111.8 against 119.5 ms per step; 40 000 sets: 49.0 against 53.3 ms).  The ring needs a shared-memory carve-out,
@@ -675,6 +685,7 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
         }();
         if (!gw_attr_ok) { set_error("g2 warp kernels: cannot reserve %zu B of shared memory", gw_smem); return LHB200_ECUDA; }
     }
+    plan[LHB200_PLAN_SIG] = g2_warp ? LHB200_K_SIG_PREPARE_WARP : LHB200_K_SIG_PREPARE;
     if (g2_warp)
         gw::k_sig_prepare_warp<<<cdiv(n, GW_WPB), 32 * GW_WPB, gw_smem, b->s2>>>(b->in_sigs, b->in_rands, n, b->d_sigr,
                                                                                b->d_status, b->d_fail);
@@ -692,6 +703,8 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
                 const uint32_t mo = cdiv(m, CH);
                 gw::k_g2_sum_warp<<<cdiv(mo, GW_WPB), 32 * GW_WPB, gw_smem, b->s2>>>(cur, m, CH, b->d_sig_tmp[flip]);
                 launches++;
+                plan[LHB200_PLAN_SUM] = LHB200_K_G2_SUM_WARP;
+                plan[LHB200_PLAN_SUM_LEVELS]++;
                 cur = b->d_sig_tmp[flip];
                 flip ^= 1;
                 m = mo;
@@ -700,6 +713,8 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
             const uint32_t mo = cdiv(m, REDUCE_CHUNK);
             k_g2_reduce<<<cdiv(mo, BLS_BLOCK), BLS_BLOCK, 0, b->s2>>>(cur, m, REDUCE_CHUNK, b->d_sig_tmp[flip]);
             launches++;
+            plan[LHB200_PLAN_SUM] = LHB200_K_G2_REDUCE;
+            plan[LHB200_PLAN_SUM_LEVELS]++;
             cur = b->d_sig_tmp[flip];
             flip ^= 1;
             m = mo;
@@ -709,9 +724,12 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
         if (!miller_coop_s2) {
             k_last_miller<<<1, 32, 0, b->s2>>>(cur, b->d_flast);
             launches++;
+            plan[LHB200_PLAN_LAST_MILLER] = 1;
         }
         LHB_CUDA(cudaEventRecord(b->e_join, b->s2));
     }
+    plan[LHB200_PLAN_HASH] = g2_warp ? LHB200_K_HASH_TO_G2_WARP
+                             : n <= HASH_PAIR_MAX_SETS ? LHB200_K_HASH_TO_G2_PAIR : LHB200_K_HASH_TO_G2;
     if (g2_warp)
         gw::k_hash_to_g2_warp<<<cdiv(n, GW_WPB), 32 * GW_WPB, gw_smem, b->s3>>>(b->in_msgs, n, b->d_h);
     else if (n <= HASH_PAIR_MAX_SETS)   // latency mode: two threads per message (one SSWU map each)
@@ -725,24 +743,28 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
     auto launch_pk = [&](uint32_t lo, uint32_t cnt, cudaStream_t st) {
         if (pk_tma) {
             k_pk_aggregate_tma<<<cdiv(cnt, BLS_BLOCK), BLS_BLOCK, 0, st>>>(b->in_pks, b->in_offsets + lo, b->in_rands + lo, cnt,
-                                                                          b->d_p + lo, b->d_status + lo, b->d_fail);
+                                                                          b->d_p + lo, b->d_pk_status + lo, b->d_fail);
         } else if (n <= PK_SPLIT_MAX_SETS) {
             k_pk_partial<<<cdiv(cnt * PK_SLICES, BLS_BLOCK), BLS_BLOCK, 0, st>>>(
                 b->in_pks, b->in_offsets + lo, cnt, b->d_pk_part + (size_t)lo * PK_SLICES, b->d_pk_part_bad + (size_t)lo * PK_SLICES);
             k_pk_combine<<<cdiv(cnt, BLS_BLOCK), BLS_BLOCK, 0, st>>>(
                 b->d_pk_part + (size_t)lo * PK_SLICES, b->d_pk_part_bad + (size_t)lo * PK_SLICES, b->in_offsets + lo,
-                b->in_rands + lo, cnt, b->d_p + lo, b->d_status + lo, b->d_fail);
+                b->in_rands + lo, cnt, b->d_p + lo, b->d_pk_status + lo, b->d_fail);
             launches++;
         } else {
             k_pk_aggregate<<<std::min<uint32_t>(grid, cdiv(cnt, BLS_BLOCK)), BLS_BLOCK, 0, st>>>(
-                b->in_pks, b->in_offsets + lo, b->in_rands + lo, cnt, b->d_p + lo, b->d_status + lo, b->d_fail);
+                b->in_pks, b->in_offsets + lo, b->in_rands + lo, cnt, b->d_p + lo, b->d_pk_status + lo, b->d_fail);
         }
         launches++;
     };
+    plan[LHB200_PLAN_KEY] = b->table ? LHB200_K_PK_AGGREGATE_INDEXED
+                            : pk_tma ? LHB200_K_PK_AGGREGATE_TMA
+                            : n <= PK_SPLIT_MAX_SETS ? LHB200_K_PK_PARTIAL_COMBINE : LHB200_K_PK_AGGREGATE;
+    plan[LHB200_PLAN_KEY_CHUNKS] = b->table ? 0 : (uint32_t)b->n_chunks;
     if (b->table) {
         launches++;
         k_pk_aggregate_indexed<<<grid, BLS_BLOCK, 0, s>>>(b->table->d_keys, (uint32_t)b->table->len, b->in_indices,
-                                                         b->in_offsets, b->in_rands, n, b->d_p, b->d_status, b->d_fail);
+                                                         b->in_offsets, b->in_rands, n, b->d_p, b->d_pk_status, b->d_fail);
     } else if (b->n_chunks) {
         // big pageable key buffers go through the library's pinned ring (see KeyStager)
         static const int stage_env = [] { const char* e = getenv("LHB_STAGE_PAGEABLE"); return e ? atoi(e) : 1; }();
@@ -809,8 +831,12 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
             const uint32_t mgrid = cdiv(n_total, wpb);
             LHB_CUDA(cudaStreamWaitEvent(s, b->e_join, 0));   // sum r sig (and -g1) ready
             LHB_CUDA(cudaEventRecord(b->e_k0, s));
-            mw::k_miller_warp<<<mgrid, 32 * wpb, mw::smem_bytes((int)wpb), s>>>(b->d_p, b->d_h, b->d_status, n,
-                                                                                         b->d_sig_sum, b->d_neg_g1, b->d_f);
+            mw::k_miller_warp<<<mgrid, 32 * wpb, mw::smem_bytes((int)wpb), s>>>(b->d_p, b->d_h, b->d_status, b->d_pk_status,
+                                                                                n, b->d_sig_sum, b->d_neg_g1, b->d_f);
+            plan[LHB200_PLAN_MILLER] = LHB200_K_MILLER_WARP;
+            plan[LHB200_PLAN_MILLER_WPB] = wpb;
+            plan[LHB200_PLAN_MILLER_SPW] = 1;
+            plan[LHB200_PLAN_MILLER_GRID] = mgrid;
             LHB_CUDA(cudaEventRecord(b->e_k1, s));
             launches += 1;
             uint32_t m = mgrid;
@@ -819,6 +845,7 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
                 const uint32_t mo = cdiv(m, REDUCE_CHUNK);
                 k_fp12_reduce<<<cdiv(mo, BLS_BLOCK), BLS_BLOCK, 0, s>>>(cur, m, REDUCE_CHUNK, b->d_f_tmp[flip]);
                 launches++;
+                plan[LHB200_PLAN_FP12_REDUCE_LEVELS]++;
                 cur = b->d_f_tmp[flip];
                 flip ^= 1;
                 m = mo;
@@ -856,8 +883,15 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
         }
         LHB_CUDA(cudaStreamWaitEvent(s, b->e_join, 0));   // sum r sig (and -g1) ready
         LHB_CUDA(cudaEventRecord(b->e_k0, s));
-        mc::k_miller_coop<<<mgrid, 32 * mc::MC_WARPS, mc::mc_smem_bytes(), s>>>(b->d_p, b->d_h, b->d_status, n, b->d_sig_sum,
-                                                                                b->d_neg_g1, spw, b->d_mc_scratch, b->d_f);
+        mc::k_miller_coop<<<mgrid, 32 * mc::MC_WARPS, mc::mc_smem_bytes(), s>>>(b->d_p, b->d_h, b->d_status, b->d_pk_status,
+                                                                                n, b->d_sig_sum, b->d_neg_g1, spw,
+                                                                                b->d_mc_scratch, b->d_f);
+        plan[LHB200_PLAN_MILLER] = LHB200_K_MILLER_COOP;
+        plan[LHB200_PLAN_MILLER_WPB] = mc::MC_WARPS;
+        plan[LHB200_PLAN_MILLER_SPW] = spw;
+        plan[LHB200_PLAN_MILLER_GRID] = mgrid;
+        plan[LHB200_PLAN_MILLER_ROUNDS_CAP] = rounds_cap;
+        plan[LHB200_PLAN_MILLER_FEW_WARPS] = n_total <= FEW_WARPS * LU;
         LHB_CUDA(cudaEventRecord(b->e_k1, s));
         launches += 1;
         uint32_t m = mgrid;   // the kernel multiplies groups and warps together: one value per block
@@ -869,6 +903,7 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
             const uint32_t mo = cdiv(m, REDUCE_CHUNK);
             k_fp12_reduce<<<cdiv(mo, BLS_BLOCK), BLS_BLOCK, 0, s>>>(cur, m, REDUCE_CHUNK, b->d_f_tmp[flip]);
             launches++;
+            plan[LHB200_PLAN_FP12_REDUCE_LEVELS]++;
             cur = b->d_f_tmp[flip];
             flip ^= 1;
             m = mo;
@@ -890,8 +925,11 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
     uint32_t mk = miller_k_env > 0 ? (uint32_t)miller_k_env : cdiv(n, resident);
     mk = std::min<uint32_t>(std::max<uint32_t>(mk, 1), MILLER_KMAX);
     const uint32_t n_groups = cdiv(n, mk);
-    k_miller_multi<<<std::min<uint32_t>(cdiv(n_groups, MILLER_BLOCK), (uint32_t)(n_sm * miller_occ)), MILLER_BLOCK, 0, s>>>(
-        b->d_p, b->d_h, b->d_status, n, mk, n_groups, b->d_f);
+    const uint32_t mgrid = std::min<uint32_t>(cdiv(n_groups, MILLER_BLOCK), (uint32_t)(n_sm * miller_occ));
+    k_miller_multi<<<mgrid, MILLER_BLOCK, 0, s>>>(b->d_p, b->d_h, b->d_status, b->d_pk_status, n, mk, n_groups, b->d_f);
+    plan[LHB200_PLAN_MILLER] = LHB200_K_MILLER_MULTI;
+    plan[LHB200_PLAN_MILLER_SPW] = mk;
+    plan[LHB200_PLAN_MILLER_GRID] = mgrid;
     LHB_CUDA(cudaEventRecord(b->e_k1, s));
     launches += 1;
     {
@@ -901,6 +939,7 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
             const uint32_t mo = cdiv(m, REDUCE_CHUNK);
             k_fp12_reduce<<<cdiv(mo, BLS_BLOCK), BLS_BLOCK, 0, s>>>(cur, m, REDUCE_CHUNK, b->d_f_tmp[flip]);
             launches++;
+            plan[LHB200_PLAN_FP12_REDUCE_LEVELS]++;
             cur = b->d_f_tmp[flip];
             flip ^= 1;
             m = mo;
@@ -916,8 +955,12 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
         }();
         if (!fe_attr_ok) { set_error("k_final_warp: cannot reserve shared memory"); return LHB200_ECUDA; }
         fe::k_final_warp<<<1, 32 * fe::FE_WARPS, fe::smem_bytes(), s>>>(cur, n_tail, b->d_fail, b->d_ok, b->d_gt);
-    } else
+        plan[LHB200_PLAN_FINAL] = LHB200_K_FINAL_WARP;
+    } else {
         k_final_coop<<<1, COOP_THREADS, sizeof(CoopFinalSmem), s>>>(cur, n_tail, f_last, b->d_fail, b->d_ok, b->d_gt);
+        plan[LHB200_PLAN_FINAL] = LHB200_K_FINAL_COOP;
+    }
+    plan[LHB200_PLAN_N_TAIL] = n_tail;
     launches++;
     LHB_CUDA(cudaGetLastError());
     count_launch(launches);
@@ -940,7 +983,12 @@ int32_t lhb200_bls_batch_result(lhb200_bls_batch* b, void* stream, uint8_t* ok, 
     if (!b || !ok) return LHB200_EINVAL;
     cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx().stream;
     LHB_CUDA(cudaMemcpyAsync(b->h_res, b->d_ok, 1, cudaMemcpyDeviceToHost, s));
-    if (set_status) LHB_CUDA(cudaMemcpyAsync(b->h_res + 64, b->d_status, b->n, cudaMemcpyDeviceToHost, s));
+    uint8_t* const h_sig = b->h_res + 64;
+    uint8_t* const h_pk = h_sig + b->cap_sets;
+    if (set_status) {
+        LHB_CUDA(cudaMemcpyAsync(h_sig, b->d_status, b->n, cudaMemcpyDeviceToHost, s));
+        LHB_CUDA(cudaMemcpyAsync(h_pk, b->d_pk_status, b->n, cudaMemcpyDeviceToHost, s));
+    }
     if (b->n >= BLOCKING_WAIT_MIN_SETS && b->e_done) {
         // a long step: sleep on a blocking event instead of spinning in cudaStreamSynchronize — with one process per GPU
         // on a shared host (8 ranks + NCCL proxies under one cgroup CPU quota) eight spinning threads get throttled and
@@ -951,7 +999,9 @@ int32_t lhb200_bls_batch_result(lhb200_bls_batch* b, void* stream, uint8_t* ok, 
         LHB_CUDA(cudaStreamSynchronize(s));
     }
     *ok = b->h_res[0];
-    if (set_status) memcpy(set_status, b->h_res + 64, b->n);
+    // the two stages' codes for each set, the signature's first (the oracle checks the signature before the keys)
+    if (set_status)
+        for (uint32_t i = 0; i < b->n; i++) set_status[i] = h_sig[i] ? h_sig[i] : h_pk[i];
     return LHB200_OK;
 }
 
@@ -1009,6 +1059,13 @@ int32_t lhb200_bls_batch_gt(lhb200_bls_batch* b, uint8_t out576[576]) {
 }
 
 uint64_t lhb200_bls_batch_launches(const lhb200_bls_batch* b) { return b ? b->launches_last : 0; }
+
+// Test hook: the kernel choices of the last verify_enqueue (word layout in lhb200.h).
+int32_t lhb200_bls_batch_plan(const lhb200_bls_batch* b, uint32_t* out, uint32_t n_words) {
+    if (!b || (n_words && !out)) return LHB200_EINVAL;
+    memcpy(out, b->plan, sizeof(uint32_t) * std::min<uint32_t>(n_words, LHB200_PLAN_WORDS));
+    return LHB200_OK;
+}
 
 // Device time (ms, CUDA events on the launching stream) of the dominant kernel k_miller_multi in the last completed
 // enqueue; negative if unavailable.  Call after the stream has been synchronised.

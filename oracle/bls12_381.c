@@ -455,7 +455,15 @@ static void g2_clear_cofactor(g2j *r, const g2j *p) { /* RFC 9380 App. G.3 */
 
 /* serialisation (ZCash format) */
 static int g1_from_uncompressed(g1a *r, const uint8_t *b) { /* 0 ok, 1 inf, 2 bad */
-    if (b[0] & 0x40) { memset(r, 0, sizeof *r); r->inf = 1; return 1; }
+    /* the 96-byte form: compression and sort flags clear, an infinity encoding all zero otherwise (blst's P1
+     * deserialize; the library's keys are decoded by the same rules) */
+    if (b[0] & 0xa0) return 2;
+    if (b[0] & 0x40) {
+        uint8_t nz = b[0] & 0x3f;
+        for (int i = 1; i < 96; i++) nz |= b[i];
+        if (nz) return 2;
+        memset(r, 0, sizeof *r); r->inf = 1; return 1;
+    }
     fp cx, cy;
     fp_from_be48(&cx, b); fp_from_be48(&cy, b + 48);
     cx.l[5] &= 0x1fffffffffffffffull;

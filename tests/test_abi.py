@@ -95,3 +95,20 @@ def test_blinding_scalars_come_from_a_csprng_stream():
     assert abs(bits.mean() - 0.5) < 0.005
     per_bit = np.unpackbits(a.view(np.uint8).reshape(n, 8), axis=1).mean(axis=0)
     assert (abs(per_bit - 0.5) < 0.02).all()
+
+
+def test_plan_layout_matches_header():
+    """Batch.plan() names the words of lhb200_bls_batch_plan in the order of the LHB200_PLAN_* indices and maps the
+    LHB200_K_* kernel ids to the right names."""
+    from lighthouse_b200 import bls
+    hdr = open(os.path.join(ROOT, "include", "lhb200.h")).read()
+    words = dict(re.findall(r"#define LHB200_PLAN_([A-Z0-9_]+) (\d+)", hdr))
+    n_words = int(words.pop("WORDS"))
+    assert n_words == len(bls.PLAN_FIELDS)
+    assert sorted(int(v) for v in words.values()) == list(range(n_words))
+    for name, v in words.items():
+        assert bls.PLAN_FIELDS[int(v)] == name.lower(), name
+    kernels = dict(re.findall(r"#define LHB200_K_([A-Z0-9_]+) (\d+)", hdr))
+    assert len(kernels) == len(bls.PLAN_KERNELS) - 1
+    for name, v in kernels.items():
+        assert bls.PLAN_KERNELS[int(v)].replace("+k_pk_", "_").upper() == "K_" + name, name
