@@ -185,7 +185,10 @@ LHB200_API int32_t lhb200_shuffle_list(const uint64_t* input, uint64_t n, uint8_
  *   sigs        n x 96 B  compressed G2 (ZCash format; all-zero = Lighthouse's "empty" signature -> false)
  *   msgs        n x 32 B  signing roots
  *   pks         K x 96 B  uncompressed affine G1, x || y big-endian (the validator_pubkey_cache.rs:195-199 format;
- *                         keys are NOT re-validated, matching pks_validate=false at blst.rs:115)
+ *                         keys are NOT re-validated, matching pks_validate=false at blst.rs:115).  Keys must be in
+ *                         G1: sets that share a message are paired once, through the sum of their r_i apk_i, and
+ *                         prod_i e(r_i apk_i, H(m)) = e(sum_i r_i apk_i, H(m)) rests on bilinearity, which holds for
+ *                         G1 points.  Lighthouse's keys are (validated at import, validator_pubkey_cache.rs:116-118).
  *   pk_offsets  n+1 u32   CSR: set i owns keys [pk_offsets[i], pk_offsets[i+1])
  *   rands       n x u64   nonzero random scalars (blst.rs:55-67), or NULL to have the library draw them
  * *ok = 1 iff  prod_i e(r_i apk_i, H(m_i)) == e(g1, sum_i r_i sig_i)  and every set passed its checks
@@ -194,13 +197,21 @@ LHB200_API int32_t lhb200_shuffle_list(const uint64_t* input, uint64_t n, uint8_
  * 4 no keys, 5 aggregate key at infinity, 6 key decode.  A set that fails several checks reports one code, in the
  * order blst.rs:73-106 checks them: a signature failure (1, 2, 3) first, then no keys (4), then key decode (6), then
  * the aggregate key at infinity (5).  fast_aggregate_verify / Signature::verify (blst.rs:196-200, :250-261) are the
- * n_sets == 1 case. */
+ * n_sets == 1 case.
+ * Sets that share a message (every unaggregated attestation of a committee, every sync-committee message of a slot)
+ * are grouped: when at least one set in eight repeats a message, hash-to-G2 and the Miller loop run once per distinct
+ * message over the sum of the group's r_i apk_i.  The verdict, the statuses and the final-exponentiated product are the same as without. */
 LHB200_API int32_t lhb200_verify_signature_sets(const uint8_t* sigs, const uint8_t* msgs, const uint8_t* pks,
                                                 const uint32_t* pk_offsets, const uint64_t* rands, uint32_t n_sets,
                                                 uint8_t* ok, uint8_t* set_status);
 
 /* Staged form of the same call (what bench.py times): create once, upload or point at device-resident inputs,
- * enqueue on a stream, read the verdict. */
+ * enqueue on a stream, read the verdict.  The three host uploads (lhb200_bls_batch_upload, _upload_async,
+ * _upload_indexed) group the sets by message on the host when at least one set in eight repeats a message, and
+ * verify_enqueue then runs
+ * hash-to-G2, the Miller loop and the product tree over the distinct messages (kernels and launch shapes chosen for
+ * that count) after one per-message sum of the key stage's points.  Other batches, and inputs bound with
+ * lhb200_bls_batch_set_device_inputs, run per set.  LHB_GROUP_MESSAGES=0 turns the grouping off. */
 typedef struct lhb200_bls_batch lhb200_bls_batch;
 LHB200_API int32_t lhb200_bls_batch_create(uint32_t max_sets, uint64_t max_keys, lhb200_bls_batch** out);
 LHB200_API int32_t lhb200_bls_batch_destroy(lhb200_bls_batch* b);
@@ -239,7 +250,7 @@ LHB200_API int32_t lhb200_bls_batch_gt(lhb200_bls_batch* b, uint8_t out576[576])
 /* Test hook: which kernels the last lhb200_bls_batch_verify_enqueue on `b` launched, so a test can tell which path a
  * batch size exercised.  Writes min(n_words, LHB200_PLAN_WORDS) words, indexed by LHB200_PLAN_*; the stage words
  * hold LHB200_K_* ids, 0 where the stage did not run (the sum tree of a single set). */
-#define LHB200_PLAN_WORDS 20
+#define LHB200_PLAN_WORDS 23
 #define LHB200_PLAN_N_SETS 0
 #define LHB200_PLAN_N_SM 1                    /* SM count the launch shapes were derived from */
 #define LHB200_PLAN_SIG 2
@@ -260,6 +271,9 @@ LHB200_API int32_t lhb200_bls_batch_gt(lhb200_bls_batch* b, uint8_t out576[576])
 #define LHB200_PLAN_LANE_GRID 17              /* blocks of the one-thread-per-set kernels */
 #define LHB200_PLAN_LANE_SETS_PER_THREAD 18   /* > 1 once the CTA cap makes them grid-stride */
 #define LHB200_PLAN_LAST_MILLER 19            /* 1 if k_last_miller ran (the pair -g1, sum r sig on its own) */
+#define LHB200_PLAN_GROUPS 20                 /* distinct messages the sets were grouped into; 0 = not grouped */
+#define LHB200_PLAN_GROUP_SUM 21              /* the per-message key sum (grouped batches only) */
+#define LHB200_PLAN_GROUP_SUM_LEVELS 22       /* levels of its segmented tree */
 #define LHB200_K_SIG_PREPARE 1
 #define LHB200_K_SIG_PREPARE_WARP 2
 #define LHB200_K_G2_REDUCE 3
@@ -276,6 +290,7 @@ LHB200_API int32_t lhb200_bls_batch_gt(lhb200_bls_batch* b, uint8_t out576[576])
 #define LHB200_K_MILLER_WARP 14
 #define LHB200_K_FINAL_COOP 15
 #define LHB200_K_FINAL_WARP 16
+#define LHB200_K_G1_GROUP_SUM 17
 LHB200_API int32_t lhb200_bls_batch_plan(const lhb200_bls_batch* b, uint32_t* out, uint32_t n_words);
 LHB200_API uint64_t lhb200_bls_batch_launches(const lhb200_bls_batch* b);
 /* Device time (ms) of the dominant kernel (k_miller) in the last completed enqueue, from CUDA events recorded on
@@ -330,6 +345,11 @@ LHB200_API int32_t lhb200_aggregate_verify(const uint8_t sig96[96], const uint8_
 /* Test hook (no device needed): n blinding scalars from the generator lhb200_verify_signature_sets uses when
  * `rands == NULL` — a ChaCha20 keystream keyed from getrandom(2), zeros skipped (blst.rs:46-68: rand::thread_rng). */
 LHB200_API int32_t lhb200_debug_rand_scalars(uint64_t* out, uint32_t n);
+/* Test hook (no device needed): the grouping of n 32-byte messages the batch uploads apply.  members (n) lists the
+ * sets group by group, groups in order of first occurrence and members ascending; group g owns
+ * members[group_offsets[g] .. group_offsets[g + 1]) (group_offsets: n + 1 words, *n_groups + 1 written). */
+LHB200_API int32_t lhb200_debug_group_messages(const uint8_t* msgs, uint32_t n, uint32_t* members,
+                                               uint32_t* group_offsets, uint32_t* n_groups);
 
 /* Test hook: run one stage of the BLS pipeline on a single device thread so `pytest -m gpu` can compare every
  * stage with the oracle.  op: 0 expand_message_xmd(32->256), 1 hash_to_g2(32->96), 2 SSWU(u 96 -> x|y 192),

@@ -122,6 +122,7 @@ _sig("lhb200_state_patch_batch", C.c_int32, vp, vp, vp, vp, C.c_uint32)
 _sig("lhb200_blinded_beacon_block_roots_deneb", C.c_int32, vp, vp, C.c_uint32, vp, vp)
 _sig("lhb200_beacon_block_roots", C.c_int32, vp, vp, C.c_uint32, C.c_int32, C.c_int32, vp, vp)
 _sig("lhb200_debug_rand_scalars", C.c_int32, vp, C.c_uint32)
+_sig("lhb200_debug_group_messages", C.c_int32, vp, C.c_uint32, vp, vp, C.POINTER(C.c_uint32))
 _sig("lhb200_g2_aggregate", C.c_int32, vp, C.c_uint32, vp)
 _sig("lhb200_g1_aggregate", C.c_int32, vp, C.c_uint32, vp, vp)
 _sig("lhb200_g1_deserialize_uncompressed", C.c_int32, vp, C.c_uint32, vp, vp)

@@ -404,12 +404,13 @@ class PubkeyTable:
 # word layout of lhb200_bls_batch_plan (LHB200_PLAN_* in include/lhb200.h) and its kernel ids (LHB200_K_*)
 PLAN_FIELDS = ("n_sets", "n_sm", "sig", "sum", "sum_levels", "hash", "key", "key_chunks", "miller", "miller_wpb",
                "miller_spw", "miller_grid", "miller_rounds_cap", "miller_few_warps", "fp12_reduce_levels", "n_tail",
-               "final", "lane_grid", "lane_sets_per_thread", "last_miller")
-_PLAN_KERNEL_FIELDS = ("sig", "sum", "hash", "key", "miller", "final")
+               "final", "lane_grid", "lane_sets_per_thread", "last_miller", "groups", "group_sum",
+               "group_sum_levels")
+_PLAN_KERNEL_FIELDS = ("sig", "sum", "hash", "key", "miller", "final", "group_sum")
 PLAN_KERNELS = ("", "k_sig_prepare", "k_sig_prepare_warp", "k_g2_reduce", "k_g2_sum_warp", "k_hash_to_g2",
                 "k_hash_to_g2_pair", "k_hash_to_g2_warp", "k_pk_aggregate", "k_pk_partial+k_pk_combine",
                 "k_pk_aggregate_tma", "k_pk_aggregate_indexed", "k_miller_multi", "k_miller_coop", "k_miller_warp",
-                "k_final_coop", "k_final_warp")
+                "k_final_coop", "k_final_warp", "k_g1_group_sum")
 
 
 class Batch:
@@ -495,6 +496,19 @@ class Batch:
             self.destroy()
         except Exception:
             pass
+
+
+def group_messages(msgs: bytes):
+    """lhb200_debug_group_messages test hook (no device): n 32-byte messages -> (members uint32[n],
+    group_offsets uint32[n_groups + 1]); groups in order of first occurrence, members ascending."""
+    n = len(msgs) // 32
+    members = np.zeros(max(n, 1), dtype=np.uint32)
+    offsets = np.zeros(n + 1, dtype=np.uint32)
+    ng = C.c_uint32(0)
+    p, k = buf(msgs if n else b"\0")
+    check(lib.lhb200_debug_group_messages(p, n, members.ctypes.data, offsets.ctypes.data, C.byref(ng)),
+          "lhb200_debug_group_messages")
+    return members[:n], offsets[:ng.value + 1]
 
 
 def debug_stage(op, data: bytes, out_len: int):

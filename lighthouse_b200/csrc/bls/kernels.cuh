@@ -7,6 +7,7 @@
 //   k_sig_prepare ...... K10 g2_decompress + K4 subgroup check + K7 r*sig        (blst.rs:73-83, :114)
 //   k_pk_aggregate ..... K5 segmented G1 sum over CSR offsets + K7 r*apk          (blst.rs:86-106, :114)
 //   k_hash_to_g2 ....... K6 hash_to_curve                                         (blst.rs:114, DST :15)
+//   k_g1_group_sum ..... per-message sums of r*apk when sets share messages (group_sum.cuh)
 //   k_miller_multi ..... K8 Miller loops, k sets per thread sharing the Fp12 squarings
 //   k_fp12_reduce / k_g2_reduce ... product / sum trees
 //   k_final ............ K8 Miller loop for (-g1, sum r*sig) + K9 final exponentiation and == 1
@@ -14,6 +15,7 @@
 #include "pairing.cuh"
 #include "miller_coop.cuh"
 #include "miller_warp.cuh"
+#include "group_sum.cuh"
 #include "h2c.cuh"
 
 namespace lhb200 {

@@ -31,6 +31,98 @@ void bls_shutdown();
 
 using namespace lhb200;
 
+// Groups sets by their 32-byte message: an open-addressing hash table over the messages (O(n) expected).  A fingerprint
+// of all 32 bytes picks the bucket, and its high half is kept in the slot so that only a matching fingerprint costs a
+// look at the stored message; two messages are equal when all 32 bytes match.  Groups come in order of first
+// occurrence, the members of a group in ascending order.  Scratch is sized once (reserve).
+struct MsgGrouper {
+    std::vector<uint64_t> slot;   // (fingerprint >> 32) << 32 | (group + 1); 0 = empty
+    std::vector<uint64_t> seen;   // pre-pass bitset over the fingerprints
+    std::vector<uint32_t> gid, first, cnt, members, offsets;
+    std::vector<uint8_t> msgs;   // one copy of each distinct message
+
+    static uint32_t table_size(uint32_t n) {
+        uint32_t t = 16;
+        while (t < 2 * (uint64_t)n) t <<= 1;
+        return t;
+    }
+    static uint64_t seen_bits(uint32_t n) { return (uint64_t)table_size(n) * 8; }   // >= 16 bits per message
+    void reserve(uint32_t cap) {
+        slot.resize(table_size(cap));
+        seen.resize(seen_bits(cap) / 64);
+        gid.resize(cap); first.resize(cap); cnt.resize(cap); members.resize(cap); offsets.resize(cap + 1);
+        msgs.resize((size_t)cap * 32);
+    }
+    static uint64_t fingerprint(const uint8_t* m) {
+        uint64_t w[4], h = 0x243F6A8885A308D3ull;
+        memcpy(w, m, 32);
+        for (int k = 0; k < 4; k++) {
+            h = (h ^ w[k]) * 0x9E3779B97F4A7C15ull;
+            h ^= h >> 32;
+        }
+        return h;
+    }
+    // Cheaper mix for the pre-pass below (one multiply); equal messages still get equal values.
+    static uint64_t quick_fingerprint(const uint8_t* m) {
+        uint64_t w[4];
+        memcpy(w, m, 32);
+        const uint64_t x = w[0] ^ ((w[1] << 17) | (w[1] >> 47)) ^ ((w[2] << 31) | (w[2] >> 33)) ^ ((w[3] << 47) | (w[3] >> 17));
+        return x * 0x9E3779B97F4A7C15ull;
+    }
+    // -> number of distinct messages.  The CSR (members, offsets[0 .. n_groups]) and `msgs` are filled, and max_group set
+    // to the size of the largest group, when at least `min_repeats` sets repeat a message (min_repeats 0: always).
+    uint32_t run(const uint8_t* m, uint32_t n, uint32_t min_repeats, uint32_t* max_group) {
+        *max_group = 0;
+        if (min_repeats > 0) {
+            // Pre-pass: a repeated message always finds its fingerprint bit set, so fewer bits found set than
+            // min_repeats rules grouping out without the table (the common all-distinct batch; at >= 16 bits per
+            // message the expected number of chance hits is about n / 32).
+            const uint64_t bits = seen_bits(n), bmask = bits - 1;
+            std::fill(seen.begin(), seen.begin() + bits / 64, 0ull);
+            uint32_t hits = 0;
+            for (uint32_t i = 0; i < n; i++) {
+                const uint64_t b = (quick_fingerprint(m + (size_t)32 * i) >> 32) & bmask, bit = 1ull << (b & 63);
+                hits += (seen[b >> 6] & bit) != 0;
+                seen[b >> 6] |= bit;
+            }
+            if (hits < min_repeats) return n;
+        }
+        const uint32_t ts = table_size(n), mask = ts - 1;
+        std::fill(slot.begin(), slot.begin() + ts, 0ull);
+        uint32_t ng = 0;
+        for (uint32_t i = 0; i < n; i++) {
+            const uint8_t* mi = m + (size_t)32 * i;
+            const uint64_t fp = fingerprint(mi), tag = fp & 0xFFFFFFFF00000000ull;
+            for (uint32_t h = (uint32_t)fp & mask;; h = (h + 1) & mask) {
+                const uint64_t s = slot[h];
+                if (s == 0) {   // new message: group ng
+                    slot[h] = tag | (ng + 1);
+                    first[ng] = i;
+                    cnt[ng] = 0;
+                    gid[i] = ng++;
+                    break;
+                }
+                const uint32_t g = (uint32_t)s - 1;
+                if ((s & 0xFFFFFFFF00000000ull) == tag && memcmp(m + (size_t)32 * first[g], mi, 32) == 0) {
+                    gid[i] = g;
+                    break;
+                }
+            }
+            cnt[gid[i]]++;
+        }
+        if (n - ng < min_repeats) return ng;
+        offsets[0] = 0;
+        for (uint32_t g = 0; g < ng; g++) {
+            offsets[g + 1] = offsets[g] + cnt[g];
+            *max_group = std::max(*max_group, cnt[g]);
+            memcpy(&msgs[(size_t)32 * g], m + (size_t)32 * first[g], 32);
+            cnt[g] = offsets[g];   // from here: the next free member slot of group g
+        }
+        for (uint32_t i = 0; i < n; i++) members[cnt[gid[i]]++] = i;
+        return ng;
+    }
+};
+
 struct lhb200_pubkey_table {
     G1Mont* d_keys = nullptr;
     uint64_t capacity = 0, len = 0;
@@ -94,6 +186,16 @@ struct lhb200_bls_batch {
     int n_chunks = 0;                        // 0: inputs already complete on the device
     std::vector<uint64_t> rbuf;              // scalars drawn by the library (must outlive the async copy)
     uint32_t plan[LHB200_PLAN_WORDS] = {};   // kernels the last verify_enqueue chose (lhb200_bls_batch_plan)
+    // sets grouped by message (host uploads where a message repeats): hash-to-G2 and Miller run per group
+    uint32_t n_groups = 0;                   // 0: not grouped
+    uint32_t max_group = 0;                  // members of the largest group (depth of the group-sum tree)
+    MsgGrouper grouper;                      // host scratch + the CSR the device copies read
+    uint32_t* d_members = nullptr;           // n set indices, grouped
+    uint32_t* d_goffsets = nullptr;          // n_groups + 1
+    uint8_t* d_gmsgs = nullptr;              // n_groups x 32 B, the distinct messages
+    G1Proj3* d_gp = nullptr;                 // per-group sum of r_i apk_i
+    uint8_t* d_gskip = nullptr;              // per group: nothing to pair (no contributing member, or the sum is O)
+    G1Jac* d_gtmp = nullptr;                 // partial sums of the group-sum tree
 };
 
 static void batch_free(lhb200_bls_batch* b) {
@@ -102,7 +204,7 @@ static void batch_free(lhb200_bls_batch* b) {
     void* ptrs[] = {b->d_sigs, b->d_msgs, b->d_pks, b->d_offsets, b->d_rands, b->d_sigr, b->d_sig_tmp[0],
                     b->d_sig_tmp[1], b->d_p, b->d_h, b->d_f, b->d_f_tmp[0], b->d_f_tmp[1], b->d_flast, b->d_gt,
                     b->d_status, b->d_pk_status, b->d_fail, b->d_ok, b->d_mc_scratch, b->d_neg_g1, b->d_pk_part,
-                    b->d_pk_part_bad};
+                    b->d_pk_part_bad, b->d_members, b->d_goffsets, b->d_gmsgs, b->d_gp, b->d_gskip, b->d_gtmp};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     if (b->h_res) cudaFreeHost(b->h_res);
@@ -318,7 +420,14 @@ int32_t lhb200_bls_batch_create(uint32_t max_sets, uint64_t max_keys, lhb200_bls
     ALLOC(b->d_neg_g1, sizeof(G1Proj3));
     ALLOC(b->d_pk_part, std::min<uint64_t>(n, PK_SPLIT_MAX_SETS) * PK_SLICES * sizeof(G1Jac));
     ALLOC(b->d_pk_part_bad, std::min<uint64_t>(n, PK_SPLIT_MAX_SETS) * PK_SLICES);
+    ALLOC(b->d_members, n * 4);
+    ALLOC(b->d_goffsets, (n + 1) * 4);
+    ALLOC(b->d_gmsgs, n * 32 + 16);
+    ALLOC(b->d_gp, n * sizeof(G1Proj3));
+    ALLOC(b->d_gskip, n);
+    ALLOC(b->d_gtmp, n * sizeof(G1Jac));
 #undef ALLOC
+    b->grouper.reserve(max_sets);
     cudaError_t e = cudaHostAlloc(reinterpret_cast<void**>(&b->h_res), 2 * n + 64 + sizeof(Fp12), cudaHostAllocDefault);
     if (e != cudaSuccess) { batch_free(b); return cuda_fail(e, "cudaHostAlloc(result)"); }
     if ((e = cudaStreamCreateWithFlags(&b->s_main, cudaStreamNonBlocking)) != cudaSuccess ||
@@ -424,6 +533,42 @@ extern "C" LHB200_API int32_t lhb200_debug_rand_scalars(uint64_t* out, uint32_t 
     return gen_rands(out, n) ? LHB200_OK : LHB200_ECUDA;
 }
 
+// Test hook: the grouping lhb200_bls_batch_upload* applies to the messages (no device needed).
+extern "C" LHB200_API int32_t lhb200_debug_group_messages(const uint8_t* msgs, uint32_t n, uint32_t* members,
+                                                          uint32_t* group_offsets, uint32_t* n_groups) {
+    if (!msgs || !members || !group_offsets || !n_groups) return LHB200_EINVAL;
+    MsgGrouper g;
+    g.reserve(n);
+    uint32_t max_group = 0;
+    const uint32_t ng = g.run(msgs, n, 0, &max_group);
+    memcpy(members, g.members.data(), (size_t)n * 4);
+    memcpy(group_offsets, g.offsets.data(), (size_t)(ng + 1) * 4);
+    *n_groups = ng;
+    return LHB200_OK;
+}
+
+// Grouping is used once at least 1/GROUP_MIN_REPEAT_DIV of the sets repeat a message.  Measured on one H100 80GB HBM3
+// at 700 W (DESIGN §2.6): 100 000 x 128-key sets with one repeated message lost ~4.5 ms per plugin call to grouping
+// (host CSR, copies, group-sum tree), while 97 952 repeats saved ~49 ms of hash-to-G2 and Miller work (~0.5 us each).
+constexpr uint32_t GROUP_MIN_REPEAT_DIV = 8;
+
+// Host uploads: group the sets by message and queue the CSR and the distinct messages on `s`.  n_groups stays 0 (the
+// ungrouped path) when too few messages repeat, or with LHB_GROUP_MESSAGES=0.
+static int32_t upload_groups(lhb200_bls_batch* b, const uint8_t* msgs, uint32_t n, cudaStream_t s) {
+    static const int group_env = [] { const char* e = getenv("LHB_GROUP_MESSAGES"); return e ? atoi(e) : 1; }();
+    b->n_groups = 0;
+    if (!group_env || n < 2) return LHB200_OK;
+    MsgGrouper& g = b->grouper;
+    const uint32_t min_repeats = std::max<uint32_t>(1, n / GROUP_MIN_REPEAT_DIV);
+    const uint32_t ng = g.run(msgs, n, min_repeats, &b->max_group);
+    if (n - ng < min_repeats) return LHB200_OK;
+    LHB_CUDA(cudaMemcpyAsync(b->d_members, g.members.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    LHB_CUDA(cudaMemcpyAsync(b->d_goffsets, g.offsets.data(), (size_t)(ng + 1) * 4, cudaMemcpyHostToDevice, s));
+    LHB_CUDA(cudaMemcpyAsync(b->d_gmsgs, g.msgs.data(), (size_t)ng * 32, cudaMemcpyHostToDevice, s));
+    b->n_groups = ng;
+    return LHB200_OK;
+}
+
 // Copy host inputs into the batch's device buffers.  rands == NULL: drawn here.
 int32_t lhb200_bls_batch_upload(lhb200_bls_batch* b, const uint8_t* sigs, const uint8_t* msgs, const uint8_t* pks,
                                 const uint32_t* pk_offsets, const uint64_t* rands, uint32_t n_sets) {
@@ -453,6 +598,7 @@ int32_t lhb200_bls_batch_upload(lhb200_bls_batch* b, const uint8_t* sigs, const 
     if (n_keys) LHB_CUDA(cudaMemcpyAsync(b->d_pks, pks, (size_t)n_keys * 96, cudaMemcpyHostToDevice, s));
     LHB_CUDA(cudaMemcpyAsync(b->d_offsets, pk_offsets, (size_t)(n_sets + 1) * 4, cudaMemcpyHostToDevice, s));
     LHB_CUDA(cudaMemcpyAsync(b->d_rands, rands, (size_t)n_sets * 8, cudaMemcpyHostToDevice, s));
+    if (int32_t rc = upload_groups(b, msgs, n_sets, s)) return rc;
     LHB_CUDA(cudaStreamSynchronize(s));  // rbuf / caller buffers may go away
     b->n = n_sets;
     b->n_chunks = 0;
@@ -494,6 +640,7 @@ int32_t lhb200_bls_batch_upload_async(lhb200_bls_batch* b, const uint8_t* sigs, 
     LHB_CUDA(cudaMemcpyAsync(b->d_msgs, msgs, (size_t)n_sets * 32, cudaMemcpyHostToDevice, s));
     LHB_CUDA(cudaMemcpyAsync(b->d_offsets, pk_offsets, (size_t)(n_sets + 1) * 4, cudaMemcpyHostToDevice, s));
     LHB_CUDA(cudaMemcpyAsync(b->d_rands, rands, (size_t)n_sets * 8, cudaMemcpyHostToDevice, s));
+    if (int32_t rc = upload_groups(b, msgs, n_sets, s)) return rc;
     LHB_CUDA(cudaEventRecord(b->e_small, s));
     // chunks of whole sets, ~equal key counts
     int nc = (int)std::min<uint64_t>(lhb200_bls_batch::MAX_CHUNKS, std::max<uint64_t>(1, n_keys * 96 / (32u << 20)));
@@ -601,6 +748,7 @@ int32_t lhb200_bls_batch_upload_indexed(lhb200_bls_batch* b, const lhb200_pubkey
     if (n_keys) LHB_CUDA(cudaMemcpyAsync(b->d_indices, key_indices, (size_t)n_keys * 4, cudaMemcpyHostToDevice, s));
     LHB_CUDA(cudaMemcpyAsync(b->d_offsets, pk_offsets, (size_t)(n_sets + 1) * 4, cudaMemcpyHostToDevice, s));
     LHB_CUDA(cudaMemcpyAsync(b->d_rands, rands, (size_t)n_sets * 8, cudaMemcpyHostToDevice, s));
+    if (int32_t rc = upload_groups(b, msgs, n_sets, s)) return rc;
     LHB_CUDA(cudaStreamSynchronize(s));
     b->n = n_sets;
     b->in_sigs = b->d_sigs; b->in_msgs = b->d_msgs; b->in_pks = nullptr;
@@ -627,6 +775,7 @@ int32_t lhb200_bls_batch_set_device_inputs(lhb200_bls_batch* b, const void* d_si
     b->in_offsets = static_cast<const uint32_t*>(d_offsets);
     b->in_rands = static_cast<const uint64_t*>(d_rands);
     b->n_chunks = 0;
+    b->n_groups = 0;   // device-resident messages are not grouped
     b->table = nullptr;
     return LHB200_OK;
 }
@@ -640,17 +789,26 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
     // LHB_BLS_CTAS_PER_SM overrides (tuning knob; 0 = one CTA per BLS_BLOCK sets, i.e. no cap).
     static const int ctas_per_sm = [] { const char* e = getenv("LHB_BLS_CTAS_PER_SM"); return e ? atoi(e) : 12; }();
     static const int n_sm = [] { int v = 132; cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, ctx().device); return v; }();
-    uint32_t grid = cdiv(n, BLS_BLOCK);
-    if (ctas_per_sm > 0 && grid > (uint32_t)(n_sm * ctas_per_sm)) {
-        const uint32_t max_thr = (uint32_t)(n_sm * ctas_per_sm) * BLS_BLOCK;
-        const uint32_t per_thread = cdiv(n, max_thr);            // sets per thread, balanced across the grid
-        grid = cdiv(n, (uint64_t)per_thread * BLS_BLOCK);
-    }
+    auto lane_grid = [&](uint32_t m) {
+        uint32_t g = cdiv(m, BLS_BLOCK);
+        if (ctas_per_sm > 0 && g > (uint32_t)(n_sm * ctas_per_sm)) {
+            const uint32_t max_thr = (uint32_t)(n_sm * ctas_per_sm) * BLS_BLOCK;
+            const uint32_t per_thread = cdiv(m, max_thr);        // sets per thread, balanced across the grid
+            g = cdiv(m, (uint64_t)per_thread * BLS_BLOCK);
+        }
+        return g;
+    };
+    const uint32_t grid = lane_grid(n);
+    // Grouped by message (host uploads with a repeated message): the signature and key stages run over the n sets, the
+    // hash, Miller and final stages over the ng distinct messages, each with the kernels and shapes chosen for its count.
+    const bool grouped = b->n_groups != 0;
+    const uint32_t ng = grouped ? b->n_groups : n;
     uint64_t launches = 0;
     uint32_t* plan = b->plan;
     memset(plan, 0, sizeof b->plan);
     plan[LHB200_PLAN_N_SETS] = n;
     plan[LHB200_PLAN_N_SM] = (uint32_t)n_sm;
+    plan[LHB200_PLAN_GROUPS] = b->n_groups;
     plan[LHB200_PLAN_LANE_GRID] = grid;
     plan[LHB200_PLAN_LANE_SETS_PER_THREAD] = cdiv(n, (uint64_t)grid * BLS_BLOCK);
     // key ingest through the TMA unit (bulk async copies into a shared-memory ring); needs 16-byte aligned keys.
@@ -675,9 +833,10 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
     // enough for the warps of one wave (four per block, at most two blocks per SM)
     static const int g2_warp_env = [] { const char* e = getenv("LHB_G2_WARP"); return e ? atoi(e) : 1; }();
     const bool g2_warp = g2_warp_env && n <= 6u * (uint32_t)n_sm;   // measured crossover with the lane-per-set kernels: ~1 000 sets
+    const bool hash_warp = g2_warp_env && ng <= 6u * (uint32_t)n_sm;
     constexpr uint32_t GW_WPB = 4;
     const size_t gw_smem = gw::smem_bytes(GW_WPB);
-    if (g2_warp) {   // working sets + a shared-memory copy of the phase tables: above the 48 KB default
+    if (g2_warp || hash_warp) {   // working sets + a shared-memory copy of the phase tables: above the 48 KB default
         static const bool gw_attr_ok = [&] {
             return cudaFuncSetAttribute(gw::k_sig_prepare_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gw_smem) == cudaSuccess &&
                    cudaFuncSetAttribute(gw::k_hash_to_g2_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gw_smem) == cudaSuccess &&
@@ -728,14 +887,16 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
         }
         LHB_CUDA(cudaEventRecord(b->e_join, b->s2));
     }
-    plan[LHB200_PLAN_HASH] = g2_warp ? LHB200_K_HASH_TO_G2_WARP
-                             : n <= HASH_PAIR_MAX_SETS ? LHB200_K_HASH_TO_G2_PAIR : LHB200_K_HASH_TO_G2;
-    if (g2_warp)
-        gw::k_hash_to_g2_warp<<<cdiv(n, GW_WPB), 32 * GW_WPB, gw_smem, b->s3>>>(b->in_msgs, n, b->d_h);
-    else if (n <= HASH_PAIR_MAX_SETS)   // latency mode: two threads per message (one SSWU map each)
-        k_hash_to_g2_pair<<<cdiv(2 * n, BLS_BLOCK), BLS_BLOCK, 0, b->s3>>>(b->in_msgs, n, b->d_h);
+    // grouped: one hash per distinct message, d_h[g] = H(message of group g)
+    const uint8_t* h_msgs = grouped ? b->d_gmsgs : b->in_msgs;
+    plan[LHB200_PLAN_HASH] = hash_warp ? LHB200_K_HASH_TO_G2_WARP
+                             : ng <= HASH_PAIR_MAX_SETS ? LHB200_K_HASH_TO_G2_PAIR : LHB200_K_HASH_TO_G2;
+    if (hash_warp)
+        gw::k_hash_to_g2_warp<<<cdiv(ng, GW_WPB), 32 * GW_WPB, gw_smem, b->s3>>>(h_msgs, ng, b->d_h);
+    else if (ng <= HASH_PAIR_MAX_SETS)   // latency mode: two threads per message (one SSWU map each)
+        k_hash_to_g2_pair<<<cdiv(2 * ng, BLS_BLOCK), BLS_BLOCK, 0, b->s3>>>(h_msgs, ng, b->d_h);
     else
-        k_hash_to_g2<<<grid, BLS_BLOCK, 0, b->s3>>>(b->in_msgs, n, b->d_h);
+        k_hash_to_g2<<<lane_grid(ng), BLS_BLOCK, 0, b->s3>>>(h_msgs, ng, b->d_h);
     launches++;
     LHB_CUDA(cudaEventRecord(b->e_h2c, b->s3));
     // explicit keys, sets [lo, lo + cnt): TMA ring for GPU-filling batches, slice-parallel sums for small and medium
@@ -801,12 +962,34 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
         launch_pk(0, n, s);
     LHB_CUDA(cudaStreamWaitEvent(s, b->e_h2c, 0));
     LHB_CUDA(cudaStreamWaitEvent(s, b->e_sig, 0));    // the Miller kernel reads the status bytes k_sig_prepare may set
+    // The Miller kernels pair (m_p[i], d_h[i]), i < ng, and skip i unless m_st[i] | m_pk_st[i] == 0: per set, or per
+    // group (the group sums, with the skip flag in both status slots).
+    const G1Proj3* m_p = b->d_p;
+    const uint8_t *m_st = b->d_status, *m_pk_st = b->d_pk_status;
+    if (grouped) {
+        GroupSumArgs ga;
+        ga.P = b->d_p; ga.status = b->d_status; ga.pk_status = b->d_pk_status;
+        ga.members = b->d_members; ga.offsets = b->d_goffsets; ga.n = n; ga.n_groups = ng;
+        ga.tmp = b->d_gtmp; ga.out_p = b->d_gp; ga.skip = b->d_gskip;
+        uint64_t span = 1;
+        uint32_t level = 0;
+        do {   // until one run of GROUP_CHUNK^(level + 1) covers the largest group
+            k_g1_group_sum<<<cdiv(n, BLS_BLOCK), BLS_BLOCK, 0, s>>>(ga, level, span);
+            launches++;
+            level++;
+            span *= GROUP_CHUNK;
+        } while (span < b->max_group);
+        plan[LHB200_PLAN_GROUP_SUM] = LHB200_K_G1_GROUP_SUM;
+        plan[LHB200_PLAN_GROUP_SUM_LEVELS] = level;
+        m_p = b->d_gp;
+        m_st = m_pk_st = b->d_gskip;
+    }
     static const int miller_coop = [] { const char* e = getenv("LHB_MILLER_COOP"); return e ? atoi(e) : 1; }();
     const Fp12* cur = b->d_f;
     uint32_t n_tail = 0;
     const Fp12* f_last = b->d_flast;
     if (miller_coop) {
-        // Cooperative shared-memory Miller loop over the n sets AND the (-g1, sum r sig) pair (bls/miller_coop.cuh):
+        // Cooperative shared-memory Miller loop over the ng pairs AND the (-g1, sum r sig) pair (bls/miller_coop.cuh):
         // one block of 8 independent warps per SM, 30 working lanes per warp, every lane runs `rounds` sets, six lanes
         // share one accumulator.  Small batches spread over more, emptier warps (latency), large ones fill 8 x n_sm.
         static const bool attr_ok = [] {
@@ -815,7 +998,7 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
         }();
         if (!attr_ok) { set_error("k_miller_coop: cannot reserve %zu B of shared memory", mc::mc_smem_bytes()); return LHB200_ECUDA; }
         constexpr uint32_t LU = 30;
-        const uint32_t n_total = n + 1;
+        const uint32_t n_total = ng + 1;
         const uint32_t max_warps = (uint32_t)n_sm * mc::MC_WARPS;
         // Latency mode (bls/miller_warp.cuh): while every pair can have a warp of its own in one wave, a whole warp runs
         // one Miller loop at Fp granularity, far shorter than a lane-per-set loop.  Four warps per block
@@ -831,8 +1014,8 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
             const uint32_t mgrid = cdiv(n_total, wpb);
             LHB_CUDA(cudaStreamWaitEvent(s, b->e_join, 0));   // sum r sig (and -g1) ready
             LHB_CUDA(cudaEventRecord(b->e_k0, s));
-            mw::k_miller_warp<<<mgrid, 32 * wpb, mw::smem_bytes((int)wpb), s>>>(b->d_p, b->d_h, b->d_status, b->d_pk_status,
-                                                                                n, b->d_sig_sum, b->d_neg_g1, b->d_f);
+            mw::k_miller_warp<<<mgrid, 32 * wpb, mw::smem_bytes((int)wpb), s>>>(m_p, b->d_h, m_st, m_pk_st,
+                                                                                ng, b->d_sig_sum, b->d_neg_g1, b->d_f);
             plan[LHB200_PLAN_MILLER] = LHB200_K_MILLER_WARP;
             plan[LHB200_PLAN_MILLER_WPB] = wpb;
             plan[LHB200_PLAN_MILLER_SPW] = 1;
@@ -883,8 +1066,8 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
         }
         LHB_CUDA(cudaStreamWaitEvent(s, b->e_join, 0));   // sum r sig (and -g1) ready
         LHB_CUDA(cudaEventRecord(b->e_k0, s));
-        mc::k_miller_coop<<<mgrid, 32 * mc::MC_WARPS, mc::mc_smem_bytes(), s>>>(b->d_p, b->d_h, b->d_status, b->d_pk_status,
-                                                                                n, b->d_sig_sum, b->d_neg_g1, spw,
+        mc::k_miller_coop<<<mgrid, 32 * mc::MC_WARPS, mc::mc_smem_bytes(), s>>>(m_p, b->d_h, m_st, m_pk_st,
+                                                                                ng, b->d_sig_sum, b->d_neg_g1, spw,
                                                                                 b->d_mc_scratch, b->d_f);
         plan[LHB200_PLAN_MILLER] = LHB200_K_MILLER_COOP;
         plan[LHB200_PLAN_MILLER_WPB] = mc::MC_WARPS;
@@ -922,11 +1105,11 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
     }();
     static const int miller_k_env = [] { const char* e = getenv("LHB_MILLER_K"); return e ? atoi(e) : 0; }();
     const uint32_t resident = (uint32_t)(n_sm * miller_occ) * MILLER_BLOCK;
-    uint32_t mk = miller_k_env > 0 ? (uint32_t)miller_k_env : cdiv(n, resident);
+    uint32_t mk = miller_k_env > 0 ? (uint32_t)miller_k_env : cdiv(ng, resident);
     mk = std::min<uint32_t>(std::max<uint32_t>(mk, 1), MILLER_KMAX);
-    const uint32_t n_groups = cdiv(n, mk);
+    const uint32_t n_groups = cdiv(ng, mk);
     const uint32_t mgrid = std::min<uint32_t>(cdiv(n_groups, MILLER_BLOCK), (uint32_t)(n_sm * miller_occ));
-    k_miller_multi<<<mgrid, MILLER_BLOCK, 0, s>>>(b->d_p, b->d_h, b->d_status, b->d_pk_status, n, mk, n_groups, b->d_f);
+    k_miller_multi<<<mgrid, MILLER_BLOCK, 0, s>>>(m_p, b->d_h, m_st, m_pk_st, ng, mk, n_groups, b->d_f);
     plan[LHB200_PLAN_MILLER] = LHB200_K_MILLER_MULTI;
     plan[LHB200_PLAN_MILLER_SPW] = mk;
     plan[LHB200_PLAN_MILLER_GRID] = mgrid;
