@@ -293,8 +293,8 @@ LHB200_API int32_t lhb200_bls_batch_gt(lhb200_bls_batch* b, uint8_t out576[576])
 #define LHB200_K_G1_GROUP_SUM 17
 LHB200_API int32_t lhb200_bls_batch_plan(const lhb200_bls_batch* b, uint32_t* out, uint32_t n_words);
 LHB200_API uint64_t lhb200_bls_batch_launches(const lhb200_bls_batch* b);
-/* Device time (ms) of the dominant kernel (k_miller) in the last completed enqueue, from CUDA events recorded on
- * the launching stream; < 0 if unavailable. */
+/* Device time (ms) of the Miller kernel that ran (k_miller_warp, k_miller_coop or k_miller_multi) in the last completed
+ * enqueue, from CUDA events recorded on the launching stream; < 0 if unavailable. */
 LHB200_API float lhb200_bls_batch_dominant_kernel_ms(const lhb200_bls_batch* b);
 
 /* TSecretKey::public_key / ::sign (crypto/bls/src/impls/blst.rs:282-298): n big-endian 32-byte scalars (< r). */

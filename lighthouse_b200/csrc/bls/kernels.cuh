@@ -9,8 +9,9 @@
 //   k_hash_to_g2 ....... K6 hash_to_curve                                         (blst.rs:114, DST :15)
 //   k_g1_group_sum ..... per-message sums of r*apk when sets share messages (group_sum.cuh)
 //   k_miller_multi ..... K8 Miller loops, k sets per thread sharing the Fp12 squarings
+//   k_last_miller ...... K8 Miller loop for (-g1, sum r*sig) next to k_miller_multi
 //   k_fp12_reduce / k_g2_reduce ... product / sum trees
-//   k_final ............ K8 Miller loop for (-g1, sum r*sig) + K9 final exponentiation and == 1
+//   k_final_coop ....... K9 product of the Miller values, final exponentiation and == 1 (coop.cuh)
 #pragma once
 #include "pairing.cuh"
 #include "miller_coop.cuh"
@@ -503,18 +504,6 @@ __global__ void k_last_miller(const G2Jac* __restrict__ sig_sum, Fp12* __restric
         miller_loop(f, p, q);
     }
     *out_f = f;
-}
-
-// verdict = !fail && final_exp(prod * f_last) == 1 ; also exposes the GT value for tests
-__global__ void k_final(const Fp12* __restrict__ prod, const Fp12* __restrict__ f_last, const uint32_t* __restrict__ fail,
-                        uint8_t* __restrict__ ok, Fp12* __restrict__ gt_out) {
-    if (threadIdx.x != 0 || blockIdx.x != 0) return;
-    if (*fail) { *ok = 0; return; }
-    Fp12 a = *prod, b = *f_last;
-    fp12_mul(a, a, b);
-    final_exp(a, a);
-    if (gt_out) *gt_out = a;
-    *ok = fp12_is_one(a) ? 1 : 0;
 }
 
 // ---------------------------------------------------------------------------------------------------------

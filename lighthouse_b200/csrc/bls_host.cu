@@ -24,7 +24,64 @@ using namespace bls;
 
 static inline uint32_t cdiv(uint64_t a, uint64_t b) { return (uint32_t)((a + b - 1) / b); }
 
-int32_t bls_init() { return LHB200_OK; }
+constexpr uint32_t GW_WPB = 4;   // warps per block of the one-warp-per-point G2 kernels (bls/g2_warp.cuh)
+
+// What the batch driver takes from the device and the environment.  bls_init fills it under the context mutex before
+// ctx().ready is set; it is read-only afterwards, so concurrent callers read it without a lock.
+struct Config {
+    uint32_t n_sm;
+    uint32_t miller_occ;   // resident blocks per SM of k_miller_multi
+    // switches (INTEGRATION.md): latency-mode kernels, cooperative Miller loop, TMA key sums, grouping, key staging
+    bool g2_warp, miller_warp, miller_coop, final_warp, pk_tma, group_messages, stage_pageable;
+};
+static Config g_cfg;
+
+static bool env_switch(const char* name, bool dflt) {
+    const char* e = getenv(name);
+    return e ? atoi(e) != 0 : dflt;
+}
+
+template <class K>
+static bool reserve_smem(K* kernel, size_t bytes) {   // dynamic shared memory above the 48 KB default
+    return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) == cudaSuccess;
+}
+
+int32_t bls_init() {
+    Config c;
+    int v = 0;
+    LHB_CUDA(cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, ctx().device));
+    c.n_sm = (uint32_t)v;
+    LHB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_miller_multi, MILLER_BLOCK, 0));
+    c.miller_occ = (uint32_t)std::max(v, 1);
+    c.g2_warp = env_switch("LHB_G2_WARP", true);
+    c.miller_warp = env_switch("LHB_MILLER_WARP", true);
+    c.miller_coop = env_switch("LHB_MILLER_COOP", true);
+    c.final_warp = env_switch("LHB_FINAL_WARP", true);
+    c.pk_tma = env_switch("LHB_PK_TMA", false);
+    c.group_messages = env_switch("LHB_GROUP_MESSAGES", true);
+    c.stage_pageable = env_switch("LHB_STAGE_PAGEABLE", true);
+    // working sets (+ a shared-memory copy of the phase tables of the warp kernels)
+    const size_t gw_smem = gw::smem_bytes(GW_WPB);
+    if (!reserve_smem(gw::k_sig_prepare_warp, gw_smem) || !reserve_smem(gw::k_hash_to_g2_warp, gw_smem) ||
+        !reserve_smem(gw::k_g2_sum_warp, gw_smem)) {
+        set_error("g2 warp kernels: cannot reserve %zu B of shared memory", gw_smem);
+        return LHB200_ECUDA;
+    }
+    if (!reserve_smem(mc::k_miller_coop, mc::mc_smem_bytes())) {
+        set_error("k_miller_coop: cannot reserve %zu B of shared memory", mc::mc_smem_bytes());
+        return LHB200_ECUDA;
+    }
+    if (!reserve_smem(mw::k_miller_warp, mw::smem_bytes(mc::MC_WARPS))) {
+        set_error("k_miller_warp: cannot reserve shared memory");
+        return LHB200_ECUDA;
+    }
+    if (!reserve_smem(fe::k_final_warp, fe::smem_bytes())) {
+        set_error("k_final_warp: cannot reserve shared memory");
+        return LHB200_ECUDA;
+    }
+    g_cfg = c;
+    return LHB200_OK;
+}
 void bls_shutdown();
 
 }  // namespace lhb200
@@ -133,7 +190,6 @@ struct lhb200_bls_batch {
     const lhb200_pubkey_table* table = nullptr;
     uint32_t* d_indices = nullptr;
     uint64_t cap_indices = 0;
-    const uint32_t* in_indices = nullptr;
     uint32_t cap_sets = 0;
     uint64_t cap_keys = 0;
     uint32_t n = 0;
@@ -162,7 +218,7 @@ struct lhb200_bls_batch {
     cudaStream_t s2 = nullptr, s3 = nullptr;
     cudaEvent_t e_h2c = nullptr, e_sig = nullptr;
     cudaEvent_t e_fork = nullptr, e_join = nullptr;
-    cudaEvent_t e_k0 = nullptr, e_k1 = nullptr;  // around the dominant kernel (k_miller_multi), for the roofline
+    cudaEvent_t e_k0 = nullptr, e_k1 = nullptr;  // around the Miller kernel, for the roofline
     cudaEvent_t e_done = nullptr;                // cudaEventBlockingSync: the host wait of long steps
     uint64_t launches_last = 0;
     // cooperative Miller kernel (bls/miller_coop.cuh): parking area for T / Q between rounds, the -g1 argument
@@ -233,6 +289,144 @@ constexpr uint32_t PK_SPLIT_MAX_SETS = 8192;
 constexpr uint32_t HASH_PAIR_MAX_SETS = 4096;    // (at 10 000 sets the plain kernel was the faster one)
 constexpr uint32_t FINAL_WARP_TAIL = 160;             // Miller block products k_final_warp takes directly (one per SM + slack)
 constexpr uint32_t BLOCKING_WAIT_MIN_SETS = 16384;   // lhb200_bls_batch_result: blocking wait for steps of tens of ms
+
+constexpr uint32_t CTAS_PER_SM = 12;          // cap of the grid-stride kernels: fewer threads keep their 1-4 KB stacks in L1/L2
+constexpr uint32_t G2_SUM_WARP_CHUNK = 4;     // points per warp and level of k_g2_sum_warp
+constexpr uint32_t MC_LANES = 30;             // working lanes per warp of k_miller_coop
+
+// Levels of a tree that combines `chunk` values per level until at most `limit` remain; *rest = the values left.
+static uint32_t tree_levels(uint32_t m, uint32_t chunk, uint32_t limit, uint32_t* rest = nullptr) {
+    uint32_t levels = 0;
+    for (; m > limit; levels++) m = cdiv(m, chunk);
+    if (rest) *rest = m;
+    return levels;
+}
+
+// Launches `levels` levels of a reduction tree over the m values at `cur`: launch(in, m, m_out, out) combines runs of
+// `chunk` values into m_out = ceil(m / chunk), alternately into tmp[0] and tmp[1].  Returns the last level's output.
+template <class T, class Launch>
+static const T* reduce_tree(const T* cur, uint32_t m, uint32_t chunk, uint32_t levels, T* const tmp[2], Launch launch) {
+    for (uint32_t l = 0; l < levels; l++, m = cdiv(m, chunk)) {
+        launch(cur, m, cdiv(m, chunk), tmp[l & 1]);
+        cur = tmp[l & 1];
+    }
+    return cur;
+}
+
+// Blocks of the one-thread-per-set kernels over m sets.  Resident CTAs per SM are capped (grid-stride kernels); above
+// the cap every thread takes ceil(m / cap threads) sets, balanced across the grid.
+static uint32_t lane_grid(const Config& c, uint32_t m) {
+    const uint32_t cap = c.n_sm * CTAS_PER_SM;
+    const uint32_t g = cdiv(m, BLS_BLOCK);
+    return g > cap ? cdiv(m, (uint64_t)cdiv(m, cap * BLS_BLOCK) * BLS_BLOCK) : g;
+}
+
+// Every kernel and launch shape of one verify_enqueue.  w is what lhb200_bls_batch_plan reports; the launches read it.
+struct Plan {
+    uint32_t w[LHB200_PLAN_WORDS] = {};
+    uint32_t ng = 0;               // pairs of the hash, Miller and final stages: the sets, or the groups of a grouped batch
+    uint32_t hash_grid = 0;
+    uint32_t miller_out = 0;       // Fp12 values the Miller kernel writes: the product tree's input
+    size_t mc_scratch_words = 0;   // k_miller_coop's parking area for T / Q between rounds
+};
+
+// The selection policy: kernels and shapes from the sizes alone.  n_groups: 0 = not grouped.
+static Plan choose(const Config& c, uint32_t n, uint32_t n_groups, uint32_t max_group, bool indexed, uint32_t n_chunks,
+                   bool pks_aligned) {
+    Plan p;
+    uint32_t* w = p.w;
+    const uint32_t ng = p.ng = n_groups ? n_groups : n;
+    w[LHB200_PLAN_N_SETS] = n;
+    w[LHB200_PLAN_N_SM] = c.n_sm;
+    w[LHB200_PLAN_GROUPS] = n_groups;
+    w[LHB200_PLAN_LANE_GRID] = lane_grid(c, n);
+    w[LHB200_PLAN_LANE_SETS_PER_THREAD] = cdiv(n, (uint64_t)w[LHB200_PLAN_LANE_GRID] * BLS_BLOCK);
+    // latency mode of the two G2 stages (bls/g2_warp.cuh): one warp per signature / message while the batch is small
+    // enough for the warps of one wave (four per block, at most two blocks per SM); measured crossover with the
+    // lane-per-set kernels: ~1 000 sets
+    const bool g2_warp = c.g2_warp && n <= 6 * c.n_sm, hash_warp = c.g2_warp && ng <= 6 * c.n_sm;
+    w[LHB200_PLAN_SIG] = g2_warp ? LHB200_K_SIG_PREPARE_WARP : LHB200_K_SIG_PREPARE;
+    w[LHB200_PLAN_SUM_LEVELS] = tree_levels(n, g2_warp ? G2_SUM_WARP_CHUNK : REDUCE_CHUNK, 1);
+    if (w[LHB200_PLAN_SUM_LEVELS]) w[LHB200_PLAN_SUM] = g2_warp ? LHB200_K_G2_SUM_WARP : LHB200_K_G2_REDUCE;
+    w[LHB200_PLAN_LAST_MILLER] = !c.miller_coop;
+    // latency mode of the plain hash: two threads per message (one SSWU map each)
+    w[LHB200_PLAN_HASH] = hash_warp ? LHB200_K_HASH_TO_G2_WARP
+                          : ng <= HASH_PAIR_MAX_SETS ? LHB200_K_HASH_TO_G2_PAIR : LHB200_K_HASH_TO_G2;
+    p.hash_grid = hash_warp ? cdiv(ng, GW_WPB) : ng <= HASH_PAIR_MAX_SETS ? cdiv(2 * ng, BLS_BLOCK) : lane_grid(c, ng);
+    // Explicit keys: slice-parallel sums for small and medium batches (a 512-key list is 64 + 8 additions deep instead
+    // of 512), one thread per set above.  Key ingest through the TMA unit (bulk async copies into a shared-memory ring;
+    // 16-byte aligned keys) is opt-in: on the H100 the plain kernel is faster at every size measured (100 000 sets x 128
+    // keys: 111.8 against 119.5 ms per step; 40 000 sets: 49.0 against 53.3 ms).  The ring needs a shared-memory
+    // carve-out, and an SM running blocks of the (shared-memory-free, full-L1) k_sig_prepare / k_hash_to_g2 cannot take
+    // a block with a different carve-out until it drains; the kernel itself is bound by stack traffic, not by key loads.
+    w[LHB200_PLAN_KEY] = indexed ? LHB200_K_PK_AGGREGATE_INDEXED
+                         : c.pk_tma && pks_aligned ? LHB200_K_PK_AGGREGATE_TMA
+                         : n <= PK_SPLIT_MAX_SETS ? LHB200_K_PK_PARTIAL_COMBINE : LHB200_K_PK_AGGREGATE;
+    w[LHB200_PLAN_KEY_CHUNKS] = n_chunks;
+    if (n_groups) {   // until one run of GROUP_CHUNK^levels covers the largest group
+        w[LHB200_PLAN_GROUP_SUM] = LHB200_K_G1_GROUP_SUM;
+        w[LHB200_PLAN_GROUP_SUM_LEVELS] = std::max<uint32_t>(1, tree_levels(max_group, GROUP_CHUNK, 1));
+    }
+    // Miller loops over the ng pairs and, except with k_miller_multi, the pair (-g1, sum r sig)
+    const uint32_t n_total = ng + 1, max_warps = c.n_sm * mc::MC_WARPS;
+    uint32_t tail_max = COOP_TAIL;   // Miller products the final kernel folds itself
+    if (c.miller_coop && c.miller_warp && n_total <= max_warps) {
+        // Latency mode (bls/miller_warp.cuh): while every pair can have a warp of its own in one wave, a whole warp runs
+        // one Miller loop at Fp granularity, far shorter than a lane-per-set loop.  Four warps per block (one per
+        // scheduler) up to 256 pairs, eight above; <= 64 block products need no k_fp12_reduce level.
+        const uint32_t wpb = n_total <= 4 * COOP_TAIL ? 4 : mc::MC_WARPS;
+        w[LHB200_PLAN_MILLER] = LHB200_K_MILLER_WARP;
+        w[LHB200_PLAN_MILLER_WPB] = wpb;
+        w[LHB200_PLAN_MILLER_SPW] = 1;
+        w[LHB200_PLAN_MILLER_GRID] = p.miller_out = cdiv(n_total, wpb);
+    } else if (c.miller_coop) {
+        // Cooperative shared-memory Miller loop (bls/miller_coop.cuh): one block of 8 independent warps per SM, 30
+        // working lanes per warp, every lane runs `rounds` sets, six lanes share one accumulator.  Small batches spread
+        // over more, emptier warps (latency), large ones fill 8 x n_sm.
+        uint32_t spw = cdiv(cdiv(n_total, max_warps), MC_LANES) * MC_LANES;   // sets per warp, whole rounds
+        uint32_t n_warps, mgrid;
+        // Batches below one full round per warp.  A warp's five groups take one set each at no extra latency (SIMT), and
+        // every further set of a group adds one serial sparse product per iteration (81 multiply units for a 1-set
+        // group, 141 for a full one).  Small batches therefore use at least five sets per warp, at most 256 warps, four
+        // per block (one per scheduler): <= 64 block products, which the final kernel folds itself (no k_fp12_reduce
+        // level, a level of single-thread latency).  Above that: as few sets per warp as the 8 x n_sm warp budget allows.
+        constexpr uint32_t FEW_WARPS = 4 * COOP_TAIL;
+        const bool few = n_total <= FEW_WARPS * MC_LANES;
+        if (few) {
+            spw = std::min<uint32_t>(MC_LANES, std::max<uint32_t>(5, cdiv(cdiv(n_total, FEW_WARPS), 5) * 5));
+            n_warps = cdiv(n_total, spw);
+            mgrid = cdiv(n_warps, 4);
+        } else {
+            if (n_total <= max_warps * MC_LANES) spw = std::max<uint32_t>(1, cdiv(n_total, max_warps));
+            n_warps = cdiv(n_total, spw);
+            // warps are dealt round-robin to blocks (gw = warp_in_block * grid + block): few warps spread over all SMs
+            mgrid = std::max<uint32_t>(std::min<uint32_t>(c.n_sm, n_warps), cdiv(n_warps, mc::MC_WARPS));
+        }
+        const uint32_t rounds_cap = cdiv(spw, MC_LANES);
+        w[LHB200_PLAN_MILLER] = LHB200_K_MILLER_COOP;
+        w[LHB200_PLAN_MILLER_WPB] = mc::MC_WARPS;
+        w[LHB200_PLAN_MILLER_SPW] = spw;
+        w[LHB200_PLAN_MILLER_GRID] = p.miller_out = mgrid;   // one product per block
+        w[LHB200_PLAN_MILLER_ROUNDS_CAP] = rounds_cap;
+        w[LHB200_PLAN_MILLER_FEW_WARPS] = few;
+        p.mc_scratch_words = (size_t)mgrid * mc::MC_WARPS * rounds_cap * 2 * mc::TWORDS * 32;
+        // k_final_warp folds the block products itself (8 warps share the products): no single-thread product level
+        if (c.final_warp) tail_max = FINAL_WARP_TAIL;
+    } else {
+        // Sets per thread: k = ceil(ng / resident threads) (<= MILLER_KMAX) share their Fp12 squarings in one thread, so
+        // a 100 k batch is ONE wave of 3-set groups instead of three waves of single Miller loops.
+        const uint32_t resident = c.n_sm * c.miller_occ * MILLER_BLOCK;
+        const uint32_t mk = std::min<uint32_t>(cdiv(ng, resident), MILLER_KMAX);
+        p.miller_out = cdiv(ng, mk);
+        w[LHB200_PLAN_MILLER] = LHB200_K_MILLER_MULTI;
+        w[LHB200_PLAN_MILLER_SPW] = mk;
+        w[LHB200_PLAN_MILLER_GRID] = std::min<uint32_t>(cdiv(p.miller_out, MILLER_BLOCK), c.n_sm * c.miller_occ);
+    }
+    w[LHB200_PLAN_FP12_REDUCE_LEVELS] = tree_levels(p.miller_out, REDUCE_CHUNK, tail_max, &w[LHB200_PLAN_N_TAIL]);
+    // k_final_warp takes no k_last_miller value: only the kernels that pair (-g1, sum r sig) themselves feed it
+    w[LHB200_PLAN_FINAL] = c.final_warp && c.miller_coop ? LHB200_K_FINAL_WARP : LHB200_K_FINAL_COOP;
+    return p;
+}
 
 // ---- pool of batch handles behind lhb200_verify_signature_sets -------------------------------------------------
 namespace {
@@ -555,9 +749,8 @@ constexpr uint32_t GROUP_MIN_REPEAT_DIV = 8;
 // Host uploads: group the sets by message and queue the CSR and the distinct messages on `s`.  n_groups stays 0 (the
 // ungrouped path) when too few messages repeat, or with LHB_GROUP_MESSAGES=0.
 static int32_t upload_groups(lhb200_bls_batch* b, const uint8_t* msgs, uint32_t n, cudaStream_t s) {
-    static const int group_env = [] { const char* e = getenv("LHB_GROUP_MESSAGES"); return e ? atoi(e) : 1; }();
     b->n_groups = 0;
-    if (!group_env || n < 2) return LHB200_OK;
+    if (!g_cfg.group_messages || n < 2) return LHB200_OK;
     MsgGrouper& g = b->grouper;
     const uint32_t min_repeats = std::max<uint32_t>(1, n / GROUP_MIN_REPEAT_DIV);
     const uint32_t ng = g.run(msgs, n, min_repeats, &b->max_group);
@@ -569,42 +762,54 @@ static int32_t upload_groups(lhb200_bls_batch* b, const uint8_t* msgs, uint32_t 
     return LHB200_OK;
 }
 
+// What the three host uploads share.  Checks the arguments, draws the scalars into b->rbuf when rands is NULL (or
+// rejects a zero one), queues the copies of the signatures, messages, offsets and scalars and the message grouping on
+// `s`, and binds the batch's own buffers as its inputs.  `keys` is the key buffer (at most cap_keys keys) or, with a
+// table, the key indices; the caller copies them.
+static int32_t stage_inputs(const char* fn, lhb200_bls_batch* b, const lhb200_pubkey_table* table, const uint8_t* sigs,
+                            const uint8_t* msgs, const void* keys, const uint32_t* pk_offsets, const uint64_t* rands,
+                            uint32_t n_sets, cudaStream_t s) {
+    if (!b || n_sets == 0 || n_sets > b->cap_sets || !sigs || !msgs || !pk_offsets) {
+        set_error("%s: bad arguments", fn);
+        return LHB200_EINVAL;
+    }
+    const uint64_t n_keys = pk_offsets[n_sets];
+    if (!table && n_keys > b->cap_keys) { set_error("%s: more keys than the batch holds", fn); return LHB200_EINVAL; }
+    if (n_keys && !keys) { set_error("%s: no keys given", fn); return LHB200_EINVAL; }
+    for (uint32_t i = 0; i < n_sets; i++)
+        if (pk_offsets[i] > pk_offsets[i + 1]) { set_error("%s: offsets not monotone", fn); return LHB200_EINVAL; }
+    if (!rands) {
+        b->rbuf.resize(n_sets);
+        if (!gen_rands(b->rbuf.data(), n_sets)) { set_error("%s: getrandom(2) failed", fn); return LHB200_ECUDA; }
+        rands = b->rbuf.data();
+    } else {
+        for (uint32_t i = 0; i < n_sets; i++)
+            if (rands[i] == 0) { set_error("%s: zero random scalar", fn); return LHB200_EINVAL; }
+    }
+    LHB_CUDA(cudaMemcpyAsync(b->d_sigs, sigs, (size_t)n_sets * 96, cudaMemcpyHostToDevice, s));
+    LHB_CUDA(cudaMemcpyAsync(b->d_msgs, msgs, (size_t)n_sets * 32, cudaMemcpyHostToDevice, s));
+    LHB_CUDA(cudaMemcpyAsync(b->d_offsets, pk_offsets, (size_t)(n_sets + 1) * 4, cudaMemcpyHostToDevice, s));
+    LHB_CUDA(cudaMemcpyAsync(b->d_rands, rands, (size_t)n_sets * 8, cudaMemcpyHostToDevice, s));
+    if (int32_t rc = upload_groups(b, msgs, n_sets, s)) return rc;
+    b->n = n_sets;
+    b->n_chunks = 0;
+    b->in_sigs = b->d_sigs; b->in_msgs = b->d_msgs; b->in_pks = table ? nullptr : b->d_pks;
+    b->in_offsets = b->d_offsets; b->in_rands = b->d_rands;
+    b->table = table;
+    return LHB200_OK;
+}
+
 // Copy host inputs into the batch's device buffers.  rands == NULL: drawn here.
 int32_t lhb200_bls_batch_upload(lhb200_bls_batch* b, const uint8_t* sigs, const uint8_t* msgs, const uint8_t* pks,
                                 const uint32_t* pk_offsets, const uint64_t* rands, uint32_t n_sets) {
     LHB_REQUIRE_READY();
-    if (!b || n_sets == 0 || n_sets > b->cap_sets || !sigs || !msgs || !pk_offsets) {
-        set_error("bls_batch_upload: bad arguments");
-        return LHB200_EINVAL;
-    }
-    const uint64_t n_keys = pk_offsets[n_sets];
-    if (n_keys > b->cap_keys || (n_keys && !pks)) { set_error("bls_batch_upload: key buffer too small"); return LHB200_EINVAL; }
-    for (uint32_t i = 0; i < n_sets; i++)
-        if (pk_offsets[i] > pk_offsets[i + 1]) { set_error("bls_batch_upload: offsets not monotone"); return LHB200_EINVAL; }
     Ctx& c = ctx();
     std::lock_guard<std::recursive_mutex> g(c.mu);
-    cudaStream_t s = c.stream;
-    std::vector<uint64_t> rbuf;
-    if (!rands) {
-        rbuf.resize(n_sets);
-        if (!gen_rands(rbuf.data(), n_sets)) { set_error("getrandom(2) failed"); return LHB200_ECUDA; }
-        rands = rbuf.data();
-    } else {
-        for (uint32_t i = 0; i < n_sets; i++)
-            if (rands[i] == 0) { set_error("bls_batch_upload: zero random scalar"); return LHB200_EINVAL; }
-    }
-    LHB_CUDA(cudaMemcpyAsync(b->d_sigs, sigs, (size_t)n_sets * 96, cudaMemcpyHostToDevice, s));
-    LHB_CUDA(cudaMemcpyAsync(b->d_msgs, msgs, (size_t)n_sets * 32, cudaMemcpyHostToDevice, s));
-    if (n_keys) LHB_CUDA(cudaMemcpyAsync(b->d_pks, pks, (size_t)n_keys * 96, cudaMemcpyHostToDevice, s));
-    LHB_CUDA(cudaMemcpyAsync(b->d_offsets, pk_offsets, (size_t)(n_sets + 1) * 4, cudaMemcpyHostToDevice, s));
-    LHB_CUDA(cudaMemcpyAsync(b->d_rands, rands, (size_t)n_sets * 8, cudaMemcpyHostToDevice, s));
-    if (int32_t rc = upload_groups(b, msgs, n_sets, s)) return rc;
-    LHB_CUDA(cudaStreamSynchronize(s));  // rbuf / caller buffers may go away
-    b->n = n_sets;
-    b->n_chunks = 0;
-    b->in_sigs = b->d_sigs; b->in_msgs = b->d_msgs; b->in_pks = b->d_pks;
-    b->in_offsets = b->d_offsets; b->in_rands = b->d_rands;
-    b->table = nullptr;
+    if (int32_t rc = stage_inputs("bls_batch_upload", b, nullptr, sigs, msgs, pks, pk_offsets, rands, n_sets, c.stream))
+        return rc;
+    const uint64_t n_keys = pk_offsets[n_sets];
+    if (n_keys) LHB_CUDA(cudaMemcpyAsync(b->d_pks, pks, (size_t)n_keys * 96, cudaMemcpyHostToDevice, c.stream));
+    LHB_CUDA(cudaStreamSynchronize(c.stream));  // caller buffers may go away
     return LHB200_OK;
 }
 
@@ -616,33 +821,15 @@ int32_t lhb200_bls_batch_upload(lhb200_bls_batch* b, const uint8_t* sigs, const 
 int32_t lhb200_bls_batch_upload_async(lhb200_bls_batch* b, const uint8_t* sigs, const uint8_t* msgs, const uint8_t* pks,
                                       const uint32_t* pk_offsets, const uint64_t* rands, uint32_t n_sets, void* stream) {
     LHB_REQUIRE_READY();
-    if (!b || n_sets == 0 || n_sets > b->cap_sets || !sigs || !msgs || !pk_offsets) {
-        set_error("bls_batch_upload_async: bad arguments");
-        return LHB200_EINVAL;
-    }
-    const uint64_t n_keys = pk_offsets[n_sets];
-    if (n_keys > b->cap_keys || (n_keys && !pks)) { set_error("bls_batch_upload_async: key buffer too small"); return LHB200_EINVAL; }
-    for (uint32_t i = 0; i < n_sets; i++)
-        if (pk_offsets[i] > pk_offsets[i + 1]) { set_error("bls_batch_upload_async: offsets not monotone"); return LHB200_EINVAL; }
     cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx().stream;
-    if (!rands) {
-        b->rbuf.resize(n_sets);
-        if (!gen_rands(b->rbuf.data(), n_sets)) { set_error("getrandom(2) failed"); return LHB200_ECUDA; }
-        rands = b->rbuf.data();
-    } else {
-        for (uint32_t i = 0; i < n_sets; i++)
-            if (rands[i] == 0) { set_error("bls_batch_upload_async: zero random scalar"); return LHB200_EINVAL; }
-    }
+    if (int32_t rc = stage_inputs("bls_batch_upload_async", b, nullptr, sigs, msgs, pks, pk_offsets, rands, n_sets, s))
+        return rc;
     // the previous verify on this batch may still be reading d_pks: order the new copies behind it
     LHB_CUDA(cudaEventRecord(b->e_copy_free, s));
     for (cudaStream_t st : b->s_pk) LHB_CUDA(cudaStreamWaitEvent(st, b->e_copy_free, 0));
-    LHB_CUDA(cudaMemcpyAsync(b->d_sigs, sigs, (size_t)n_sets * 96, cudaMemcpyHostToDevice, s));
-    LHB_CUDA(cudaMemcpyAsync(b->d_msgs, msgs, (size_t)n_sets * 32, cudaMemcpyHostToDevice, s));
-    LHB_CUDA(cudaMemcpyAsync(b->d_offsets, pk_offsets, (size_t)(n_sets + 1) * 4, cudaMemcpyHostToDevice, s));
-    LHB_CUDA(cudaMemcpyAsync(b->d_rands, rands, (size_t)n_sets * 8, cudaMemcpyHostToDevice, s));
-    if (int32_t rc = upload_groups(b, msgs, n_sets, s)) return rc;
     LHB_CUDA(cudaEventRecord(b->e_small, s));
     // chunks of whole sets, ~equal key counts
+    const uint64_t n_keys = pk_offsets[n_sets];
     int nc = (int)std::min<uint64_t>(lhb200_bls_batch::MAX_CHUNKS, std::max<uint64_t>(1, n_keys * 96 / (32u << 20)));
     nc = std::min<int>(nc, (int)n_sets);
     b->chunk_lo[0] = 0;
@@ -662,10 +849,6 @@ int32_t lhb200_bls_batch_upload_async(lhb200_bls_batch* b, const uint8_t* sigs, 
     }
     b->n_chunks = nc;
     b->h_pks = pks;
-    b->n = n_sets;
-    b->in_sigs = b->d_sigs; b->in_msgs = b->d_msgs; b->in_pks = b->d_pks;
-    b->in_offsets = b->d_offsets; b->in_rands = b->d_rands;
-    b->table = nullptr;
     return LHB200_OK;
 }
 
@@ -720,41 +903,22 @@ int32_t lhb200_bls_batch_upload_indexed(lhb200_bls_batch* b, const lhb200_pubkey
                                         const uint8_t* msgs, const uint32_t* key_indices, const uint32_t* pk_offsets,
                                         const uint64_t* rands, uint32_t n_sets) {
     LHB_REQUIRE_READY();
-    if (!b || !table || n_sets == 0 || n_sets > b->cap_sets || !sigs || !msgs || !pk_offsets) {
-        set_error("bls_batch_upload_indexed: bad arguments");
-        return LHB200_EINVAL;
-    }
-    const uint64_t n_keys = pk_offsets[n_sets];
-    if (n_keys && !key_indices) return LHB200_EINVAL;
-    for (uint32_t i = 0; i < n_sets; i++)
-        if (pk_offsets[i] > pk_offsets[i + 1]) { set_error("bls_batch_upload_indexed: offsets not monotone"); return LHB200_EINVAL; }
+    if (!table) { set_error("bls_batch_upload_indexed: no pubkey table"); return LHB200_EINVAL; }
     Ctx& c = ctx();
     std::lock_guard<std::recursive_mutex> g(c.mu);
     cudaStream_t s = c.stream;
+    if (int32_t rc = stage_inputs("bls_batch_upload_indexed", b, table, sigs, msgs, key_indices, pk_offsets, rands, n_sets, s))
+        return rc;
+    const uint64_t n_keys = pk_offsets[n_sets];
     if (n_keys > b->cap_indices) {
-        if (b->d_indices) { cudaStreamSynchronize(s); cudaFree(b->d_indices); b->d_indices = nullptr; }
+        b->n = 0;   // no inputs until the indices have a buffer
+        if (b->d_indices) { cudaStreamSynchronize(s); cudaFree(b->d_indices); b->d_indices = nullptr; b->cap_indices = 0; }
         LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&b->d_indices), std::max<uint64_t>(n_keys, 1) * 4));
         b->cap_indices = n_keys;
+        b->n = n_sets;
     }
-    std::vector<uint64_t> rbuf;
-    if (!rands) {
-        rbuf.resize(n_sets);
-        if (!gen_rands(rbuf.data(), n_sets)) { set_error("getrandom(2) failed"); return LHB200_ECUDA; }
-        rands = rbuf.data();
-    }
-    else for (uint32_t i = 0; i < n_sets; i++) if (rands[i] == 0) { set_error("zero random scalar"); return LHB200_EINVAL; }
-    LHB_CUDA(cudaMemcpyAsync(b->d_sigs, sigs, (size_t)n_sets * 96, cudaMemcpyHostToDevice, s));
-    LHB_CUDA(cudaMemcpyAsync(b->d_msgs, msgs, (size_t)n_sets * 32, cudaMemcpyHostToDevice, s));
     if (n_keys) LHB_CUDA(cudaMemcpyAsync(b->d_indices, key_indices, (size_t)n_keys * 4, cudaMemcpyHostToDevice, s));
-    LHB_CUDA(cudaMemcpyAsync(b->d_offsets, pk_offsets, (size_t)(n_sets + 1) * 4, cudaMemcpyHostToDevice, s));
-    LHB_CUDA(cudaMemcpyAsync(b->d_rands, rands, (size_t)n_sets * 8, cudaMemcpyHostToDevice, s));
-    if (int32_t rc = upload_groups(b, msgs, n_sets, s)) return rc;
     LHB_CUDA(cudaStreamSynchronize(s));
-    b->n = n_sets;
-    b->in_sigs = b->d_sigs; b->in_msgs = b->d_msgs; b->in_pks = nullptr;
-    b->in_offsets = b->d_offsets; b->in_rands = b->d_rands; b->in_indices = b->d_indices;
-    b->n_chunks = 0;
-    b->table = table;
     return LHB200_OK;
 }
 
@@ -780,132 +944,65 @@ int32_t lhb200_bls_batch_set_device_inputs(lhb200_bls_batch* b, const void* d_si
     return LHB200_OK;
 }
 
-int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
-    LHB_REQUIRE_READY();
-    if (!b || b->n == 0 || !b->in_sigs) { set_error("bls_batch_verify_enqueue: no inputs"); return LHB200_EINVAL; }
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx().stream;
-    const uint32_t n = b->n;
-    // Resident CTAs per SM are capped (grid-stride kernels): fewer threads keep their 1-4 KB stacks in L1/L2.
-    // LHB_BLS_CTAS_PER_SM overrides (tuning knob; 0 = one CTA per BLS_BLOCK sets, i.e. no cap).
-    static const int ctas_per_sm = [] { const char* e = getenv("LHB_BLS_CTAS_PER_SM"); return e ? atoi(e) : 12; }();
-    static const int n_sm = [] { int v = 132; cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, ctx().device); return v; }();
-    auto lane_grid = [&](uint32_t m) {
-        uint32_t g = cdiv(m, BLS_BLOCK);
-        if (ctas_per_sm > 0 && g > (uint32_t)(n_sm * ctas_per_sm)) {
-            const uint32_t max_thr = (uint32_t)(n_sm * ctas_per_sm) * BLS_BLOCK;
-            const uint32_t per_thread = cdiv(m, max_thr);        // sets per thread, balanced across the grid
-            g = cdiv(m, (uint64_t)per_thread * BLS_BLOCK);
-        }
-        return g;
-    };
-    const uint32_t grid = lane_grid(n);
-    // Grouped by message (host uploads with a repeated message): the signature and key stages run over the n sets, the
-    // hash, Miller and final stages over the ng distinct messages, each with the kernels and shapes chosen for its count.
-    const bool grouped = b->n_groups != 0;
-    const uint32_t ng = grouped ? b->n_groups : n;
-    uint64_t launches = 0;
-    uint32_t* plan = b->plan;
-    memset(plan, 0, sizeof b->plan);
-    plan[LHB200_PLAN_N_SETS] = n;
-    plan[LHB200_PLAN_N_SM] = (uint32_t)n_sm;
-    plan[LHB200_PLAN_GROUPS] = b->n_groups;
-    plan[LHB200_PLAN_LANE_GRID] = grid;
-    plan[LHB200_PLAN_LANE_SETS_PER_THREAD] = cdiv(n, (uint64_t)grid * BLS_BLOCK);
-    // key ingest through the TMA unit (bulk async copies into a shared-memory ring); needs 16-byte aligned keys.
-    // Opt-in (LHB_PK_TMA=1): on the H100 the plain kernel is faster at every size measured (100 000 sets x 128 keys:
-    // 111.8 against 119.5 ms per step; 40 000 sets: 49.0 against 53.3 ms).  The ring needs a shared-memory carve-out,
-    // and an SM running blocks of the (shared-memory-free, full-L1) k_sig_prepare / k_hash_to_g2 cannot take a block
-    // with a different carve-out until it drains; the kernel itself is bound by stack traffic, not by key loads.
-    static const int pk_tma_env = [] { const char* e = getenv("LHB_PK_TMA"); return e ? atoi(e) : 0; }();
-    const bool pk_tma_fit = b->in_pks && ((uintptr_t)b->in_pks & 15) == 0;
-    const bool pk_tma = pk_tma_fit && pk_tma_env != 0;
-    if (b->n_chunks) LHB_CUDA(cudaStreamWaitEvent(s, b->e_small, 0));  // streamed upload: small arrays first
-    LHB_CUDA(cudaMemsetAsync(b->d_status, 0, n, s));
-    LHB_CUDA(cudaMemsetAsync(b->d_fail, 0, 4, s));
-    LHB_CUDA(cudaMemsetAsync(b->d_ok, 0, 4, s));
-    // Three independent per-set stages run concurrently (they matter for small batches, where each kernel is a
-    // latency-bound handful of warps): s2 = signatures (+ their sum tree + the last Miller loop), s3 = hash_to_g2,
-    // s = key aggregation; the Miller kernel joins s and s3, k_final joins s2.
-    LHB_CUDA(cudaEventRecord(b->e_fork, s));
-    LHB_CUDA(cudaStreamWaitEvent(b->s2, b->e_fork, 0));
-    LHB_CUDA(cudaStreamWaitEvent(b->s3, b->e_fork, 0));
-    // latency mode of the two G2 stages (bls/g2_warp.cuh): one warp per signature / message while the batch is small
-    // enough for the warps of one wave (four per block, at most two blocks per SM)
-    static const int g2_warp_env = [] { const char* e = getenv("LHB_G2_WARP"); return e ? atoi(e) : 1; }();
-    const bool g2_warp = g2_warp_env && n <= 6u * (uint32_t)n_sm;   // measured crossover with the lane-per-set kernels: ~1 000 sets
-    const bool hash_warp = g2_warp_env && ng <= 6u * (uint32_t)n_sm;
-    constexpr uint32_t GW_WPB = 4;
+// ---- verify_enqueue: one launch helper per stage, following the Plan ------------------------------------------
+// s2: r_i sig_i, their sum tree and, with k_miller_multi, the pair (-g1, sum r sig) on its own
+static int32_t launch_signatures(lhb200_bls_batch* b, const Plan& p, uint64_t& launches) {
+    const uint32_t n = b->n, *w = p.w;
     const size_t gw_smem = gw::smem_bytes(GW_WPB);
-    if (g2_warp || hash_warp) {   // working sets + a shared-memory copy of the phase tables: above the 48 KB default
-        static const bool gw_attr_ok = [&] {
-            return cudaFuncSetAttribute(gw::k_sig_prepare_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gw_smem) == cudaSuccess &&
-                   cudaFuncSetAttribute(gw::k_hash_to_g2_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gw_smem) == cudaSuccess &&
-                   cudaFuncSetAttribute(gw::k_g2_sum_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gw_smem) == cudaSuccess;
-        }();
-        if (!gw_attr_ok) { set_error("g2 warp kernels: cannot reserve %zu B of shared memory", gw_smem); return LHB200_ECUDA; }
-    }
-    plan[LHB200_PLAN_SIG] = g2_warp ? LHB200_K_SIG_PREPARE_WARP : LHB200_K_SIG_PREPARE;
-    if (g2_warp)
+    if (w[LHB200_PLAN_SIG] == LHB200_K_SIG_PREPARE_WARP)
         gw::k_sig_prepare_warp<<<cdiv(n, GW_WPB), 32 * GW_WPB, gw_smem, b->s2>>>(b->in_sigs, b->in_rands, n, b->d_sigr,
                                                                                b->d_status, b->d_fail);
     else
-        k_sig_prepare<<<grid, BLS_BLOCK, 0, b->s2>>>(b->in_sigs, b->in_rands, n, b->d_sigr, b->d_status, b->d_fail);
-    launches++;
+        k_sig_prepare<<<w[LHB200_PLAN_LANE_GRID], BLS_BLOCK, 0, b->s2>>>(b->in_sigs, b->in_rands, n, b->d_sigr, b->d_status,
+                                                                        b->d_fail);
     LHB_CUDA(cudaEventRecord(b->e_sig, b->s2));
-    {
-        const G2Jac* cur = b->d_sigr;
-        uint32_t m = n;
-        int flip = 0;
-        while (m > 1) {
-            if (g2_warp) {   // latency mode: warp-wide additions, four points per warp and level
-                constexpr uint32_t CH = 4;
-                const uint32_t mo = cdiv(m, CH);
-                gw::k_g2_sum_warp<<<cdiv(mo, GW_WPB), 32 * GW_WPB, gw_smem, b->s2>>>(cur, m, CH, b->d_sig_tmp[flip]);
-                launches++;
-                plan[LHB200_PLAN_SUM] = LHB200_K_G2_SUM_WARP;
-                plan[LHB200_PLAN_SUM_LEVELS]++;
-                cur = b->d_sig_tmp[flip];
-                flip ^= 1;
-                m = mo;
-                continue;
-            }
-            const uint32_t mo = cdiv(m, REDUCE_CHUNK);
-            k_g2_reduce<<<cdiv(mo, BLS_BLOCK), BLS_BLOCK, 0, b->s2>>>(cur, m, REDUCE_CHUNK, b->d_sig_tmp[flip]);
-            launches++;
-            plan[LHB200_PLAN_SUM] = LHB200_K_G2_REDUCE;
-            plan[LHB200_PLAN_SUM_LEVELS]++;
-            cur = b->d_sig_tmp[flip];
-            flip ^= 1;
-            m = mo;
-        }
-        b->d_sig_sum = cur;
-        static const int miller_coop_s2 = [] { const char* e = getenv("LHB_MILLER_COOP"); return e ? atoi(e) : 1; }();
-        if (!miller_coop_s2) {
-            k_last_miller<<<1, 32, 0, b->s2>>>(cur, b->d_flast);
-            launches++;
-            plan[LHB200_PLAN_LAST_MILLER] = 1;
-        }
-        LHB_CUDA(cudaEventRecord(b->e_join, b->s2));
+    const bool warp = w[LHB200_PLAN_SUM] == LHB200_K_G2_SUM_WARP;   // latency mode: warp-wide additions
+    b->d_sig_sum = reduce_tree(b->d_sigr, n, warp ? G2_SUM_WARP_CHUNK : REDUCE_CHUNK, w[LHB200_PLAN_SUM_LEVELS], b->d_sig_tmp,
+                               [&](const G2Jac* in, uint32_t m, uint32_t mo, G2Jac* out) {
+                                   if (warp)
+                                       gw::k_g2_sum_warp<<<cdiv(mo, GW_WPB), 32 * GW_WPB, gw_smem, b->s2>>>(in, m, G2_SUM_WARP_CHUNK, out);
+                                   else
+                                       k_g2_reduce<<<cdiv(mo, BLS_BLOCK), BLS_BLOCK, 0, b->s2>>>(in, m, REDUCE_CHUNK, out);
+                               });
+    launches += 1 + w[LHB200_PLAN_SUM_LEVELS];
+    if (w[LHB200_PLAN_LAST_MILLER]) {
+        k_last_miller<<<1, 32, 0, b->s2>>>(b->d_sig_sum, b->d_flast);
+        launches++;
     }
-    // grouped: one hash per distinct message, d_h[g] = H(message of group g)
-    const uint8_t* h_msgs = grouped ? b->d_gmsgs : b->in_msgs;
-    plan[LHB200_PLAN_HASH] = hash_warp ? LHB200_K_HASH_TO_G2_WARP
-                             : ng <= HASH_PAIR_MAX_SETS ? LHB200_K_HASH_TO_G2_PAIR : LHB200_K_HASH_TO_G2;
-    if (hash_warp)
-        gw::k_hash_to_g2_warp<<<cdiv(ng, GW_WPB), 32 * GW_WPB, gw_smem, b->s3>>>(h_msgs, ng, b->d_h);
-    else if (ng <= HASH_PAIR_MAX_SETS)   // latency mode: two threads per message (one SSWU map each)
-        k_hash_to_g2_pair<<<cdiv(2 * ng, BLS_BLOCK), BLS_BLOCK, 0, b->s3>>>(h_msgs, ng, b->d_h);
-    else
-        k_hash_to_g2<<<lane_grid(ng), BLS_BLOCK, 0, b->s3>>>(h_msgs, ng, b->d_h);
+    LHB_CUDA(cudaEventRecord(b->e_join, b->s2));
+    return LHB200_OK;
+}
+
+// s3: H(m_i), or H(message of group g) in a grouped batch
+static int32_t launch_hash(lhb200_bls_batch* b, const Plan& p, uint64_t& launches) {
+    const uint8_t* msgs = b->n_groups ? b->d_gmsgs : b->in_msgs;
+    switch (p.w[LHB200_PLAN_HASH]) {
+    case LHB200_K_HASH_TO_G2_WARP:
+        gw::k_hash_to_g2_warp<<<p.hash_grid, 32 * GW_WPB, gw::smem_bytes(GW_WPB), b->s3>>>(msgs, p.ng, b->d_h);
+        break;
+    case LHB200_K_HASH_TO_G2_PAIR: k_hash_to_g2_pair<<<p.hash_grid, BLS_BLOCK, 0, b->s3>>>(msgs, p.ng, b->d_h); break;
+    default: k_hash_to_g2<<<p.hash_grid, BLS_BLOCK, 0, b->s3>>>(msgs, p.ng, b->d_h);
+    }
     launches++;
     LHB_CUDA(cudaEventRecord(b->e_h2c, b->s3));
-    // explicit keys, sets [lo, lo + cnt): TMA ring for GPU-filling batches, slice-parallel sums for small and medium
-    // ones (a 512-key list is 64 + 8 additions deep instead of 512), one thread per set in between
-    auto launch_pk = [&](uint32_t lo, uint32_t cnt, cudaStream_t st) {
-        if (pk_tma) {
+    return LHB200_OK;
+}
+
+// r_i apk_i: from the pubkey table or the key buffer on s, or, after a streamed upload, chunk by chunk on the
+// (high-priority) stream that copies the chunk, as soon as its keys have landed
+static int32_t launch_keys(lhb200_bls_batch* b, const Plan& p, cudaStream_t s, uint64_t& launches) {
+    const uint32_t key = p.w[LHB200_PLAN_KEY], grid = p.w[LHB200_PLAN_LANE_GRID];
+    if (key == LHB200_K_PK_AGGREGATE_INDEXED) {
+        k_pk_aggregate_indexed<<<grid, BLS_BLOCK, 0, s>>>(b->table->d_keys, (uint32_t)b->table->len, b->d_indices,
+                                                         b->in_offsets, b->in_rands, b->n, b->d_p, b->d_pk_status, b->d_fail);
+        launches++;
+        return LHB200_OK;
+    }
+    auto launch_pk = [&](uint32_t lo, uint32_t cnt, cudaStream_t st) {   // sets [lo, lo + cnt)
+        if (key == LHB200_K_PK_AGGREGATE_TMA) {
             k_pk_aggregate_tma<<<cdiv(cnt, BLS_BLOCK), BLS_BLOCK, 0, st>>>(b->in_pks, b->in_offsets + lo, b->in_rands + lo, cnt,
                                                                           b->d_p + lo, b->d_pk_status + lo, b->d_fail);
-        } else if (n <= PK_SPLIT_MAX_SETS) {
+        } else if (key == LHB200_K_PK_PARTIAL_COMBINE) {
             k_pk_partial<<<cdiv(cnt * PK_SLICES, BLS_BLOCK), BLS_BLOCK, 0, st>>>(
                 b->in_pks, b->in_offsets + lo, cnt, b->d_pk_part + (size_t)lo * PK_SLICES, b->d_pk_part_bad + (size_t)lo * PK_SLICES);
             k_pk_combine<<<cdiv(cnt, BLS_BLOCK), BLS_BLOCK, 0, st>>>(
@@ -918,232 +1015,120 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
         }
         launches++;
     };
-    plan[LHB200_PLAN_KEY] = b->table ? LHB200_K_PK_AGGREGATE_INDEXED
-                            : pk_tma ? LHB200_K_PK_AGGREGATE_TMA
-                            : n <= PK_SPLIT_MAX_SETS ? LHB200_K_PK_PARTIAL_COMBINE : LHB200_K_PK_AGGREGATE;
-    plan[LHB200_PLAN_KEY_CHUNKS] = b->table ? 0 : (uint32_t)b->n_chunks;
-    if (b->table) {
-        launches++;
-        k_pk_aggregate_indexed<<<grid, BLS_BLOCK, 0, s>>>(b->table->d_keys, (uint32_t)b->table->len, b->in_indices,
-                                                         b->in_offsets, b->in_rands, n, b->d_p, b->d_pk_status, b->d_fail);
-    } else if (b->n_chunks) {
-        // big pageable key buffers go through the library's pinned ring (see KeyStager)
-        static const int stage_env = [] { const char* e = getenv("LHB_STAGE_PAGEABLE"); return e ? atoi(e) : 1; }();
-        const uint64_t key_bytes = (b->chunk_key[b->n_chunks] - b->chunk_key[0]) * 96;
-        std::unique_lock<std::mutex> stage_lock(g_stager_use, std::defer_lock);
-        bool stage_keys = false;
-        if (stage_env && key_bytes >= STAGE_MIN_BYTES && host_pointer_is_pageable(b->h_pks)) {
-            stage_lock.lock();
-            stage_keys = g_stager.init();
-            if (!stage_keys) stage_lock.unlock();
+    if (!b->n_chunks) {
+        launch_pk(0, b->n, s);
+        return LHB200_OK;
+    }
+    // big pageable key buffers go through the library's pinned ring (see KeyStager)
+    const uint64_t key_bytes = (b->chunk_key[b->n_chunks] - b->chunk_key[0]) * 96;
+    std::unique_lock<std::mutex> stage_lock(g_stager_use, std::defer_lock);
+    bool stage_keys = false;
+    if (g_cfg.stage_pageable && key_bytes >= STAGE_MIN_BYTES && host_pointer_is_pageable(b->h_pks)) {
+        stage_lock.lock();
+        stage_keys = g_stager.init();
+        if (!stage_keys) stage_lock.unlock();
+    }
+    for (int j = 0; j < lhb200_bls_batch::N_PK_STREAMS; j++) LHB_CUDA(cudaStreamWaitEvent(b->s_pk[j], b->e_fork, 0));
+    for (int c = 0; c < b->n_chunks; c++) {
+        const uint32_t lo = b->chunk_lo[c], cnt = b->chunk_lo[c + 1] - lo;
+        const uint64_t k0 = b->chunk_key[c], k1 = b->chunk_key[c + 1];
+        cudaStream_t st = b->s_pk[c % lhb200_bls_batch::N_PK_STREAMS];
+        if (k1 > k0) {
+            if (stage_keys) LHB_CUDA(g_stager.copy(b->d_pks + k0 * 96, b->h_pks + k0 * 96, (k1 - k0) * 96, st));
+            else LHB_CUDA(cudaMemcpyAsync(b->d_pks + k0 * 96, b->h_pks + k0 * 96, (k1 - k0) * 96, cudaMemcpyHostToDevice, st));
         }
-        // aggregate each chunk of sets on the (high-priority) stream that copies it, as soon as its keys have landed
-        for (int j = 0; j < lhb200_bls_batch::N_PK_STREAMS; j++) LHB_CUDA(cudaStreamWaitEvent(b->s_pk[j], b->e_fork, 0));
-        for (int c = 0; c < b->n_chunks; c++) {
-            const uint32_t lo = b->chunk_lo[c], cnt = b->chunk_lo[c + 1] - lo;
-            const uint64_t k0 = b->chunk_key[c], k1 = b->chunk_key[c + 1];
-            if (k1 > k0) {
-                if (stage_keys) {
-                    LHB_CUDA(g_stager.copy(b->d_pks + k0 * 96, b->h_pks + k0 * 96, (k1 - k0) * 96,
-                                           b->s_pk[c % lhb200_bls_batch::N_PK_STREAMS]));
-                } else {
-                    LHB_CUDA(cudaMemcpyAsync(b->d_pks + k0 * 96, b->h_pks + k0 * 96, (k1 - k0) * 96, cudaMemcpyHostToDevice,
-                                             b->s_pk[c % lhb200_bls_batch::N_PK_STREAMS]));
-                }
-            }
-            if (cnt == 0) continue;
-            launch_pk(lo, cnt, b->s_pk[c % lhb200_bls_batch::N_PK_STREAMS]);
-        }
-        for (int j = 0; j < lhb200_bls_batch::N_PK_STREAMS; j++) {
-            LHB_CUDA(cudaEventRecord(b->e_pk[j], b->s_pk[j]));
-            LHB_CUDA(cudaStreamWaitEvent(s, b->e_pk[j], 0));
-        }
-    } else
-        launch_pk(0, n, s);
+        if (cnt) launch_pk(lo, cnt, st);
+    }
+    for (int j = 0; j < lhb200_bls_batch::N_PK_STREAMS; j++) {
+        LHB_CUDA(cudaEventRecord(b->e_pk[j], b->s_pk[j]));
+        LHB_CUDA(cudaStreamWaitEvent(s, b->e_pk[j], 0));
+    }
+    return LHB200_OK;
+}
+
+// Grouped batches: per group, the sum of r_i apk_i over its contributing members, and a skip flag
+static void launch_group_sum(lhb200_bls_batch* b, const Plan& p, cudaStream_t s, uint64_t& launches) {
+    GroupSumArgs ga;
+    ga.P = b->d_p; ga.status = b->d_status; ga.pk_status = b->d_pk_status;
+    ga.members = b->d_members; ga.offsets = b->d_goffsets; ga.n = b->n; ga.n_groups = p.ng;
+    ga.tmp = b->d_gtmp; ga.out_p = b->d_gp; ga.skip = b->d_gskip;
+    const uint32_t levels = p.w[LHB200_PLAN_GROUP_SUM_LEVELS];
+    uint64_t span = 1;
+    for (uint32_t level = 0; level < levels; level++, span *= GROUP_CHUNK)
+        k_g1_group_sum<<<cdiv(b->n, BLS_BLOCK), BLS_BLOCK, 0, s>>>(ga, level, span);
+    launches += levels;
+}
+
+// The Miller kernel between e_k0 and e_k1, then the product tree down to the final kernel's tail (-> *prod).  The
+// kernels pair (P[i], d_h[i]), i < ng, and skip i unless st[i] | pk_st[i] == 0: per set, or per group (the group sums,
+// with the skip flag in both status slots).
+static int32_t launch_miller(lhb200_bls_batch* b, const Plan& p, cudaStream_t s, uint64_t& launches, const Fp12** prod) {
+    const uint32_t* w = p.w;
+    const bool grouped = b->n_groups != 0, multi = w[LHB200_PLAN_MILLER] == LHB200_K_MILLER_MULTI;
+    const G1Proj3* P = grouped ? b->d_gp : b->d_p;
+    const uint8_t* st = grouped ? b->d_gskip : b->d_status;
+    const uint8_t* pk_st = grouped ? b->d_gskip : b->d_pk_status;
+    const uint32_t grid = w[LHB200_PLAN_MILLER_GRID], wpb = w[LHB200_PLAN_MILLER_WPB];
+    if (!multi) LHB_CUDA(cudaStreamWaitEvent(s, b->e_join, 0));   // sum r sig (and -g1) ready
+    LHB_CUDA(cudaEventRecord(b->e_k0, s));
+    if (w[LHB200_PLAN_MILLER] == LHB200_K_MILLER_WARP)
+        mw::k_miller_warp<<<grid, 32 * wpb, mw::smem_bytes((int)wpb), s>>>(P, b->d_h, st, pk_st, p.ng, b->d_sig_sum,
+                                                                         b->d_neg_g1, b->d_f);
+    else if (w[LHB200_PLAN_MILLER] == LHB200_K_MILLER_COOP)
+        mc::k_miller_coop<<<grid, 32 * wpb, mc::mc_smem_bytes(), s>>>(P, b->d_h, st, pk_st, p.ng, b->d_sig_sum, b->d_neg_g1,
+                                                                      w[LHB200_PLAN_MILLER_SPW], b->d_mc_scratch, b->d_f);
+    else
+        k_miller_multi<<<grid, MILLER_BLOCK, 0, s>>>(P, b->d_h, st, pk_st, p.ng, w[LHB200_PLAN_MILLER_SPW], p.miller_out,
+                                                     b->d_f);
+    LHB_CUDA(cudaEventRecord(b->e_k1, s));
+    *prod = reduce_tree<Fp12>(b->d_f, p.miller_out, REDUCE_CHUNK, w[LHB200_PLAN_FP12_REDUCE_LEVELS], b->d_f_tmp,
+                              [&](const Fp12* in, uint32_t m, uint32_t mo, Fp12* out) {
+                                  k_fp12_reduce<<<cdiv(mo, BLS_BLOCK), BLS_BLOCK, 0, s>>>(in, m, REDUCE_CHUNK, out);
+                              });
+    launches += 1 + w[LHB200_PLAN_FP12_REDUCE_LEVELS];
+    if (multi) LHB_CUDA(cudaStreamWaitEvent(s, b->e_join, 0));   // k_final_coop reads k_last_miller's value
+    return LHB200_OK;
+}
+
+int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
+    LHB_REQUIRE_READY();
+    if (!b || b->n == 0 || !b->in_sigs) { set_error("bls_batch_verify_enqueue: no inputs"); return LHB200_EINVAL; }
+    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx().stream;
+    const uint32_t n = b->n;
+    const Plan p = choose(g_cfg, n, b->n_groups, b->max_group, b->table != nullptr, (uint32_t)b->n_chunks,
+                          b->in_pks && ((uintptr_t)b->in_pks & 15) == 0);
+    memcpy(b->plan, p.w, sizeof b->plan);
+    if (p.mc_scratch_words > b->mc_scratch_words) {
+        LHB_CUDA(cudaStreamSynchronize(s));
+        if (b->d_mc_scratch) cudaFree(b->d_mc_scratch);
+        b->d_mc_scratch = nullptr;
+        LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&b->d_mc_scratch), p.mc_scratch_words * 4));
+        b->mc_scratch_words = p.mc_scratch_words;
+    }
+    if (b->n_chunks) LHB_CUDA(cudaStreamWaitEvent(s, b->e_small, 0));  // streamed upload: small arrays first
+    LHB_CUDA(cudaMemsetAsync(b->d_status, 0, n, s));
+    LHB_CUDA(cudaMemsetAsync(b->d_fail, 0, 4, s));
+    LHB_CUDA(cudaMemsetAsync(b->d_ok, 0, 4, s));
+    // Three independent per-set stages run concurrently (they matter for small batches, where each kernel is a
+    // latency-bound handful of warps): s2 = signatures, s3 = hash_to_g2, s = keys.  The Miller kernel joins all three.
+    LHB_CUDA(cudaEventRecord(b->e_fork, s));
+    LHB_CUDA(cudaStreamWaitEvent(b->s2, b->e_fork, 0));
+    LHB_CUDA(cudaStreamWaitEvent(b->s3, b->e_fork, 0));
+    uint64_t launches = 0;
+    const Fp12* prod = nullptr;
+    if (int32_t rc = launch_signatures(b, p, launches)) return rc;
+    if (int32_t rc = launch_hash(b, p, launches)) return rc;
+    if (int32_t rc = launch_keys(b, p, s, launches)) return rc;
     LHB_CUDA(cudaStreamWaitEvent(s, b->e_h2c, 0));
     LHB_CUDA(cudaStreamWaitEvent(s, b->e_sig, 0));    // the Miller kernel reads the status bytes k_sig_prepare may set
-    // The Miller kernels pair (m_p[i], d_h[i]), i < ng, and skip i unless m_st[i] | m_pk_st[i] == 0: per set, or per
-    // group (the group sums, with the skip flag in both status slots).
-    const G1Proj3* m_p = b->d_p;
-    const uint8_t *m_st = b->d_status, *m_pk_st = b->d_pk_status;
-    if (grouped) {
-        GroupSumArgs ga;
-        ga.P = b->d_p; ga.status = b->d_status; ga.pk_status = b->d_pk_status;
-        ga.members = b->d_members; ga.offsets = b->d_goffsets; ga.n = n; ga.n_groups = ng;
-        ga.tmp = b->d_gtmp; ga.out_p = b->d_gp; ga.skip = b->d_gskip;
-        uint64_t span = 1;
-        uint32_t level = 0;
-        do {   // until one run of GROUP_CHUNK^(level + 1) covers the largest group
-            k_g1_group_sum<<<cdiv(n, BLS_BLOCK), BLS_BLOCK, 0, s>>>(ga, level, span);
-            launches++;
-            level++;
-            span *= GROUP_CHUNK;
-        } while (span < b->max_group);
-        plan[LHB200_PLAN_GROUP_SUM] = LHB200_K_G1_GROUP_SUM;
-        plan[LHB200_PLAN_GROUP_SUM_LEVELS] = level;
-        m_p = b->d_gp;
-        m_st = m_pk_st = b->d_gskip;
-    }
-    static const int miller_coop = [] { const char* e = getenv("LHB_MILLER_COOP"); return e ? atoi(e) : 1; }();
-    const Fp12* cur = b->d_f;
-    uint32_t n_tail = 0;
-    const Fp12* f_last = b->d_flast;
-    if (miller_coop) {
-        // Cooperative shared-memory Miller loop over the ng pairs AND the (-g1, sum r sig) pair (bls/miller_coop.cuh):
-        // one block of 8 independent warps per SM, 30 working lanes per warp, every lane runs `rounds` sets, six lanes
-        // share one accumulator.  Small batches spread over more, emptier warps (latency), large ones fill 8 x n_sm.
-        static const bool attr_ok = [] {
-            return cudaFuncSetAttribute(mc::k_miller_coop, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)mc::mc_smem_bytes()) == cudaSuccess;
-        }();
-        if (!attr_ok) { set_error("k_miller_coop: cannot reserve %zu B of shared memory", mc::mc_smem_bytes()); return LHB200_ECUDA; }
-        constexpr uint32_t LU = 30;
-        const uint32_t n_total = ng + 1;
-        const uint32_t max_warps = (uint32_t)n_sm * mc::MC_WARPS;
-        // Latency mode (bls/miller_warp.cuh): while every pair can have a warp of its own in one wave, a whole warp runs
-        // one Miller loop at Fp granularity, far shorter than a lane-per-set loop.  Four warps per block
-        // (one per scheduler) up to 256 pairs, eight above; <= 64 block products go straight to k_final_coop.
-        static const int miller_warp_env = [] { const char* e = getenv("LHB_MILLER_WARP"); return e ? atoi(e) : 1; }();
-        if (miller_warp_env && n_total <= max_warps) {
-            static const bool mw_attr_ok = [] {
-                return cudaFuncSetAttribute(mw::k_miller_warp, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                            (int)mw::smem_bytes(mc::MC_WARPS)) == cudaSuccess;
-            }();
-            if (!mw_attr_ok) { set_error("k_miller_warp: cannot reserve shared memory"); return LHB200_ECUDA; }
-            const uint32_t wpb = n_total <= 4 * COOP_TAIL ? 4 : mc::MC_WARPS;
-            const uint32_t mgrid = cdiv(n_total, wpb);
-            LHB_CUDA(cudaStreamWaitEvent(s, b->e_join, 0));   // sum r sig (and -g1) ready
-            LHB_CUDA(cudaEventRecord(b->e_k0, s));
-            mw::k_miller_warp<<<mgrid, 32 * wpb, mw::smem_bytes((int)wpb), s>>>(m_p, b->d_h, m_st, m_pk_st,
-                                                                                ng, b->d_sig_sum, b->d_neg_g1, b->d_f);
-            plan[LHB200_PLAN_MILLER] = LHB200_K_MILLER_WARP;
-            plan[LHB200_PLAN_MILLER_WPB] = wpb;
-            plan[LHB200_PLAN_MILLER_SPW] = 1;
-            plan[LHB200_PLAN_MILLER_GRID] = mgrid;
-            LHB_CUDA(cudaEventRecord(b->e_k1, s));
-            launches += 1;
-            uint32_t m = mgrid;
-            int flip = 0;
-            while (m > COOP_TAIL) {
-                const uint32_t mo = cdiv(m, REDUCE_CHUNK);
-                k_fp12_reduce<<<cdiv(mo, BLS_BLOCK), BLS_BLOCK, 0, s>>>(cur, m, REDUCE_CHUNK, b->d_f_tmp[flip]);
-                launches++;
-                plan[LHB200_PLAN_FP12_REDUCE_LEVELS]++;
-                cur = b->d_f_tmp[flip];
-                flip ^= 1;
-                m = mo;
-            }
-            n_tail = m;
-            f_last = nullptr;
-        } else {
-        uint32_t spw = cdiv(n_total, max_warps);             // sets per warp
-        spw = cdiv(spw, LU) * LU;                            // whole rounds
-        uint32_t n_warps, mgrid;
-        // Batches below one full round per warp.  A warp's five groups take one set each at no extra latency (SIMT), and
-        // every further set of a group adds one serial sparse product per iteration (81 multiply units for a 1-set
-        // group, 141 for a full one).  Small batches therefore use at least five sets per warp, at most 256 warps, four
-        // per block (one per scheduler): <= 64 block products, which k_final_coop folds itself (no k_fp12_reduce level,
-        // a level of single-thread latency).  Above that: as few sets per warp as the 8 x n_sm warp budget allows.
-        constexpr uint32_t FEW_WARPS = 4 * COOP_TAIL;
-        if (n_total <= FEW_WARPS * LU) {
-            spw = std::min<uint32_t>(LU, std::max<uint32_t>(5, cdiv(cdiv(n_total, FEW_WARPS), 5) * 5));
-            n_warps = cdiv(n_total, spw);
-            mgrid = cdiv(n_warps, 4);
-        } else {
-            if (n_total <= max_warps * LU) spw = std::max<uint32_t>(1, cdiv(n_total, max_warps));
-            n_warps = cdiv(n_total, spw);
-            // warps are dealt round-robin to blocks (gw = warp_in_block * grid + block): few warps spread over all SMs
-            mgrid = std::max<uint32_t>(std::min<uint32_t>((uint32_t)n_sm, n_warps), cdiv(n_warps, mc::MC_WARPS));
-        }
-        const uint32_t rounds_cap = cdiv(spw, LU);
-        const size_t need = (size_t)mgrid * mc::MC_WARPS * rounds_cap * 2 * mc::TWORDS * 32;
-        if (need > b->mc_scratch_words) {
-            LHB_CUDA(cudaStreamSynchronize(s));
-            if (b->d_mc_scratch) cudaFree(b->d_mc_scratch);
-            b->d_mc_scratch = nullptr;
-            LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&b->d_mc_scratch), need * 4));
-            b->mc_scratch_words = need;
-        }
-        LHB_CUDA(cudaStreamWaitEvent(s, b->e_join, 0));   // sum r sig (and -g1) ready
-        LHB_CUDA(cudaEventRecord(b->e_k0, s));
-        mc::k_miller_coop<<<mgrid, 32 * mc::MC_WARPS, mc::mc_smem_bytes(), s>>>(m_p, b->d_h, m_st, m_pk_st,
-                                                                                ng, b->d_sig_sum, b->d_neg_g1, spw,
-                                                                                b->d_mc_scratch, b->d_f);
-        plan[LHB200_PLAN_MILLER] = LHB200_K_MILLER_COOP;
-        plan[LHB200_PLAN_MILLER_WPB] = mc::MC_WARPS;
-        plan[LHB200_PLAN_MILLER_SPW] = spw;
-        plan[LHB200_PLAN_MILLER_GRID] = mgrid;
-        plan[LHB200_PLAN_MILLER_ROUNDS_CAP] = rounds_cap;
-        plan[LHB200_PLAN_MILLER_FEW_WARPS] = n_total <= FEW_WARPS * LU;
-        LHB_CUDA(cudaEventRecord(b->e_k1, s));
-        launches += 1;
-        uint32_t m = mgrid;   // the kernel multiplies groups and warps together: one value per block
-        int flip = 0;
-        // k_final_warp folds the block products itself (8 warps share the products): no single-thread product level
-        static const int fw_env = [] { const char* e = getenv("LHB_FINAL_WARP"); return e ? atoi(e) : 1; }();
-        const uint32_t tail_max = fw_env ? FINAL_WARP_TAIL : COOP_TAIL;
-        while (m > tail_max) {
-            const uint32_t mo = cdiv(m, REDUCE_CHUNK);
-            k_fp12_reduce<<<cdiv(mo, BLS_BLOCK), BLS_BLOCK, 0, s>>>(cur, m, REDUCE_CHUNK, b->d_f_tmp[flip]);
-            launches++;
-            plan[LHB200_PLAN_FP12_REDUCE_LEVELS]++;
-            cur = b->d_f_tmp[flip];
-            flip ^= 1;
-            m = mo;
-        }
-        n_tail = m;
-        f_last = nullptr;
-        }
-    } else {
-    LHB_CUDA(cudaEventRecord(b->e_k0, s));
-    // Sets per thread: k = ceil(n / resident threads) (<= MILLER_KMAX) share their Fp12 squarings in one thread, so a
-    // 100 k batch is ONE wave of 3-set groups instead of three waves of single Miller loops.  LHB_MILLER_K overrides.
-    static const int miller_occ = [] {
-        int v = 4;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_miller_multi, MILLER_BLOCK, 0);
-        return std::max(v, 1);
-    }();
-    static const int miller_k_env = [] { const char* e = getenv("LHB_MILLER_K"); return e ? atoi(e) : 0; }();
-    const uint32_t resident = (uint32_t)(n_sm * miller_occ) * MILLER_BLOCK;
-    uint32_t mk = miller_k_env > 0 ? (uint32_t)miller_k_env : cdiv(ng, resident);
-    mk = std::min<uint32_t>(std::max<uint32_t>(mk, 1), MILLER_KMAX);
-    const uint32_t n_groups = cdiv(ng, mk);
-    const uint32_t mgrid = std::min<uint32_t>(cdiv(n_groups, MILLER_BLOCK), (uint32_t)(n_sm * miller_occ));
-    k_miller_multi<<<mgrid, MILLER_BLOCK, 0, s>>>(m_p, b->d_h, m_st, m_pk_st, ng, mk, n_groups, b->d_f);
-    plan[LHB200_PLAN_MILLER] = LHB200_K_MILLER_MULTI;
-    plan[LHB200_PLAN_MILLER_SPW] = mk;
-    plan[LHB200_PLAN_MILLER_GRID] = mgrid;
-    LHB_CUDA(cudaEventRecord(b->e_k1, s));
-    launches += 1;
-    {
-        uint32_t m = n_groups;
-        int flip = 0;
-        while (m > COOP_TAIL) {   // the last <= 16 values are folded cooperatively inside k_final_coop
-            const uint32_t mo = cdiv(m, REDUCE_CHUNK);
-            k_fp12_reduce<<<cdiv(mo, BLS_BLOCK), BLS_BLOCK, 0, s>>>(cur, m, REDUCE_CHUNK, b->d_f_tmp[flip]);
-            launches++;
-            plan[LHB200_PLAN_FP12_REDUCE_LEVELS]++;
-            cur = b->d_f_tmp[flip];
-            flip ^= 1;
-            m = mo;
-        }
-        n_tail = m;
-    }
-    LHB_CUDA(cudaStreamWaitEvent(s, b->e_join, 0));
-    }
-    static const int final_warp_env = [] { const char* e = getenv("LHB_FINAL_WARP"); return e ? atoi(e) : 1; }();
-    if (final_warp_env && !f_last) {   // phase-interpreter tail (bls/fe_warp.cuh)
-        static const bool fe_attr_ok = [] {
-            return cudaFuncSetAttribute(fe::k_final_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fe::smem_bytes()) == cudaSuccess;
-        }();
-        if (!fe_attr_ok) { set_error("k_final_warp: cannot reserve shared memory"); return LHB200_ECUDA; }
-        fe::k_final_warp<<<1, 32 * fe::FE_WARPS, fe::smem_bytes(), s>>>(cur, n_tail, b->d_fail, b->d_ok, b->d_gt);
-        plan[LHB200_PLAN_FINAL] = LHB200_K_FINAL_WARP;
-    } else {
-        k_final_coop<<<1, COOP_THREADS, sizeof(CoopFinalSmem), s>>>(cur, n_tail, f_last, b->d_fail, b->d_ok, b->d_gt);
-        plan[LHB200_PLAN_FINAL] = LHB200_K_FINAL_COOP;
-    }
-    plan[LHB200_PLAN_N_TAIL] = n_tail;
+    if (b->n_groups) launch_group_sum(b, p, s, launches);
+    if (int32_t rc = launch_miller(b, p, s, launches, &prod)) return rc;
+    const uint32_t n_tail = p.w[LHB200_PLAN_N_TAIL];
+    if (p.w[LHB200_PLAN_FINAL] == LHB200_K_FINAL_WARP)   // phase-interpreter tail (bls/fe_warp.cuh)
+        fe::k_final_warp<<<1, 32 * fe::FE_WARPS, fe::smem_bytes(), s>>>(prod, n_tail, b->d_fail, b->d_ok, b->d_gt);
+    else
+        k_final_coop<<<1, COOP_THREADS, sizeof(CoopFinalSmem), s>>>(prod, n_tail, p.w[LHB200_PLAN_LAST_MILLER] ? b->d_flast : nullptr,
+                                                                    b->d_fail, b->d_ok, b->d_gt);
     launches++;
     LHB_CUDA(cudaGetLastError());
     count_launch(launches);
@@ -1250,8 +1235,8 @@ int32_t lhb200_bls_batch_plan(const lhb200_bls_batch* b, uint32_t* out, uint32_t
     return LHB200_OK;
 }
 
-// Device time (ms, CUDA events on the launching stream) of the dominant kernel k_miller_multi in the last completed
-// enqueue; negative if unavailable.  Call after the stream has been synchronised.
+// Device time (ms, CUDA events on the launching stream) of the Miller kernel that ran in the last completed enqueue
+// (k_miller_warp, k_miller_coop or k_miller_multi); negative if unavailable.  Call after the stream has been synchronised.
 float lhb200_bls_batch_dominant_kernel_ms(const lhb200_bls_batch* b) {
     float ms = -1.f;
     if (!b || cudaEventElapsedTime(&ms, b->e_k0, b->e_k1) != cudaSuccess) { cudaGetLastError(); return -1.f; }
@@ -1426,20 +1411,12 @@ int32_t lhb200_g2_aggregate(const uint8_t* sigs96, uint32_t n, uint8_t out96[96]
     LHB_CUDA(cudaMemcpyAsync(d, sigs96, (size_t)n * 96, cudaMemcpyHostToDevice, c.stream));
     LHB_CUDA(cudaMemsetAsync(d_bad, 0, 4, c.stream));
     k_g2_load_points<<<cdiv(n, BLS_BLOCK), BLS_BLOCK, 0, c.stream>>>(d, n, pts, d_bad);
-    uint64_t launches = 2;
-    const G2Jac* cur = pts;
-    uint32_t m = n;
-    int flip = 0;
-    while (m > 1) {
-        const uint32_t mo = cdiv(m, REDUCE_CHUNK);
-        k_g2_reduce<<<cdiv(mo, BLS_BLOCK), BLS_BLOCK, 0, c.stream>>>(cur, m, REDUCE_CHUNK, tmp[flip]);
-        launches++;
-        cur = tmp[flip];
-        flip ^= 1;
-        m = mo;
-    }
-    k_g2_store_point<<<1, 32, 0, c.stream>>>(cur, d_out);
-    count_launch(launches);
+    const uint32_t levels = tree_levels(n, REDUCE_CHUNK, 1);
+    const G2Jac* sum = reduce_tree<G2Jac>(pts, n, REDUCE_CHUNK, levels, tmp, [&](const G2Jac* in, uint32_t m, uint32_t mo, G2Jac* out) {
+        k_g2_reduce<<<cdiv(mo, BLS_BLOCK), BLS_BLOCK, 0, c.stream>>>(in, m, REDUCE_CHUNK, out);
+    });
+    k_g2_store_point<<<1, 32, 0, c.stream>>>(sum, d_out);
+    count_launch(2 + levels);
     LHB_CUDA(cudaGetLastError());
     uint8_t h[96];
     uint32_t bad = 0;
@@ -1470,20 +1447,12 @@ int32_t lhb200_g1_aggregate(const uint8_t* pks96, uint32_t n, uint8_t* out48, ui
     LHB_CUDA(cudaMemcpyAsync(d, pks96, (size_t)n * 96, cudaMemcpyHostToDevice, c.stream));
     LHB_CUDA(cudaMemsetAsync(d_bad, 0, 4, c.stream));
     k_g1_load_points<<<cdiv(n, BLS_BLOCK), BLS_BLOCK, 0, c.stream>>>(d, n, pts, nullptr, nullptr, d_bad);
-    uint64_t launches = 2;
-    const G1Jac* cur = pts;
-    uint32_t m = n;
-    int flip = 0;
-    while (m > 1) {
-        const uint32_t mo = cdiv(m, REDUCE_CHUNK);
-        k_g1_reduce<<<cdiv(mo, BLS_BLOCK), BLS_BLOCK, 0, c.stream>>>(cur, m, REDUCE_CHUNK, tmp[flip]);
-        launches++;
-        cur = tmp[flip];
-        flip ^= 1;
-        m = mo;
-    }
-    k_g1_store_point<<<1, 32, 0, c.stream>>>(cur, d_out, d_out + 64);
-    count_launch(launches);
+    const uint32_t levels = tree_levels(n, REDUCE_CHUNK, 1);
+    const G1Jac* sum = reduce_tree<G1Jac>(pts, n, REDUCE_CHUNK, levels, tmp, [&](const G1Jac* in, uint32_t m, uint32_t mo, G1Jac* out) {
+        k_g1_reduce<<<cdiv(mo, BLS_BLOCK), BLS_BLOCK, 0, c.stream>>>(in, m, REDUCE_CHUNK, out);
+    });
+    k_g1_store_point<<<1, 32, 0, c.stream>>>(sum, d_out, d_out + 64);
+    count_launch(2 + levels);
     LHB_CUDA(cudaGetLastError());
     uint8_t h[160];
     uint32_t bad = 0;

@@ -1,7 +1,8 @@
 """Runs the batches stored in .npz files through the batch verifier and prints one JSON line per file: verdict, per-set
-statuses, GT bytes (the final-exponentiated product) and the kernel plan the library chose.  The kernel-selection
-switches (LHB_G2_WARP, LHB_MILLER_WARP, LHB_MILLER_COOP, LHB_FINAL_WARP, LHB_PK_TMA) are read once per process, so
-tests/test_bls_regimes_gpu.py runs this script once per switch set and compares the output with the oracle.
+statuses, GT bytes (the final-exponentiated product), the kernel plan the library chose and its kernel launches.  The
+kernel-selection switches (LHB_G2_WARP, LHB_MILLER_WARP, LHB_MILLER_COOP, LHB_FINAL_WARP, LHB_PK_TMA) are read at
+lhb200_init, so tests/test_bls_regimes_gpu.py runs this script once per switch set and compares the output with the
+oracle.
 
 A file holds sigs, msgs, pks (uint8), offsets (uint32), rands (uint64) and optionally indices (uint32) + table
 (uint8[T, 96]): with indices the keys come from a device pubkey table (upload_indexed), without them from the explicit
@@ -37,7 +38,7 @@ def run(path):
         b.enqueue()
         ok, st = b.result(want_status=True)
         return {"file": os.path.basename(path), "n": n, "ok": bool(ok), "status": bytes(st).hex(),
-                "gt": b.gt_bytes().hex() if not st.any() else None, "plan": b.plan()}
+                "gt": b.gt_bytes().hex() if not st.any() else None, "plan": b.plan(), "launches": b.launches}
     finally:
         b.destroy()
         if table is not None:
