@@ -200,10 +200,30 @@ LHB200_API int32_t lhb200_shuffle_list(const uint64_t* input, uint64_t n, uint8_
  * n_sets == 1 case.
  * Sets that share a message (every unaggregated attestation of a committee, every sync-committee message of a slot)
  * are grouped: when at least one set in eight repeats a message, hash-to-G2 and the Miller loop run once per distinct
- * message over the sum of the group's r_i apk_i.  The verdict, the statuses and the final-exponentiated product are the same as without. */
+ * message over the sum of the group's r_i apk_i.  The verdict, the statuses and the final-exponentiated product are the same as without.
+ * Concurrent calls of at most 64 sets are coalesced: a call that finds a free slot (at most sixteen passes run at
+ * once) runs alone, as above.  A call that arrives while every slot is taken validates its arguments in its own thread
+ * (an argument error is returned to that caller alone, as above), draws its own scalars when rands is NULL, and waits.
+ * When a slot frees, the first waiting call takes the waiting calls that fit one segmented pass (see
+ * lhb200_verify_signature_set_batches) and verifies them in one device pass, each as its own batch with its own
+ * scalars, so its verdict and statuses are the ones it would get alone.  A CUDA error (or an allocation failure) in a
+ * shared pass is returned to every call of that pass.  The call blocks until its own result is written. */
 LHB200_API int32_t lhb200_verify_signature_sets(const uint8_t* sigs, const uint8_t* msgs, const uint8_t* pks,
                                                 const uint32_t* pk_offsets, const uint64_t* rands, uint32_t n_sets,
                                                 uint8_t* ok, uint8_t* set_status);
+/* n_batches independent verify_signature_sets calls in one: batch k is sets [batch_offsets[k], batch_offsets[k + 1])
+ * of the SoA buffers above (pk_offsets over all n_sets sets), and ok[k] is exactly what lhb200_verify_signature_sets
+ * gives for batch k alone with the same scalars; an empty batch gives 0 (blst.rs:42-44).  set_status (optional,
+ * n_sets bytes) as above.  Consecutive batches are packed into segmented passes: one device pass runs the per-set
+ * stages over all of a pass's sets, then per batch one sum of r_i sig_i, one pair (-g1, sum) and one final
+ * exponentiation, so no batch's verdict depends on another's sets.  A pass holds batches while their sets plus their
+ * count stay within 8 x the SM count (the warps of one wave of the one-warp-per-pairing Miller kernel); a batch too
+ * large for a pass alone runs through lhb200_verify_signature_sets.  n_batches == 0 does nothing.  Non-monotone or
+ * inconsistent offsets, a zero scalar or a null pointer -> LHB200_EINVAL ("verify_signature_set_batches: <reason>"). */
+LHB200_API int32_t lhb200_verify_signature_set_batches(const uint8_t* sigs, const uint8_t* msgs, const uint8_t* pks,
+                                                       const uint32_t* pk_offsets, const uint64_t* rands,
+                                                       uint32_t n_sets, const uint32_t* batch_offsets,
+                                                       uint32_t n_batches, uint8_t* ok, uint8_t* set_status);
 
 /* Staged form of the same call (what bench.py times): create once, upload or point at device-resident inputs,
  * enqueue on a stream, read the verdict.  The three host uploads (lhb200_bls_batch_upload, _upload_async,
@@ -231,6 +251,18 @@ LHB200_API int32_t lhb200_bls_batch_upload_async(lhb200_bls_batch* b, const uint
                                                  uint32_t n_sets, void* stream);
 LHB200_API int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream);
 LHB200_API int32_t lhb200_bls_batch_result(lhb200_bls_batch* b, void* stream, uint8_t* ok, uint8_t* set_status);
+/* Segmented pass, staged form (lhb200_verify_signature_set_batches splits its input into such passes): the sets of
+ * the next upload are n_batches independent batches, batch k = sets [batch_offsets[k], batch_offsets[k + 1]).  Call
+ * before the upload (the upload groups messages within each batch only; any earlier upload on `b` is dropped); the
+ * next verify_enqueue checks every batch on its own and consumes the segments.  Batches must be non-empty, offsets
+ * start at 0 and increase, and sets + n_batches must fit one pass (8 x the SM count) -> else LHB200_EINVAL.  The
+ * upload must then carry batch_offsets[n_batches] sets.
+ * lhb200_bls_batch_segment_result: ok[k] per batch (n_batches bytes) and, optionally, the per-set statuses.
+ * lhb200_bls_batch_segment_gt: test hook, batch k's final-exponentiated product in the format of lhb200_bls_batch_gt
+ * (zeros for a batch with a failed set). */
+LHB200_API int32_t lhb200_bls_batch_set_segments(lhb200_bls_batch* b, const uint32_t* batch_offsets, uint32_t n_batches);
+LHB200_API int32_t lhb200_bls_batch_segment_result(lhb200_bls_batch* b, void* stream, uint8_t* ok, uint8_t* set_status);
+LHB200_API int32_t lhb200_bls_batch_segment_gt(lhb200_bls_batch* b, uint32_t k, uint8_t out576[576]);
 /* Device-resident validator pubkey table — the mirror of ValidatorPubkeyCache
  * (beacon_node/beacon_chain/src/validator_pubkey_cache.rs:20-25,138-140; same 96-byte key format it persists, :195-199).
  * Keys are decoded to Montgomery form once at import; SignatureSets then carry u32 validator indices
@@ -250,7 +282,7 @@ LHB200_API int32_t lhb200_bls_batch_gt(lhb200_bls_batch* b, uint8_t out576[576])
 /* Test hook: which kernels the last lhb200_bls_batch_verify_enqueue on `b` launched, so a test can tell which path a
  * batch size exercised.  Writes min(n_words, LHB200_PLAN_WORDS) words, indexed by LHB200_PLAN_*; the stage words
  * hold LHB200_K_* ids, 0 where the stage did not run (the sum tree of a single set). */
-#define LHB200_PLAN_WORDS 23
+#define LHB200_PLAN_WORDS 24
 #define LHB200_PLAN_N_SETS 0
 #define LHB200_PLAN_N_SM 1                    /* SM count the launch shapes were derived from */
 #define LHB200_PLAN_SIG 2
@@ -274,6 +306,10 @@ LHB200_API int32_t lhb200_bls_batch_gt(lhb200_bls_batch* b, uint8_t out576[576])
 #define LHB200_PLAN_GROUPS 20                 /* distinct messages the sets were grouped into; 0 = not grouped */
 #define LHB200_PLAN_GROUP_SUM 21              /* the per-message key sum (grouped batches only) */
 #define LHB200_PLAN_GROUP_SUM_LEVELS 22       /* levels of its segmented tree */
+#define LHB200_PLAN_SEGMENTS 23               /* independent batches of a segmented pass; 0 = one batch.  The sum word
+                                               * then names the per-segment signature sum, the Miller word the
+                                               * one-value-per-warp variant of k_miller_warp, the final word the
+                                               * per-segment tail */
 #define LHB200_K_SIG_PREPARE 1
 #define LHB200_K_SIG_PREPARE_WARP 2
 #define LHB200_K_G2_REDUCE 3
@@ -291,6 +327,8 @@ LHB200_API int32_t lhb200_bls_batch_gt(lhb200_bls_batch* b, uint8_t out576[576])
 #define LHB200_K_FINAL_COOP 15
 #define LHB200_K_FINAL_WARP 16
 #define LHB200_K_G1_GROUP_SUM 17
+#define LHB200_K_G2_SEGMENT_SUM 18
+#define LHB200_K_FINAL_SEGMENTS 19
 LHB200_API int32_t lhb200_bls_batch_plan(const lhb200_bls_batch* b, uint32_t* out, uint32_t n_words);
 LHB200_API uint64_t lhb200_bls_batch_launches(const lhb200_bls_batch* b);
 /* Device time (ms) of the Miller kernel that ran (k_miller_warp, k_miller_coop or k_miller_multi) in the last completed

@@ -136,3 +136,7 @@ _sig("lhb200_bls_batch_allreduce_verdict", C.c_int32, vp, vp)
 _sig("lhb200_state_root_sharded", C.c_int32, vp, vp)
 _sig("lhb200_beacon_state_root", C.c_int32, vp, C.c_uint64, C.c_int32, vp, vp)
 _sig("lhb200_state_stage", C.c_int32, vp, C.c_uint64, C.c_int32, C.POINTER(vp))
+_sig("lhb200_verify_signature_set_batches", C.c_int32, vp, vp, vp, vp, vp, C.c_uint32, vp, C.c_uint32, vp, vp)
+_sig("lhb200_bls_batch_set_segments", C.c_int32, vp, vp, C.c_uint32)
+_sig("lhb200_bls_batch_segment_result", C.c_int32, vp, vp, vp, vp)
+_sig("lhb200_bls_batch_segment_gt", C.c_int32, vp, C.c_uint32, vp)

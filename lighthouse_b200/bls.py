@@ -344,6 +344,26 @@ def verify_signature_sets_raw(sigs, msgs, pks, offsets, rands=None, want_status=
     return (res, st[:n]) if want_status else res
 
 
+def verify_signature_set_batches(sigs, msgs, pks, offsets, batch_offsets, rands=None, want_status=False):
+    """lhb200_verify_signature_set_batches: independent verify_signature_sets calls in one (batch k = sets
+    batch_offsets[k] .. batch_offsets[k + 1] of the flattened buffers) -> bool array of verdicts (and the statuses)."""
+    n = len(offsets) - 1
+    bo = np.ascontiguousarray(batch_offsets, dtype=np.uint32)
+    k = len(bo) - 1
+    ok = np.zeros(max(k, 1), dtype=np.uint8)
+    st = np.zeros(max(n, 1), dtype=np.uint8)
+    offs = np.ascontiguousarray(offsets, dtype=np.uint32)
+    r = None if rands is None else np.ascontiguousarray(rands, dtype=np.uint64)
+    ps, k1 = buf(sigs if len(sigs) else b"\0")
+    pm, k2 = buf(msgs if len(msgs) else b"\0")
+    pp, k3 = buf(pks if len(pks) else b"\0")
+    check(lib.lhb200_verify_signature_set_batches(ps, pm, pp, offs.ctypes.data, None if r is None else r.ctypes.data, n,
+                                                  bo.ctypes.data, k, ok.ctypes.data, st.ctypes.data),
+          "lhb200_verify_signature_set_batches")
+    res = ok[:k] == 1
+    return (res, st[:n]) if want_status else res
+
+
 def verify_signature_sets(sets, rands=None) -> bool:
     """bls::verify_signature_sets (impls/blst.rs:37-119).  Empty iterator -> False."""
     sets = list(sets)
@@ -405,12 +425,12 @@ class PubkeyTable:
 PLAN_FIELDS = ("n_sets", "n_sm", "sig", "sum", "sum_levels", "hash", "key", "key_chunks", "miller", "miller_wpb",
                "miller_spw", "miller_grid", "miller_rounds_cap", "miller_few_warps", "fp12_reduce_levels", "n_tail",
                "final", "lane_grid", "lane_sets_per_thread", "last_miller", "groups", "group_sum",
-               "group_sum_levels")
+               "group_sum_levels", "segments")
 _PLAN_KERNEL_FIELDS = ("sig", "sum", "hash", "key", "miller", "final", "group_sum")
 PLAN_KERNELS = ("", "k_sig_prepare", "k_sig_prepare_warp", "k_g2_reduce", "k_g2_sum_warp", "k_hash_to_g2",
                 "k_hash_to_g2_pair", "k_hash_to_g2_warp", "k_pk_aggregate", "k_pk_partial+k_pk_combine",
                 "k_pk_aggregate_tma", "k_pk_aggregate_indexed", "k_miller_multi", "k_miller_coop", "k_miller_warp",
-                "k_final_coop", "k_final_warp", "k_g1_group_sum")
+                "k_final_coop", "k_final_warp", "k_g1_group_sum", "k_g2_segment_sum", "k_final_segments")
 
 
 class Batch:
@@ -420,6 +440,7 @@ class Batch:
         self._h = C.c_void_p()
         check(lib.lhb200_bls_batch_create(max_sets, max_keys, C.byref(self._h)), "lhb200_bls_batch_create")
         self.n = 0
+        self.n_seg = 0
 
     def upload(self, sigs, msgs, pks, offsets, rands=None):
         offs = np.ascontiguousarray(offsets, dtype=np.uint32)
@@ -465,6 +486,26 @@ class Batch:
         check(lib.lhb200_bls_batch_result(self._h, stream, ok, st.ctypes.data if want_status else None),
               "lhb200_bls_batch_result")
         return (ok.raw[0] == 1, st[: self.n]) if want_status else ok.raw[0] == 1
+
+    def set_segments(self, batch_offsets):
+        """lhb200_bls_batch_set_segments: the next upload carries independent batches (call before the upload)."""
+        bo = np.ascontiguousarray(batch_offsets, dtype=np.uint32)
+        self.n_seg = len(bo) - 1
+        check(lib.lhb200_bls_batch_set_segments(self._h, bo.ctypes.data, self.n_seg), "lhb200_bls_batch_set_segments")
+
+    def segment_result(self, stream=None, want_status=False):
+        """Verdicts of the last segmented enqueue (bool array, one per segment), and the per-set statuses."""
+        ok = np.zeros(max(self.n_seg, 1), dtype=np.uint8)
+        st = np.zeros(max(self.n, 1), dtype=np.uint8)
+        check(lib.lhb200_bls_batch_segment_result(self._h, stream, ok.ctypes.data, st.ctypes.data if want_status else None),
+              "lhb200_bls_batch_segment_result")
+        res = ok[: self.n_seg] == 1
+        return (res, st[: self.n]) if want_status else res
+
+    def segment_gt(self, k):
+        out = C.create_string_buffer(576)
+        check(lib.lhb200_bls_batch_segment_gt(self._h, k, out), "lhb200_bls_batch_segment_gt")
+        return out.raw
 
     def gt_bytes(self):
         out = C.create_string_buffer(576)

@@ -79,6 +79,36 @@ __global__ void __launch_bounds__(64) k_g1_group_sum(GroupSumArgs a, uint32_t le
     const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p < a.n) group_sum_position(a, level, span, p);
 }
+
+// Segmented passes (several batch checks in one launch): the sum of r_i sig_i over each segment of sets
+// [seg_off[k], seg_off[k + 1]), the same tree as above on contiguous runs.  Level l combines runs of GROUP_CHUNK values at
+// stride GROUP_CHUNK^l in place in `sig_r` (the signature kernels' r_i sig_i, infinity for a failed set); the level whose
+// span covers segment k writes its sum to out[k].  Segments are not empty.
+__global__ void __launch_bounds__(64) k_g2_segment_sum(G2Jac* __restrict__ sig_r, const uint32_t* __restrict__ seg_off,
+                                                       uint32_t n, uint32_t n_seg, uint32_t level, uint64_t span,
+                                                       G2Jac* __restrict__ out) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n) return;
+    uint32_t lo = 0, hi = n_seg;   // the segment of p: seg_off[lo] <= p < seg_off[lo + 1]
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (seg_off[mid] <= p) lo = mid; else hi = mid;
+    }
+    const uint32_t start = seg_off[lo], end = seg_off[lo + 1], size = end - start;
+    const uint64_t out_span = span * GROUP_CHUNK;
+    if ((p - start) % out_span != 0) return;
+    if (level > 0 && size <= span) return;   // finished at an earlier level
+    G2Jac acc;
+    jac_set_inf(acc);
+    for (uint32_t j = 0; j < GROUP_CHUNK; j++) {
+        const uint64_t q = p + j * span;
+        if (q >= end) break;
+        G2Jac x = sig_r[q];
+        jac_add(acc, acc, x);
+    }
+    if (size > out_span) sig_r[p] = acc;
+    else out[lo] = acc;
+}
 #endif
 
 }  // namespace bls

@@ -175,25 +175,39 @@ LHB_HD LHB_INLINE void set_one_words(uint32_t* R, int word) {   // word < 24 * S
 
 constexpr size_t smem_bytes(int warps) { return ((size_t)warps * REGION_WORDS + table_words(MW_N_MUL, MW_N_LIN, MW_N_PHASES)) * 4; }
 #if !defined(LHB_HOSTSIM)
-// One warp per pair (P_i, H_i), i < n, plus the pair (extra_p, extra_q) = (-g1, sum r sig) as pair n.  Invalid sets
-// (status or pk_status != 0, H at infinity) contribute f = 1, like k_miller_coop.  The warps of a block multiply their values
-// (dense section) and the block writes ONE Fp12.  Dynamic shared memory: smem_bytes(warps_per_block).
-__global__ void __launch_bounds__(256, 1) k_miller_warp(const G1Proj3* __restrict__ P, const G2Jac* __restrict__ H,
-                                                        const uint8_t* __restrict__ status,
-                                                        const uint8_t* __restrict__ pk_status, uint32_t n,
-                                                        const G2Jac* __restrict__ extra_q, const G1Proj3* __restrict__ extra_p,
-                                                        Fp12* __restrict__ out_f) {
+// w-basis coefficient k -> tower: 0 c0.c0, 1 c1.c0, 2 c0.c1, 3 c1.c1, 4 c0.c2, 5 c1.c2 (coop.cuh)
+__device__ __forceinline__ void store_f(Fp12* out, const uint32_t* R, int lane) {
+    uint32_t* o = reinterpret_cast<uint32_t*>(out);
+    for (int w = lane; w < 12 * NL; w += 32) {
+        const int fp2_idx = w / (2 * NL), comp = (w / NL) & 1, limb = w % NL;   // tower order: c0.c0 c0.c1 c0.c2 c1.c0 c1.c1 c1.c2
+        const int k = fp2_idx < 3 ? 2 * fp2_idx : 2 * (fp2_idx - 3) + 1;
+        o[w] = R[(MW_S_F0_0 + 4 * k + comp) * SL + limb];
+    }
+}
+
+// The body of both Miller kernels below.  Pairs i < n are (P_i, H_i); pairs n .. n + n_extra - 1 are (extra_p,
+// extra_q[i - n]).  PER_WARP = false: the block multiplies its warps' values and writes one Fp12 (n_extra <= 1);
+// PER_WARP = true: every warp writes its own pair's value to out_f[pair], so no product mixes two pairs.
+template <bool PER_WARP>
+__device__ __forceinline__ void miller_warp_body(const G1Proj3* __restrict__ P, const G2Jac* __restrict__ H,
+                                                 const uint8_t* __restrict__ status, const uint8_t* __restrict__ pk_status,
+                                                 uint32_t n, const G2Jac* __restrict__ extra_q, uint32_t n_extra,
+                                                 const G1Proj3* __restrict__ extra_p, Fp12* __restrict__ out_f) {
     const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
     uint32_t* R = lhb_dyn_smem + (size_t)wib * REGION_WORDS;
     const Tables T = stage_tables(lhb_dyn_smem + (size_t)nw * REGION_WORDS, miller_tables(), MW_N_MUL, MW_N_LIN, MW_N_PHASES);
-    const uint32_t n_total = n + (extra_q ? 1u : 0u);
+    const uint32_t n_total = n + n_extra;
     const uint32_t set = blockIdx.x * nw + wib;
     for (int w = lane; w < 24 * SL; w += 32) set_one_words(R, w);
     bool active = set < n_total;
     const G2Jac* q = nullptr;
     const G1Proj3* p = nullptr;
     if (active) {
-        if (set >= n) { q = extra_q; p = extra_p; }
+        if (set >= n) {
+            if constexpr (PER_WARP) q = extra_q + (set - n);
+            else q = extra_q;
+            p = extra_p;
+        }
         else { q = H + set; p = P + set; active = (status[set] | pk_status[set]) == 0; }
         if (active) active = !jac_is_inf(*q);
     }
@@ -216,26 +230,49 @@ __global__ void __launch_bounds__(256, 1) k_miller_warp(const G1Proj3* __restric
         }
         MW_RUN(R, lane, CONJ);
     }
-    // product over the block's warps
-    for (int stride = 1; stride < nw; stride *= 2) {
-        __syncthreads();
-        if (wib % (2 * stride) == 0 && wib + stride < nw) {
-            const uint32_t* O = R + (size_t)stride * REGION_WORDS;
-            for (int w = lane; w < 24 * SL; w += 32) R[MW_S_G0_0 * SL + w] = O[MW_S_F0_0 * SL + w];
+    if constexpr (PER_WARP) {
+        if (set < n_total) {
             __syncwarp();
-            MW_RUN(R, lane, DENSE);
+            store_f(out_f + set, R, lane);
+        }
+    } else {
+        // product over the block's warps
+        for (int stride = 1; stride < nw; stride *= 2) {
+            __syncthreads();
+            if (wib % (2 * stride) == 0 && wib + stride < nw) {
+                const uint32_t* O = R + (size_t)stride * REGION_WORDS;
+                for (int w = lane; w < 24 * SL; w += 32) R[MW_S_G0_0 * SL + w] = O[MW_S_F0_0 * SL + w];
+                __syncwarp();
+                MW_RUN(R, lane, DENSE);
+            }
+        }
+        if (wib == 0) {
+            __syncwarp();
+            store_f(out_f + blockIdx.x, R, lane);
         }
     }
-    if (wib == 0) {
-        __syncwarp();
-        // w-basis coefficient k -> tower: 0 c0.c0, 1 c1.c0, 2 c0.c1, 3 c1.c1, 4 c0.c2, 5 c1.c2 (coop.cuh)
-        uint32_t* o = reinterpret_cast<uint32_t*>(out_f + blockIdx.x);
-        for (int w = lane; w < 12 * NL; w += 32) {
-            const int fp2_idx = w / (2 * NL), comp = (w / NL) & 1, limb = w % NL;   // tower order: c0.c0 c0.c1 c0.c2 c1.c0 c1.c1 c1.c2
-            const int k = fp2_idx < 3 ? 2 * fp2_idx : 2 * (fp2_idx - 3) + 1;
-            o[w] = R[(MW_S_F0_0 + 4 * k + comp) * SL + limb];
-        }
-    }
+}
+
+// One warp per pair (P_i, H_i), i < n, plus the pair (extra_p, extra_q) = (-g1, sum r sig) as pair n.  Invalid sets
+// (status or pk_status != 0, H at infinity) contribute f = 1, like k_miller_coop.  The warps of a block multiply their values
+// (dense section) and the block writes ONE Fp12.  Dynamic shared memory: smem_bytes(warps_per_block).
+__global__ void __launch_bounds__(256, 1) k_miller_warp(const G1Proj3* __restrict__ P, const G2Jac* __restrict__ H,
+                                                        const uint8_t* __restrict__ status,
+                                                        const uint8_t* __restrict__ pk_status, uint32_t n,
+                                                        const G2Jac* __restrict__ extra_q, const G1Proj3* __restrict__ extra_p,
+                                                        Fp12* __restrict__ out_f) {
+    miller_warp_body<false>(P, H, status, pk_status, n, extra_q, extra_q ? 1u : 0u, extra_p, out_f);
+}
+
+// Segmented passes (several independent batch checks in one launch): pairs i < n as above, then one pair
+// (extra_p, extra_q[k]) = (-g1, sum of segment k's r sig) per segment k < n_seg.  Every warp writes the value of its own
+// pair to out_f[pair] (n + n_seg values): a block product would mix the verdicts of two segments.
+__global__ void __launch_bounds__(256, 1) k_miller_warp_segments(const G1Proj3* __restrict__ P, const G2Jac* __restrict__ H,
+                                                                 const uint8_t* __restrict__ status,
+                                                                 const uint8_t* __restrict__ pk_status, uint32_t n,
+                                                                 const G2Jac* __restrict__ extra_q, uint32_t n_seg,
+                                                                 const G1Proj3* __restrict__ extra_p, Fp12* __restrict__ out_f) {
+    miller_warp_body<true>(P, H, status, pk_status, n, extra_q, n_seg, extra_p, out_f);
 }
 #endif
 

@@ -16,6 +16,8 @@
 #include "bls/debug.cuh"
 #include <condition_variable>
 #include <thread>
+#include <deque>
+#include <string>
 #include "ctx.h"
 
 namespace lhb200 {
@@ -71,11 +73,12 @@ int32_t bls_init() {
         set_error("k_miller_coop: cannot reserve %zu B of shared memory", mc::mc_smem_bytes());
         return LHB200_ECUDA;
     }
-    if (!reserve_smem(mw::k_miller_warp, mw::smem_bytes(mc::MC_WARPS))) {
+    if (!reserve_smem(mw::k_miller_warp, mw::smem_bytes(mc::MC_WARPS)) ||
+        !reserve_smem(mw::k_miller_warp_segments, mw::smem_bytes(mc::MC_WARPS))) {
         set_error("k_miller_warp: cannot reserve shared memory");
         return LHB200_ECUDA;
     }
-    if (!reserve_smem(fe::k_final_warp, fe::smem_bytes())) {
+    if (!reserve_smem(fe::k_final_warp, fe::smem_bytes()) || !reserve_smem(fe::k_final_segments, fe::smem_bytes())) {
         set_error("k_final_warp: cannot reserve shared memory");
         return LHB200_ECUDA;
     }
@@ -252,6 +255,20 @@ struct lhb200_bls_batch {
     G1Proj3* d_gp = nullptr;                 // per-group sum of r_i apk_i
     uint8_t* d_gskip = nullptr;              // per group: nothing to pair (no contributing member, or the sum is O)
     G1Jac* d_gtmp = nullptr;                 // partial sums of the group-sum tree
+    // segmented pass (lhb200_bls_batch_set_segments): independent batch checks over contiguous runs of sets
+    uint32_t n_seg = 0;                      // segments of the next upload + verify_enqueue; 0: one batch
+    uint32_t n_seg_last = 0;                 // segments of the last verify_enqueue (segment_result, segment_gt)
+    uint32_t max_seg = 0;                    // sets of the largest segment
+    std::vector<uint32_t> seg_h;             // set offsets (n_seg + 1), then pair offsets (n_seg + 1): copied to d_seg_off
+    std::vector<uint32_t> seg_members, seg_goffsets;   // grouping within segments (the CSR d_members / d_goffsets get)
+    std::vector<uint8_t> seg_gmsgs;
+    // allocated on the first set_segments, sized for the largest pass (pass_limit())
+    uint32_t* d_seg_off = nullptr;           // set offsets, then pair offsets
+    G2Jac* d_seg_sig = nullptr;              // per segment: sum of r_i sig_i
+    Fp12* d_seg_f = nullptr;                 // Miller values: one per pair, then one per segment
+    Fp12* d_seg_gt = nullptr;
+    uint8_t* d_seg_ok = nullptr;
+    uint8_t* h_seg_ok = nullptr;             // pinned
 };
 
 static void batch_free(lhb200_bls_batch* b) {
@@ -260,10 +277,12 @@ static void batch_free(lhb200_bls_batch* b) {
     void* ptrs[] = {b->d_sigs, b->d_msgs, b->d_pks, b->d_offsets, b->d_rands, b->d_sigr, b->d_sig_tmp[0],
                     b->d_sig_tmp[1], b->d_p, b->d_h, b->d_f, b->d_f_tmp[0], b->d_f_tmp[1], b->d_flast, b->d_gt,
                     b->d_status, b->d_pk_status, b->d_fail, b->d_ok, b->d_mc_scratch, b->d_neg_g1, b->d_pk_part,
-                    b->d_pk_part_bad, b->d_members, b->d_goffsets, b->d_gmsgs, b->d_gp, b->d_gskip, b->d_gtmp};
+                    b->d_pk_part_bad, b->d_members, b->d_goffsets, b->d_gmsgs, b->d_gp, b->d_gskip, b->d_gtmp,
+                    b->d_seg_off, b->d_seg_sig, b->d_seg_f, b->d_seg_gt, b->d_seg_ok};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     if (b->h_res) cudaFreeHost(b->h_res);
+    if (b->h_seg_ok) cudaFreeHost(b->h_seg_ok);
     if (b->s_main) cudaStreamDestroy(b->s_main);
     if (b->s2) cudaStreamDestroy(b->s2);
     if (b->s3) cudaStreamDestroy(b->s3);
@@ -330,9 +349,14 @@ struct Plan {
     size_t mc_scratch_words = 0;   // k_miller_coop's parking area for T / Q between rounds
 };
 
-// The selection policy: kernels and shapes from the sizes alone.  n_groups: 0 = not grouped.
+// Sets plus segments of one segmented pass: every pair (and every segment's pair (-g1, sum r sig)) has a warp of its
+// own in one wave of k_miller_warp_segments (8 warps per block, one block per SM).
+static uint32_t pass_limit(const Config& c) { return c.n_sm * mc::MC_WARPS; }
+
+// The selection policy: kernels and shapes from the sizes alone.  n_groups: 0 = not grouped; n_seg: 0 = one batch, else
+// the segments of a segmented pass (max_seg sets in the largest).
 static Plan choose(const Config& c, uint32_t n, uint32_t n_groups, uint32_t max_group, bool indexed, uint32_t n_chunks,
-                   bool pks_aligned) {
+                   bool pks_aligned, uint32_t n_seg, uint32_t max_seg) {
     Plan p;
     uint32_t* w = p.w;
     const uint32_t ng = p.ng = n_groups ? n_groups : n;
@@ -366,6 +390,23 @@ static Plan choose(const Config& c, uint32_t n, uint32_t n_groups, uint32_t max_
     if (n_groups) {   // until one run of GROUP_CHUNK^levels covers the largest group
         w[LHB200_PLAN_GROUP_SUM] = LHB200_K_G1_GROUP_SUM;
         w[LHB200_PLAN_GROUP_SUM_LEVELS] = std::max<uint32_t>(1, tree_levels(max_group, GROUP_CHUNK, 1));
+    }
+    if (n_seg) {
+        // Segmented pass: the per-set stages above, then per segment its own sum of r sig (a tree over its run of sets),
+        // its own pair (-g1, sum) and its own tail.  Miller in latency mode only, one value per warp: no product may
+        // combine two segments.  The callers keep ng + n_seg <= n + n_seg <= pass_limit(c).
+        const uint32_t n_total = ng + n_seg, wpb = n_total <= 4 * COOP_TAIL ? 4 : mc::MC_WARPS;
+        w[LHB200_PLAN_SEGMENTS] = n_seg;
+        w[LHB200_PLAN_SUM] = LHB200_K_G2_SEGMENT_SUM;
+        w[LHB200_PLAN_SUM_LEVELS] = std::max<uint32_t>(1, tree_levels(max_seg, GROUP_CHUNK, 1));
+        w[LHB200_PLAN_LAST_MILLER] = 0;
+        w[LHB200_PLAN_MILLER] = LHB200_K_MILLER_WARP;
+        w[LHB200_PLAN_MILLER_WPB] = wpb;
+        w[LHB200_PLAN_MILLER_SPW] = 1;
+        w[LHB200_PLAN_MILLER_GRID] = cdiv(n_total, wpb);
+        p.miller_out = n_total;
+        w[LHB200_PLAN_FINAL] = LHB200_K_FINAL_SEGMENTS;
+        return p;
     }
     // Miller loops over the ng pairs and, except with k_miller_multi, the pair (-g1, sum r sig)
     const uint32_t n_total = ng + 1, max_warps = c.n_sm * mc::MC_WARPS;
@@ -748,8 +789,49 @@ constexpr uint32_t GROUP_MIN_REPEAT_DIV = 8;
 
 // Host uploads: group the sets by message and queue the CSR and the distinct messages on `s`.  n_groups stays 0 (the
 // ungrouped path) when too few messages repeat, or with LHB_GROUP_MESSAGES=0.
+// Segmented pass: the same policy over the whole pass, with (segment, message) as the group key.  Each segment is grouped
+// on its own and the CSRs are concatenated, so a group never spans two segments and a segment's groups (its pairs) stay
+// contiguous.  Queues the set and pair offsets of the segments on `s`.
+static int32_t upload_segment_groups(lhb200_bls_batch* b, const uint8_t* msgs, uint32_t n, cudaStream_t s) {
+    const uint32_t K = b->n_seg;
+    uint32_t* set_off = b->seg_h.data();
+    uint32_t* pair_off = set_off + K + 1;
+    memcpy(pair_off, set_off, (size_t)(K + 1) * 4);
+    if (g_cfg.group_messages && n >= 2) {
+        MsgGrouper& g = b->grouper;
+        b->seg_members.resize(n);
+        b->seg_goffsets.resize(n + 1);
+        b->seg_gmsgs.resize((size_t)n * 32);
+        uint32_t ng = 0, max_group = 0;
+        b->seg_goffsets[0] = 0;
+        for (uint32_t k = 0; k < K; k++) {
+            const uint32_t lo = set_off[k], m = set_off[k + 1] - lo;
+            uint32_t mg = 0;
+            const uint32_t gk = g.run(msgs + (size_t)32 * lo, m, 0, &mg);
+            for (uint32_t i = 0; i < m; i++) b->seg_members[lo + i] = lo + g.members[i];
+            for (uint32_t j = 0; j < gk; j++) b->seg_goffsets[ng + j + 1] = lo + g.offsets[j + 1];
+            memcpy(&b->seg_gmsgs[(size_t)32 * ng], g.msgs.data(), (size_t)32 * gk);
+            ng += gk;
+            max_group = std::max(max_group, mg);
+            pair_off[k + 1] = ng;
+        }
+        if (n - ng >= std::max<uint32_t>(1, n / GROUP_MIN_REPEAT_DIV)) {
+            LHB_CUDA(cudaMemcpyAsync(b->d_members, b->seg_members.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
+            LHB_CUDA(cudaMemcpyAsync(b->d_goffsets, b->seg_goffsets.data(), (size_t)(ng + 1) * 4, cudaMemcpyHostToDevice, s));
+            LHB_CUDA(cudaMemcpyAsync(b->d_gmsgs, b->seg_gmsgs.data(), (size_t)ng * 32, cudaMemcpyHostToDevice, s));
+            b->n_groups = ng;
+            b->max_group = max_group;
+        } else {
+            memcpy(pair_off, set_off, (size_t)(K + 1) * 4);
+        }
+    }
+    LHB_CUDA(cudaMemcpyAsync(b->d_seg_off, set_off, (size_t)2 * (K + 1) * 4, cudaMemcpyHostToDevice, s));
+    return LHB200_OK;
+}
+
 static int32_t upload_groups(lhb200_bls_batch* b, const uint8_t* msgs, uint32_t n, cudaStream_t s) {
     b->n_groups = 0;
+    if (b->n_seg) return upload_segment_groups(b, msgs, n, s);
     if (!g_cfg.group_messages || n < 2) return LHB200_OK;
     MsgGrouper& g = b->grouper;
     const uint32_t min_repeats = std::max<uint32_t>(1, n / GROUP_MIN_REPEAT_DIV);
@@ -778,6 +860,10 @@ static int32_t stage_inputs(const char* fn, lhb200_bls_batch* b, const lhb200_pu
     if (n_keys && !keys) { set_error("%s: no keys given", fn); return LHB200_EINVAL; }
     for (uint32_t i = 0; i < n_sets; i++)
         if (pk_offsets[i] > pk_offsets[i + 1]) { set_error("%s: offsets not monotone", fn); return LHB200_EINVAL; }
+    if (b->n_seg && b->seg_h[b->n_seg] != n_sets) {
+        set_error("%s: the segments cover %u sets, not %u", fn, b->seg_h[b->n_seg], n_sets);
+        return LHB200_EINVAL;
+    }
     if (!rands) {
         b->rbuf.resize(n_sets);
         if (!gen_rands(b->rbuf.data(), n_sets)) { set_error("%s: getrandom(2) failed", fn); return LHB200_ECUDA; }
@@ -940,6 +1026,7 @@ int32_t lhb200_bls_batch_set_device_inputs(lhb200_bls_batch* b, const void* d_si
     b->in_rands = static_cast<const uint64_t*>(d_rands);
     b->n_chunks = 0;
     b->n_groups = 0;   // device-resident messages are not grouped
+    b->n_seg = 0;      // segments apply to the host uploads only
     b->table = nullptr;
     return LHB200_OK;
 }
@@ -956,6 +1043,16 @@ static int32_t launch_signatures(lhb200_bls_batch* b, const Plan& p, uint64_t& l
         k_sig_prepare<<<w[LHB200_PLAN_LANE_GRID], BLS_BLOCK, 0, b->s2>>>(b->in_sigs, b->in_rands, n, b->d_sigr, b->d_status,
                                                                         b->d_fail);
     LHB_CUDA(cudaEventRecord(b->e_sig, b->s2));
+    if (w[LHB200_PLAN_SEGMENTS]) {   // one sum per segment, in place over the set positions
+        uint64_t span = 1;
+        for (uint32_t level = 0; level < w[LHB200_PLAN_SUM_LEVELS]; level++, span *= GROUP_CHUNK)
+            k_g2_segment_sum<<<cdiv(n, BLS_BLOCK), BLS_BLOCK, 0, b->s2>>>(b->d_sigr, b->d_seg_off, n, w[LHB200_PLAN_SEGMENTS],
+                                                                           level, span, b->d_seg_sig);
+        b->d_sig_sum = b->d_seg_sig;
+        launches += 1 + w[LHB200_PLAN_SUM_LEVELS];
+        LHB_CUDA(cudaEventRecord(b->e_join, b->s2));
+        return LHB200_OK;
+    }
     const bool warp = w[LHB200_PLAN_SUM] == LHB200_K_G2_SUM_WARP;   // latency mode: warp-wide additions
     b->d_sig_sum = reduce_tree(b->d_sigr, n, warp ? G2_SUM_WARP_CHUNK : REDUCE_CHUNK, w[LHB200_PLAN_SUM_LEVELS], b->d_sig_tmp,
                                [&](const G2Jac* in, uint32_t m, uint32_t mo, G2Jac* out) {
@@ -1069,9 +1166,14 @@ static int32_t launch_miller(lhb200_bls_batch* b, const Plan& p, cudaStream_t s,
     const uint8_t* st = grouped ? b->d_gskip : b->d_status;
     const uint8_t* pk_st = grouped ? b->d_gskip : b->d_pk_status;
     const uint32_t grid = w[LHB200_PLAN_MILLER_GRID], wpb = w[LHB200_PLAN_MILLER_WPB];
+    const uint32_t n_seg = w[LHB200_PLAN_SEGMENTS];
+    Fp12* const f = n_seg ? b->d_seg_f : b->d_f;
     if (!multi) LHB_CUDA(cudaStreamWaitEvent(s, b->e_join, 0));   // sum r sig (and -g1) ready
     LHB_CUDA(cudaEventRecord(b->e_k0, s));
-    if (w[LHB200_PLAN_MILLER] == LHB200_K_MILLER_WARP)
+    if (n_seg)
+        mw::k_miller_warp_segments<<<grid, 32 * wpb, mw::smem_bytes((int)wpb), s>>>(P, b->d_h, st, pk_st, p.ng, b->d_seg_sig,
+                                                                                  n_seg, b->d_neg_g1, f);
+    else if (w[LHB200_PLAN_MILLER] == LHB200_K_MILLER_WARP)
         mw::k_miller_warp<<<grid, 32 * wpb, mw::smem_bytes((int)wpb), s>>>(P, b->d_h, st, pk_st, p.ng, b->d_sig_sum,
                                                                          b->d_neg_g1, b->d_f);
     else if (w[LHB200_PLAN_MILLER] == LHB200_K_MILLER_COOP)
@@ -1081,7 +1183,7 @@ static int32_t launch_miller(lhb200_bls_batch* b, const Plan& p, cudaStream_t s,
         k_miller_multi<<<grid, MILLER_BLOCK, 0, s>>>(P, b->d_h, st, pk_st, p.ng, w[LHB200_PLAN_MILLER_SPW], p.miller_out,
                                                      b->d_f);
     LHB_CUDA(cudaEventRecord(b->e_k1, s));
-    *prod = reduce_tree<Fp12>(b->d_f, p.miller_out, REDUCE_CHUNK, w[LHB200_PLAN_FP12_REDUCE_LEVELS], b->d_f_tmp,
+    *prod = reduce_tree<Fp12>(f, p.miller_out, REDUCE_CHUNK, w[LHB200_PLAN_FP12_REDUCE_LEVELS], b->d_f_tmp,
                               [&](const Fp12* in, uint32_t m, uint32_t mo, Fp12* out) {
                                   k_fp12_reduce<<<cdiv(mo, BLS_BLOCK), BLS_BLOCK, 0, s>>>(in, m, REDUCE_CHUNK, out);
                               });
@@ -1095,8 +1197,10 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
     if (!b || b->n == 0 || !b->in_sigs) { set_error("bls_batch_verify_enqueue: no inputs"); return LHB200_EINVAL; }
     cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx().stream;
     const uint32_t n = b->n;
+    const uint32_t n_seg = b->n_seg;
+    if (n_seg && b->seg_h[n_seg] != n) { set_error("bls_batch_verify_enqueue: the segments do not cover the sets"); return LHB200_EINVAL; }
     const Plan p = choose(g_cfg, n, b->n_groups, b->max_group, b->table != nullptr, (uint32_t)b->n_chunks,
-                          b->in_pks && ((uintptr_t)b->in_pks & 15) == 0);
+                          b->in_pks && ((uintptr_t)b->in_pks & 15) == 0, n_seg, b->max_seg);
     memcpy(b->plan, p.w, sizeof b->plan);
     if (p.mc_scratch_words > b->mc_scratch_words) {
         LHB_CUDA(cudaStreamSynchronize(s));
@@ -1124,7 +1228,11 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
     if (b->n_groups) launch_group_sum(b, p, s, launches);
     if (int32_t rc = launch_miller(b, p, s, launches, &prod)) return rc;
     const uint32_t n_tail = p.w[LHB200_PLAN_N_TAIL];
-    if (p.w[LHB200_PLAN_FINAL] == LHB200_K_FINAL_WARP)   // phase-interpreter tail (bls/fe_warp.cuh)
+    if (n_seg)   // one block per segment; pair offsets follow the set offsets in d_seg_off
+        fe::k_final_segments<<<n_seg, 32 * fe::FE_WARPS, fe::smem_bytes(), s>>>(prod, p.ng, b->d_seg_off + n_seg + 1,
+                                                                                b->d_seg_off, b->d_status, b->d_pk_status,
+                                                                                b->d_seg_ok, b->d_seg_gt);
+    else if (p.w[LHB200_PLAN_FINAL] == LHB200_K_FINAL_WARP)   // phase-interpreter tail (bls/fe_warp.cuh)
         fe::k_final_warp<<<1, 32 * fe::FE_WARPS, fe::smem_bytes(), s>>>(prod, n_tail, b->d_fail, b->d_ok, b->d_gt);
     else
         k_final_coop<<<1, COOP_THREADS, sizeof(CoopFinalSmem), s>>>(prod, n_tail, p.w[LHB200_PLAN_LAST_MILLER] ? b->d_flast : nullptr,
@@ -1133,6 +1241,8 @@ int32_t lhb200_bls_batch_verify_enqueue(lhb200_bls_batch* b, void* stream) {
     LHB_CUDA(cudaGetLastError());
     count_launch(launches);
     b->launches_last = launches;
+    b->n_seg_last = n_seg;
+    b->n_seg = 0;
     return LHB200_OK;
 }
 
@@ -1146,11 +1256,10 @@ int32_t lhb200_bls_batch_allreduce_verdict(lhb200_bls_batch* b, void* stream) {
     return comm_allreduce_min_u8(b->d_ok, 1, s);
 }
 
-int32_t lhb200_bls_batch_result(lhb200_bls_batch* b, void* stream, uint8_t* ok, uint8_t* set_status) {
-    LHB_REQUIRE_READY();
-    if (!b || !ok) return LHB200_EINVAL;
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx().stream;
-    LHB_CUDA(cudaMemcpyAsync(b->h_res, b->d_ok, 1, cudaMemcpyDeviceToHost, s));
+// The verdicts (n_ok bytes at d_ok, through the pinned h_ok) and optionally the per-set statuses of the last verify.
+static int32_t fetch_results(lhb200_bls_batch* b, cudaStream_t s, const uint8_t* d_ok, uint8_t* h_ok, uint32_t n_ok,
+                             uint8_t* ok, uint8_t* set_status) {
+    LHB_CUDA(cudaMemcpyAsync(h_ok, d_ok, n_ok, cudaMemcpyDeviceToHost, s));
     uint8_t* const h_sig = b->h_res + 64;
     uint8_t* const h_pk = h_sig + b->cap_sets;
     if (set_status) {
@@ -1166,21 +1275,69 @@ int32_t lhb200_bls_batch_result(lhb200_bls_batch* b, void* stream, uint8_t* ok, 
     } else {
         LHB_CUDA(cudaStreamSynchronize(s));
     }
-    *ok = b->h_res[0];
+    memcpy(ok, h_ok, n_ok);
     // the two stages' codes for each set, the signature's first (the oracle checks the signature before the keys)
     if (set_status)
         for (uint32_t i = 0; i < b->n; i++) set_status[i] = h_sig[i] ? h_sig[i] : h_pk[i];
     return LHB200_OK;
 }
 
+int32_t lhb200_bls_batch_result(lhb200_bls_batch* b, void* stream, uint8_t* ok, uint8_t* set_status) {
+    LHB_REQUIRE_READY();
+    if (!b || !ok) return LHB200_EINVAL;
+    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx().stream;
+    return fetch_results(b, s, b->d_ok, b->h_res, 1, ok, set_status);
+}
+
+// ---- segmented passes ------------------------------------------------------------------------------------------
+int32_t lhb200_bls_batch_set_segments(lhb200_bls_batch* b, const uint32_t* batch_offsets, uint32_t n_batches) {
+    LHB_REQUIRE_READY();
+    const char* fn = "bls_batch_set_segments";
+    if (!b || !batch_offsets || n_batches == 0) { set_error("%s: bad arguments", fn); return LHB200_EINVAL; }
+    if (batch_offsets[0] != 0) { set_error("%s: offsets do not start at 0", fn); return LHB200_EINVAL; }
+    uint32_t max_seg = 0;
+    for (uint32_t k = 0; k < n_batches; k++) {
+        if (batch_offsets[k + 1] <= batch_offsets[k]) { set_error("%s: empty or non-monotone segment", fn); return LHB200_EINVAL; }
+        max_seg = std::max(max_seg, batch_offsets[k + 1] - batch_offsets[k]);
+    }
+    const uint32_t n = batch_offsets[n_batches], limit = pass_limit(g_cfg);
+    if (n > b->cap_sets) { set_error("%s: more sets than the batch holds", fn); return LHB200_EINVAL; }
+    if ((uint64_t)n + n_batches > limit) {
+        set_error("%s: %u sets in %u segments exceed one pass (%u sets + segments)", fn, n, n_batches, limit);
+        return LHB200_EINVAL;
+    }
+    if (!b->d_seg_off) {   // first segmented pass on this handle: buffers for the largest pass
+#define ALLOC(p, bytes)                                                                                  \
+    do {                                                                                                 \
+        cudaError_t e = (p) ? cudaSuccess : cudaMalloc(reinterpret_cast<void**>(&(p)), (bytes));         \
+        if (e != cudaSuccess) return cuda_fail(e, "cudaMalloc(" #p ")");                                 \
+    } while (0)
+        ALLOC(b->d_seg_sig, (size_t)limit * sizeof(G2Jac));
+        ALLOC(b->d_seg_f, (size_t)limit * sizeof(Fp12));
+        ALLOC(b->d_seg_gt, (size_t)limit * sizeof(Fp12));
+        ALLOC(b->d_seg_ok, limit);
+        if (!b->h_seg_ok) LHB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&b->h_seg_ok), limit, cudaHostAllocDefault));
+        ALLOC(b->d_seg_off, (size_t)2 * (limit + 1) * 4);   // last: it marks the set as complete
+#undef ALLOC
+    }
+    b->n = 0;   // inputs uploaded before do not carry the segments' grouping
+    b->seg_h.assign(2 * (n_batches + 1), 0);
+    memcpy(b->seg_h.data(), batch_offsets, (size_t)(n_batches + 1) * 4);
+    b->max_seg = max_seg;
+    b->n_seg = n_batches;
+    return LHB200_OK;
+}
+
+int32_t lhb200_bls_batch_segment_result(lhb200_bls_batch* b, void* stream, uint8_t* ok, uint8_t* set_status) {
+    LHB_REQUIRE_READY();
+    if (!b || !ok || !b->n_seg_last) { set_error("bls_batch_segment_result: no segmented verify on this batch"); return LHB200_EINVAL; }
+    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx().stream;
+    return fetch_results(b, s, b->d_seg_ok, b->h_seg_ok, b->n_seg_last, ok, set_status);
+}
+
 // Test hook: the value final_exp(product)^... of the last verify as 12 x 48-byte big-endian canonical Fp
 // (order c0.c0.c0, c0.c0.c1, c0.c1.c0, ... c1.c2.c1).  It is the CUBE of the canonical GT element (pairing.cuh).
-int32_t lhb200_bls_batch_gt(lhb200_bls_batch* b, uint8_t out576[576]) {
-    LHB_REQUIRE_READY();
-    if (!b || !out576) return LHB200_EINVAL;
-    Fp12 f;
-    LHB_CUDA(cudaDeviceSynchronize());
-    LHB_CUDA(cudaMemcpy(&f, b->d_gt, sizeof f, cudaMemcpyDeviceToHost));
+static void gt_to_bytes(const Fp12& f, uint8_t out576[576]) {
     const Fp* c = reinterpret_cast<const Fp*>(&f);
     // host-side conversion out of Montgomery form (plain integer arithmetic on 12 limbs, test hook only)
     for (int k = 0; k < 12; k++) {
@@ -1223,6 +1380,26 @@ int32_t lhb200_bls_batch_gt(lhb200_bls_batch* b, uint8_t out576[576]) {
             q[0] = t[j] >> 24; q[1] = t[j] >> 16; q[2] = t[j] >> 8; q[3] = t[j];
         }
     }
+}
+
+int32_t lhb200_bls_batch_gt(lhb200_bls_batch* b, uint8_t out576[576]) {
+    LHB_REQUIRE_READY();
+    if (!b || !out576) return LHB200_EINVAL;
+    Fp12 f;
+    LHB_CUDA(cudaDeviceSynchronize());
+    LHB_CUDA(cudaMemcpy(&f, b->d_gt, sizeof f, cudaMemcpyDeviceToHost));
+    gt_to_bytes(f, out576);
+    return LHB200_OK;
+}
+
+// Test hook: segment k's value of the last segmented verify, in the format of lhb200_bls_batch_gt.
+int32_t lhb200_bls_batch_segment_gt(lhb200_bls_batch* b, uint32_t k, uint8_t out576[576]) {
+    LHB_REQUIRE_READY();
+    if (!b || !out576 || k >= b->n_seg_last) { set_error("bls_batch_segment_gt: no segment %u in the last verify", k); return LHB200_EINVAL; }
+    Fp12 f;
+    LHB_CUDA(cudaDeviceSynchronize());
+    LHB_CUDA(cudaMemcpy(&f, b->d_seg_gt + k, sizeof f, cudaMemcpyDeviceToHost));
+    gt_to_bytes(f, out576);
     return LHB200_OK;
 }
 
@@ -1243,6 +1420,117 @@ float lhb200_bls_batch_dominant_kernel_ms(const lhb200_bls_batch* b) {
     return ms;
 }
 
+// bls::verify_signature_sets (crypto/bls/src/impls/blst.rs:37-119) on one pooled handle, alone.  Re-entrant: every call
+// borrows a batch handle (device buffers, streams, events — no cudaMalloc on the steady path) from a pool and drives it
+// on the handle's own stream, so concurrent calls overlap on the device instead of queueing behind one mutex.
+static int32_t verify_alone(const uint8_t* sigs, const uint8_t* msgs, const uint8_t* pks, const uint32_t* pk_offsets,
+                            const uint64_t* rands, uint32_t n_sets, uint8_t* ok, uint8_t* set_status) {
+    const uint64_t n_keys = pk_offsets[n_sets];
+    lhb200_bls_batch* b = pool_acquire(n_sets, n_keys);
+    if (!b) return LHB200_ENOMEM;
+    int32_t rc = lhb200_bls_batch_upload_async(b, sigs, msgs, pks, pk_offsets, rands, n_sets, b->s_main);
+    if (!rc) rc = lhb200_bls_batch_verify_enqueue(b, b->s_main);
+    if (!rc) rc = lhb200_bls_batch_result(b, b->s_main, ok, set_status);
+    cudaStreamSynchronize(b->s2);
+    cudaStreamSynchronize(b->s3);
+    pool_release(b);
+    return rc;
+}
+
+// One segmented pass on a pooled handle: n sets (keys indexed from pk_offsets[0] == 0) in n_seg non-empty batches
+// seg_off[0 .. n_seg] -> ok[n_seg] and, optionally, the n statuses.  rands NULL: drawn for the whole pass.
+static int32_t verify_pass(const uint8_t* sigs, const uint8_t* msgs, const uint8_t* pks, const uint32_t* pk_offsets,
+                           const uint64_t* rands, uint32_t n, const uint32_t* seg_off, uint32_t n_seg, uint8_t* ok,
+                           uint8_t* set_status) {
+    lhb200_bls_batch* b = pool_acquire(n, pk_offsets[n]);
+    if (!b) return LHB200_ENOMEM;
+    int32_t rc = lhb200_bls_batch_set_segments(b, seg_off, n_seg);
+    if (!rc) rc = lhb200_bls_batch_upload_async(b, sigs, msgs, pks, pk_offsets, rands, n, b->s_main);
+    if (!rc) rc = lhb200_bls_batch_verify_enqueue(b, b->s_main);
+    if (!rc) rc = lhb200_bls_batch_segment_result(b, b->s_main, ok, set_status);
+    b->n_seg = 0;   // (left set by a failed upload)
+    cudaStreamSynchronize(b->s2);
+    cudaStreamSynchronize(b->s3);
+    pool_release(b);
+    return rc;
+}
+
+// The argument checks of the host uploads, made before a call is queued (so that its error is its own).
+static int32_t check_sets(const char* fn, const uint8_t* sigs, const uint8_t* msgs, const uint8_t* pks,
+                          const uint32_t* pk_offsets, const uint64_t* rands, uint32_t n) {
+    if (n && (!sigs || !msgs || !pk_offsets)) { set_error("%s: bad arguments", fn); return LHB200_EINVAL; }
+    for (uint32_t i = 0; i < n; i++)
+        if (pk_offsets[i] > pk_offsets[i + 1]) { set_error("%s: offsets not monotone", fn); return LHB200_EINVAL; }
+    if (n && pk_offsets[n] > pk_offsets[0] && !pks) { set_error("%s: no keys given", fn); return LHB200_EINVAL; }
+    if (rands)
+        for (uint32_t i = 0; i < n; i++)
+            if (rands[i] == 0) { set_error("%s: zero random scalar", fn); return LHB200_EINVAL; }
+    return LHB200_OK;
+}
+
+// ---- coalescing of concurrent plugin calls ----------------------------------------------------------------------
+// Lighthouse calls verify_signature_sets from up to num_cpus blocking workers with <= 64-set gossip batches
+// (beacon_processor/src/lib.rs:202-203,256).  Alone, such a batch is one wave of warps and a one-warp final
+// exponentiation; concurrent calls are merged into segmented passes instead (leader / follower, no timer, no thread).
+namespace {
+constexpr uint32_t COALESCE_MAX_SETS = 64;   // calls above run alone: they are not what the gossip workers send
+// Passes (lone calls included) on the device at once.  Measured on the H100 (DESIGN.md §2.7): with 2, 64 threads of
+// 1-key gossip batches got 1.55x the batches/s of uncoalesced calls, but 8 and 16 threads lost a third (a lone call
+// overlaps better with other lone calls than a queued call with a pass); with 8, 16 threads still lost 10-17 %.  With
+// 16, up to 16 concurrent callers run exactly as before, and callers beyond them are merged.
+constexpr uint32_t PASSES_IN_FLIGHT = 16;
+struct Waiter {   // a queued call; its thread blocks in the call, so its buffers stay valid
+    const uint8_t *sigs, *msgs, *pks;
+    const uint32_t* pk_offsets;
+    const uint64_t* rands;   // the caller's, or drawn by the caller
+    uint32_t n;
+    uint8_t *ok, *set_status;
+    int32_t rc = LHB200_OK;
+    std::string err;
+    bool done = false;
+};
+std::mutex g_co_mu;
+std::condition_variable g_co_cv;
+uint32_t g_co_running = 0;   // passes in flight
+std::deque<Waiter*> g_co_queue;
+
+// The leader's work: the calls of `pass` as one segmented pass; every call gets its own verdict and statuses, or the
+// pass's error.
+void run_coalesced(const std::vector<Waiter*>& pass) {
+    uint32_t n = 0;
+    uint64_t n_keys = 0;
+    for (const Waiter* w : pass) { n += w->n; n_keys += w->pk_offsets[w->n] - w->pk_offsets[0]; }
+    std::vector<uint8_t> sigs((size_t)n * 96), msgs((size_t)n * 32), pks((size_t)n_keys * 96), st(n), ok(pass.size());
+    std::vector<uint32_t> offs(n + 1), seg(pass.size() + 1);
+    std::vector<uint64_t> rands(n);
+    uint32_t lo = 0;
+    uint64_t kb = 0;
+    offs[0] = 0;
+    for (size_t k = 0; k < pass.size(); k++) {
+        const Waiter* w = pass[k];
+        const uint32_t k0 = w->pk_offsets[0], kn = w->pk_offsets[w->n] - k0;
+        seg[k] = lo;
+        memcpy(&sigs[(size_t)96 * lo], w->sigs, (size_t)96 * w->n);
+        memcpy(&msgs[(size_t)32 * lo], w->msgs, (size_t)32 * w->n);
+        if (kn) memcpy(&pks[96 * kb], w->pks + (size_t)96 * k0, (size_t)96 * kn);
+        memcpy(&rands[lo], w->rands, (size_t)8 * w->n);
+        for (uint32_t i = 1; i <= w->n; i++) offs[lo + i] = (uint32_t)(kb + w->pk_offsets[i] - k0);
+        lo += w->n;
+        kb += kn;
+    }
+    seg[pass.size()] = n;
+    const int32_t rc = verify_pass(sigs.data(), msgs.data(), pks.data(), offs.data(), rands.data(), n, seg.data(),
+                                   (uint32_t)pass.size(), ok.data(), st.data());
+    for (size_t k = 0; k < pass.size(); k++) {
+        Waiter* w = pass[k];
+        w->rc = rc;
+        if (rc) { w->err = lhb200_last_error(); continue; }
+        *w->ok = ok[k];
+        if (w->set_status) memcpy(w->set_status, &st[seg[k]], w->n);
+    }
+}
+}  // namespace
+
 // bls::verify_signature_sets (crypto/bls/src/impls/blst.rs:37-119).  *ok = 1 iff every set verifies.
 // n_sets == 0 -> *ok = 0 (blst.rs:42-44).  rands may be NULL (drawn internally, 64 nonzero bits each).
 // set_status (optional, n bytes): per-set preparation status (0 = fine; see SetStatus in kernels.cuh).
@@ -1254,20 +1542,110 @@ int32_t lhb200_verify_signature_sets(const uint8_t* sigs, const uint8_t* msgs, c
     *ok = 0;
     if (n_sets == 0) return LHB200_OK;
     if (!pk_offsets) { set_error("verify_signature_sets: null offsets"); return LHB200_EINVAL; }
-    // Re-entrant: Lighthouse calls this from up to num_cpus blocking workers with <= 64-set gossip batches
-    // (beacon_processor/src/lib.rs:202-203,256).  Every call borrows a batch handle (device buffers, streams, events —
-    // no cudaMalloc on the steady path) from a pool and drives it on the handle's own stream, so concurrent calls
-    // overlap on the device instead of queueing behind one mutex.
-    const uint64_t n_keys = pk_offsets[n_sets];
-    lhb200_bls_batch* b = pool_acquire(n_sets, n_keys);
-    if (!b) return LHB200_ENOMEM;
-    int32_t rc = lhb200_bls_batch_upload_async(b, sigs, msgs, pks, pk_offsets, rands, n_sets, b->s_main);
-    if (!rc) rc = lhb200_bls_batch_verify_enqueue(b, b->s_main);
-    if (!rc) rc = lhb200_bls_batch_result(b, b->s_main, ok, set_status);
-    cudaStreamSynchronize(b->s2);
-    cudaStreamSynchronize(b->s3);
-    pool_release(b);
-    return rc;
+    if (n_sets > COALESCE_MAX_SETS) return verify_alone(sigs, msgs, pks, pk_offsets, rands, n_sets, ok, set_status);
+    std::unique_lock<std::mutex> lk(g_co_mu);
+    if (g_co_running < PASSES_IN_FLIGHT && g_co_queue.empty()) {   // a free slot: today's path, alone
+        g_co_running++;
+        lk.unlock();
+        const int32_t rc = verify_alone(sigs, msgs, pks, pk_offsets, rands, n_sets, ok, set_status);
+        lk.lock();
+        g_co_running--;
+        lk.unlock();
+        g_co_cv.notify_all();
+        return rc;
+    }
+    lk.unlock();
+    // queue: this caller's own argument checks and scalars first
+    if (int32_t rc = check_sets("verify_signature_sets", sigs, msgs, pks, pk_offsets, rands, n_sets)) return rc;
+    std::vector<uint64_t> own_rands;
+    if (!rands) {
+        own_rands.resize(n_sets);
+        if (!gen_rands(own_rands.data(), n_sets)) { set_error("verify_signature_sets: getrandom(2) failed"); return LHB200_ECUDA; }
+        rands = own_rands.data();
+    }
+    Waiter me;
+    me.sigs = sigs; me.msgs = msgs; me.pks = pks; me.pk_offsets = pk_offsets; me.rands = rands; me.n = n_sets;
+    me.ok = ok; me.set_status = set_status;
+    lk.lock();
+    g_co_queue.push_back(&me);
+    g_co_cv.wait(lk, [&] {   // (a leader may have taken this call already: the queue can be empty)
+        return me.done || (!g_co_queue.empty() && g_co_queue.front() == &me && g_co_running < PASSES_IN_FLIGHT);
+    });
+    if (me.done) {   // a leader ran this call
+        lk.unlock();
+        if (me.rc) set_error("%s", me.err.c_str());
+        return me.rc;
+    }
+    // leader: the waiting calls that fit one pass, in arrival order
+    g_co_running++;
+    std::vector<Waiter*> pass;
+    uint32_t sets = 0;
+    const uint32_t limit = pass_limit(g_cfg);
+    while (!g_co_queue.empty() && sets + g_co_queue.front()->n + pass.size() + 1 <= limit) {
+        pass.push_back(g_co_queue.front());
+        sets += g_co_queue.front()->n;
+        g_co_queue.pop_front();
+    }
+    lk.unlock();
+    g_co_cv.notify_all();   // the next waiting call may lead the other slot
+    if (pass.size() == 1) me.rc = verify_alone(sigs, msgs, pks, pk_offsets, rands, n_sets, ok, set_status);
+    else run_coalesced(pass);
+    lk.lock();
+    for (Waiter* w : pass) w->done = true;
+    g_co_running--;
+    lk.unlock();
+    g_co_cv.notify_all();
+    if (me.rc && !me.err.empty()) set_error("%s", me.err.c_str());   // (a lone run set it on this thread already)
+    return me.rc;
+}
+
+int32_t lhb200_verify_signature_set_batches(const uint8_t* sigs, const uint8_t* msgs, const uint8_t* pks,
+                                            const uint32_t* pk_offsets, const uint64_t* rands, uint32_t n_sets,
+                                            const uint32_t* batch_offsets, uint32_t n_batches, uint8_t* ok,
+                                            uint8_t* set_status) {
+    LHB_REQUIRE_READY();
+    const char* fn = "verify_signature_set_batches";
+    if (n_batches == 0) return LHB200_OK;
+    if (!ok || !batch_offsets || (n_sets && !pk_offsets)) { set_error("%s: bad arguments", fn); return LHB200_EINVAL; }
+    if (batch_offsets[0] != 0 || batch_offsets[n_batches] != n_sets) {
+        set_error("%s: batch offsets do not span the %u sets", fn, n_sets);
+        return LHB200_EINVAL;
+    }
+    for (uint32_t k = 0; k < n_batches; k++)
+        if (batch_offsets[k] > batch_offsets[k + 1]) { set_error("%s: batch offsets not monotone", fn); return LHB200_EINVAL; }
+    if (int32_t rc = check_sets(fn, sigs, msgs, pks, pk_offsets, rands, n_sets)) return rc;
+    const uint32_t limit = pass_limit(g_cfg);
+    std::vector<uint32_t> offs, seg;
+    for (uint32_t k = 0; k < n_batches;) {
+        const uint32_t lo = batch_offsets[k];
+        if (batch_offsets[k + 1] == lo) { ok[k++] = 0; continue; }   // an empty batch (blst.rs:42-44)
+        if (batch_offsets[k + 1] - lo + 1 > limit) {                 // too large for a pass of its own
+            const uint32_t n = batch_offsets[k + 1] - lo;
+            offs.assign(pk_offsets + lo, pk_offsets + lo + n + 1);
+            for (uint32_t& o : offs) o -= pk_offsets[lo];
+            if (int32_t rc = verify_alone(sigs + (size_t)96 * lo, msgs + (size_t)32 * lo, pks + (size_t)96 * pk_offsets[lo],
+                                          offs.data(), rands ? rands + lo : nullptr, n, ok + k,
+                                          set_status ? set_status + lo : nullptr))
+                return rc;
+            k++;
+            continue;
+        }
+        // the following non-empty batches while sets + batches fit one pass
+        seg.assign(1, 0);
+        uint32_t e = k;
+        for (; e < n_batches && batch_offsets[e + 1] > batch_offsets[e] &&
+               batch_offsets[e + 1] - lo + (e - k + 1) <= limit; e++)
+            seg.push_back(batch_offsets[e + 1] - lo);
+        const uint32_t n = batch_offsets[e] - lo;
+        offs.assign(pk_offsets + lo, pk_offsets + lo + n + 1);
+        for (uint32_t& o : offs) o -= pk_offsets[lo];
+        if (int32_t rc = verify_pass(sigs + (size_t)96 * lo, msgs + (size_t)32 * lo, pks + (size_t)96 * pk_offsets[lo],
+                                     offs.data(), rands ? rands + lo : nullptr, n, seg.data(), e - k, ok + k,
+                                     set_status ? set_status + lo : nullptr))
+            return rc;
+        k = e;
+    }
+    return LHB200_OK;
 }
 
 // verify_signature_sets over the ranks of the library's communicator: every rank passes ITS shard of the sets (possibly
