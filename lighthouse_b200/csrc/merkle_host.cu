@@ -42,8 +42,20 @@ int32_t merkle_init() {
 // ---------------------------------------------------------------------------------------------------------
 // Plan: everything needed to hash one object — leaf kernels, reduce passes, the tail hash program.
 // All device memory a plan touches lives in one arena: [staged inputs | scratch nodes | literals | slots].
+
+// The leaf kernel of a big list turns each fixed-size SSZ item into its 32-byte root, at `units` hash32_concat each.
+struct LeafKind {
+    enum Kernel { NONE, VALIDATORS, RECORDS, HASH_PAIRS } kernel;   // NONE: the items already are the chunks
+    int record;                                                     // k_record_roots kind (RECORDS only)
+    uint32_t units;
+};
+constexpr LeafKind LEAF_NONE{LeafKind::NONE, 0, 0}, LEAF_VALIDATOR{LeafKind::VALIDATORS, 0, 8},
+                   LEAF_PUBKEY{LeafKind::RECORDS, 0, 1}, LEAF_ETH1_DATA{LeafKind::RECORDS, 1, 3},
+                   LEAF_U64_PAIR{LeafKind::RECORDS, 2, 1}, LEAF_U64_TRIPLE{LeafKind::RECORDS, 3, 3},
+                   LEAF_CHUNK_PAIR{LeafKind::HASH_PAIRS, 0, 1};
+
 struct LeafLaunch {
-    int kind;  // 0 validator roots, 1 pubkey roots, 2 eth1data roots, 3 hash pairs
+    LeafKind kind;
     const uint8_t* in;
     uint8_t* out;
     uint64_t n;
@@ -85,7 +97,6 @@ struct Plan {
     HashOp* d_ops = nullptr;
     int32_t* d_waves = nullptr;
     int n_waves = 0;
-    uint64_t root_addr = 0;
 
     uint8_t* alloc(size_t nbytes, size_t align = 256) {  // device sub-allocation
         size_t off = align_up(bump, align);
@@ -207,11 +218,10 @@ struct Plan {
         for (uint32_t l = level; l < depth; l++) r = op_hash(r, zero_op(l));
         return r;
     }
-    uint8_t* leaf_kernel(int kind, const uint8_t* in, uint64_t n) {
+    uint8_t* leaf_kernel(LeafKind kind, const uint8_t* in, uint64_t n) {
         uint8_t* out = alloc(std::max<uint64_t>(n, 1) * 32);
         if (n) leaves.push_back({kind, in, out, n});
-        static const int units[6] = {8, 1, 3, 1, 1, 3};
-        hash_units += (uint64_t)units[kind] * n;
+        hash_units += (uint64_t)kind.units * n;
         return out;
     }
 };
@@ -220,26 +230,20 @@ static int32_t plan_enqueue_tail(Plan& pl, cudaStream_t s);
 // Enqueue a finished plan on `s`.  Literals must already be in the arena.
 static int32_t plan_enqueue(Plan& pl, cudaStream_t s, cudaEvent_t e0 = nullptr, cudaEvent_t e1 = nullptr) {
     for (const LeafLaunch& L : pl.leaves) {
-        switch (L.kind) {
-            case 0:
+        switch (L.kind.kernel) {
+            case LeafKind::VALIDATORS:
                 if (e0) cudaEventRecord(e0, s);
                 k_validator_roots<<<(unsigned)ceil_div(L.n, VAL_PER_CTA), VAL_PER_CTA, 0, s>>>(L.in, L.n, L.out);
                 if (e1) cudaEventRecord(e1, s);
                 break;
-            case 1:
-                k_record_roots<<<(unsigned)ceil_div(L.n, 128), 128, 0, s>>>(L.in, L.n, 0, L.out);
+            case LeafKind::RECORDS:
+                k_record_roots<<<(unsigned)ceil_div(L.n, 128), 128, 0, s>>>(L.in, L.n, L.kind.record, L.out);
                 break;
-            case 2:
-                k_record_roots<<<(unsigned)ceil_div(L.n, 128), 128, 0, s>>>(L.in, L.n, 1, L.out);
-                break;
-            case 4:
-                k_record_roots<<<(unsigned)ceil_div(L.n, 128), 128, 0, s>>>(L.in, L.n, 2, L.out);
-                break;
-            case 5:
-                k_record_roots<<<(unsigned)ceil_div(L.n, 128), 128, 0, s>>>(L.in, L.n, 3, L.out);
-                break;
-            default:
+            case LeafKind::HASH_PAIRS:
                 k_hash_pairs<<<(unsigned)ceil_div(L.n, 256), 256, 0, s>>>(L.in, L.out, L.n);
+                break;
+            case LeafKind::NONE:
+                break;   // leaf_kernel is never called without a kernel
         }
         count_launch();
     }
@@ -284,24 +288,22 @@ static int32_t plan_enqueue_tail(Plan& pl, cudaStream_t s) {
     return LHB200_OK;
 }
 
-// Sort ops by wave, build wave table; returns host blobs to upload.
-static void plan_finalize_program(Plan& pl, std::vector<HashOp>& ops_sorted, std::vector<int32_t>& waves) {
-    int nw = 0;
-    for (int w : pl.op_wave) nw = std::max(nw, w + 1);
-    std::vector<std::vector<HashOp>> by(nw);
-    for (size_t i = 0; i < pl.ops.size(); i++) by[pl.op_wave[i]].push_back(pl.ops[i]);
-    waves.assign(1, 0);
-    for (int w = 0; w < nw; w++) {
-        for (auto& o : by[w]) ops_sorted.push_back(o);
-        waves.push_back((int32_t)ops_sorted.size());
-    }
-    pl.n_waves = nw;
-    pl.h_waves = waves;
+// ---------------------------------------------------------------------------------------------------------
+// Plan lifecycle: size, take an arena, build, upload literals and program, enqueue, read the root.
+
+// Device bytes of the program blobs plan_upload allocates from the arena: ops, wave table (at most one entry per op,
+// plus one) and byte items, each 256-byte aligned.
+static size_t program_bytes(size_t n_ops, size_t n_items) {
+    return align_up(n_ops * sizeof(HashOp), 256) + align_up((n_ops + 2) * 4, 256) +
+           align_up(n_items * sizeof(ByteItem), 256) + 512;
+}
+// Pinned staging plan_upload needs: literals, then the program blobs.
+static size_t plan_stage_bytes(const Plan& pl) {
+    return align_up(pl.lit.size(), 256) + program_bytes(pl.ops.size(), pl.items.size());
 }
 
-// ---------------------------------------------------------------------------------------------------------
-// A "session": dry-run the planner to size the arena, allocate, then plan for real.  `build` must be
-// deterministic in its allocation sequence.
+// Run `build` over the arena (null: a dry run that only sizes).  `build` must be deterministic in its allocation
+// sequence and returns a status.
 template <class F>
 static int32_t build_plan(Plan& pl, uint8_t* arena, size_t arena_bytes, size_t lit_cap, F&& build,
                           size_t node_cap = 8192) {
@@ -313,7 +315,8 @@ static int32_t build_plan(Plan& pl, uint8_t* arena, size_t arena_bytes, size_t l
     pl.node_off = align_up(lit_cap, 256);   // literals first, then the node pool
     pl.node_cap = node_cap;
     pl.bump = pl.node_off + node_cap * 32;
-    build(pl);
+    const int32_t rc = build(pl);
+    if (rc) return rc;
     if (pl.lit.size() > lit_cap) {
         set_error("internal: literal block overflow (%zu > %zu)", pl.lit.size(), lit_cap);
         return LHB200_EINVAL;
@@ -325,105 +328,134 @@ static int32_t build_plan(Plan& pl, uint8_t* arena, size_t arena_bytes, size_t l
     return LHB200_OK;
 }
 
-// upload literals + program; program blobs live at the end of the arena
-static int32_t plan_upload(Plan& pl, cudaStream_t s, std::vector<HashOp>& ops_sorted, std::vector<int32_t>& waves,
-                           void* h_stage) {
-    // h_stage: pinned host staging of at least lit + ops + waves bytes
-    uint8_t* h = static_cast<uint8_t*>(h_stage);
-    size_t o = 0;
-    if (!pl.lit.empty()) {
-        memcpy(h + o, pl.lit.data(), pl.lit.size());
-        LHB_CUDA(cudaMemcpyAsync(pl.arena + pl.lit_off, h + o, pl.lit.size(), cudaMemcpyHostToDevice, s));
-        o += align_up(pl.lit.size(), 256);
+// Size-then-build: a dry run over a null arena gives the plan's footprint; take(need, &arena, &bytes) supplies an
+// arena of bytes >= need (the build, its program blobs and `extra` bytes the caller allocates after the build), and
+// the build runs again over it.
+template <class F, class T>
+static int32_t build_sized(Plan& pl, size_t lit_cap, size_t extra, F&& build, T&& take) {
+    Plan dry;
+    int32_t rc = build_plan(dry, nullptr, 0, lit_cap, build);
+    if (rc) return rc;
+    uint8_t* arena = nullptr;
+    size_t bytes = 0;
+    rc = take(align_up(dry.bump, 256) + program_bytes(dry.ops.size(), dry.items.size()) + extra, &arena, &bytes);
+    if (rc) return rc;
+    return build_plan(pl, arena, bytes, lit_cap, build);
+}
+static int32_t scratch_arena(size_t need, uint8_t** arena, size_t* bytes) {
+    *arena = static_cast<uint8_t*>(dev_scratch(need));
+    *bytes = need;
+    return *arena ? LHB200_OK : LHB200_ENOMEM;
+}
+
+// Sort the ops by wave and upload literals and program (ops, wave table, byte items) through the pinned `h_stage`
+// (plan_stage_bytes).  The program blobs are allocated from the arena after everything else the plan holds; a plan
+// they would not fit is refused before any copy.
+static int32_t plan_upload(Plan& pl, cudaStream_t s, uint8_t* h_stage) {
+    const size_t prog = program_bytes(pl.ops.size(), pl.items.size());
+    if (pl.bump + prog > pl.arena_bytes) {
+        set_error("internal: plan exceeds its arena (%zu + %zu program bytes of %zu)", pl.bump, prog, pl.arena_bytes);
+        return LHB200_EINVAL;
     }
-    if (!ops_sorted.empty()) {
-        size_t nb = ops_sorted.size() * sizeof(HashOp);
+    uint8_t* h = h_stage;
+    if (!pl.lit.empty()) {
+        memcpy(h, pl.lit.data(), pl.lit.size());
+        LHB_CUDA(cudaMemcpyAsync(pl.arena + pl.lit_off, h, pl.lit.size(), cudaMemcpyHostToDevice, s));
+        h += align_up(pl.lit.size(), 256);
+    }
+    int nw = 0;
+    for (int w : pl.op_wave) nw = std::max(nw, w + 1);
+    pl.n_waves = nw;
+    pl.h_waves.assign(nw + 1, 0);   // h_waves[w]: first op of wave w (stable counting sort)
+    for (int w : pl.op_wave) pl.h_waves[w + 1]++;
+    for (int w = 0; w < nw; w++) pl.h_waves[w + 1] += pl.h_waves[w];
+    if (!pl.ops.empty()) {
+        const size_t nb = pl.ops.size() * sizeof(HashOp), wb = pl.h_waves.size() * sizeof(int32_t);
+        HashOp* h_ops = reinterpret_cast<HashOp*>(h);
+        std::vector<int32_t> next(pl.h_waves.begin(), pl.h_waves.end() - 1);
+        for (size_t i = 0; i < pl.ops.size(); i++) h_ops[next[pl.op_wave[i]]++] = pl.ops[i];
         pl.d_ops = reinterpret_cast<HashOp*>(pl.alloc(nb));
-        memcpy(h + o, ops_sorted.data(), nb);
-        LHB_CUDA(cudaMemcpyAsync(pl.d_ops, h + o, nb, cudaMemcpyHostToDevice, s));
-        o += align_up(nb, 256);
-        size_t wb = waves.size() * sizeof(int32_t);
+        LHB_CUDA(cudaMemcpyAsync(pl.d_ops, h, nb, cudaMemcpyHostToDevice, s));
+        h += align_up(nb, 256);
+        memcpy(h, pl.h_waves.data(), wb);
         pl.d_waves = reinterpret_cast<int32_t*>(pl.alloc(wb));
-        memcpy(h + o, waves.data(), wb);
-        LHB_CUDA(cudaMemcpyAsync(pl.d_waves, h + o, wb, cudaMemcpyHostToDevice, s));
-        o += align_up(wb, 256);
+        LHB_CUDA(cudaMemcpyAsync(pl.d_waves, h, wb, cudaMemcpyHostToDevice, s));
+        h += align_up(wb, 256);
     }
     if (!pl.items.empty()) {
-        size_t ib = pl.items.size() * sizeof(ByteItem);
+        const size_t ib = pl.items.size() * sizeof(ByteItem);
+        memcpy(h, pl.items.data(), ib);
         pl.d_items = reinterpret_cast<ByteItem*>(pl.alloc(ib));
-        memcpy(h + o, pl.items.data(), ib);
-        LHB_CUDA(cudaMemcpyAsync(pl.d_items, h + o, ib, cudaMemcpyHostToDevice, s));
+        LHB_CUDA(cudaMemcpyAsync(pl.d_items, h, ib, cudaMemcpyHostToDevice, s));
     }
+    return LHB200_OK;
+}
+
+// Host input of H2D copies.  Pinned host memory (and device memory) is read by the copy engine directly; pageable
+// memory is first bounced through the pinned slab, which then needs bounce_bytes() for it.
+struct HostInput {
+    const uint8_t* p;
+    size_t n;
+    bool direct;
+    HostInput(const uint8_t* p_, size_t n_, bool on_device = false) : p(p_), n(n_), direct(on_device || !n) {
+        cudaPointerAttributes at;
+        if (!direct) direct = cudaPointerGetAttributes(&at, p) == cudaSuccess && at.type == cudaMemoryTypeHost;
+        cudaGetLastError();
+    }
+    size_t bounce_bytes() const { return direct ? 0 : align_up(n, 256); }
+    const uint8_t* source(uint8_t* slab) const { return direct ? p : static_cast<const uint8_t*>(memcpy(slab, p, n)); }
+};
+
+// Copy a root operand to `dst` on s.  A zero-hash constant has no device address: it comes from the host table,
+// through the pinned `h32` (which may be `dst` itself).
+static int32_t read_root(uint64_t root, void* dst, cudaMemcpyKind kind, uint8_t* h32, cudaStream_t s) {
+    if (!(root & OP_ZERO_FLAG)) {
+        LHB_CUDA(cudaMemcpyAsync(dst, reinterpret_cast<const void*>(root), 32, kind, s));
+        return LHB200_OK;
+    }
+    memcpy(h32, ctx().zero_hashes[root & 0xff], 32);
+    if (dst != h32) LHB_CUDA(cudaMemcpyAsync(dst, h32, 32, cudaMemcpyHostToDevice, s));
     return LHB200_OK;
 }
 
 // Generic runner for "one input blob -> one root" host entry points.
-//   stage(plan, d_in) describes the work given the device copy of the input.
+//   describe(plan, d_in) describes the work given the device copy of the input and returns the root operand.
 template <class F>
 static int32_t run_simple(const uint8_t* h_in, size_t in_bytes, uint8_t out[32], F&& describe, bool in_on_device = false) {
     Ctx& c = ctx();
     std::lock_guard<std::recursive_mutex> g(c.mu);
-    // pass 1: dry run to size
-    Plan dry;
-    const size_t lit_cap = 4096;
-    size_t in_pad = align_up(in_bytes + 32, 256);
-    uint64_t root_dry = 0;
-    build_plan(dry, nullptr, 0, lit_cap, [&](Plan& p) {
-        uint8_t* d_in = p.alloc(in_pad);
-        root_dry = describe(p, d_in);
-    });
-    size_t prog_bytes = align_up(dry.ops.size() * sizeof(HashOp), 256) + align_up((dry.ops.size() + 2) * 4, 256) + 512;
-    size_t need = align_up(dry.bump, 256) + prog_bytes + 256;
-    uint8_t* arena = static_cast<uint8_t*>(dev_scratch(need));
-    if (!arena) return LHB200_ENOMEM;
-    size_t stage_bytes = in_bytes + lit_cap + prog_bytes + 1024;
-    uint8_t* hst = static_cast<uint8_t*>(pinned_scratch(stage_bytes));
-    if (!hst) return LHB200_ENOMEM;
-    Plan pl;
+    const size_t in_pad = align_up(in_bytes + 32, 256);
     uint64_t root = 0;
     uint8_t* d_in = nullptr;
-    int32_t rc = build_plan(pl, arena, need, lit_cap, [&](Plan& p) {
+    Plan pl;
+    int32_t rc = build_sized(pl, 4096, 256, [&](Plan& p) {
         d_in = p.alloc(in_pad);
         root = describe(p, d_in);
-    });
+        return LHB200_OK;
+    }, scratch_arena);
     if (rc) return rc;
+    const HostInput in(h_in, in_bytes, in_on_device);
+    const size_t ho = in.bounce_bytes(), hr = ho + align_up(plan_stage_bytes(pl), 256);
+    uint8_t* hst = static_cast<uint8_t*>(pinned_scratch(hr + 32));
+    if (!hst) return LHB200_ENOMEM;
     // H2D input (zero the padding tail so packed lists see zero-filled last chunks)
     LHB_CUDA(cudaMemsetAsync(d_in + in_bytes / 256 * 256, 0, in_pad - in_bytes / 256 * 256, c.stream));
-    if (in_bytes && in_on_device) {
-        LHB_CUDA(cudaMemcpyAsync(d_in, h_in, in_bytes, cudaMemcpyDeviceToDevice, c.stream));
-    } else if (in_bytes) {
-        cudaPointerAttributes at;
-        bool pinned = cudaPointerGetAttributes(&at, h_in) == cudaSuccess && at.type == cudaMemoryTypeHost;
-        cudaGetLastError();
-        const void* src = h_in;
-        if (!pinned) {
-            memcpy(hst, h_in, in_bytes);
-            src = hst;
-        }
-        LHB_CUDA(cudaMemcpyAsync(d_in, src, in_bytes, cudaMemcpyHostToDevice, c.stream));
-    }
-    std::vector<HashOp> ops_sorted;
-    std::vector<int32_t> waves;
-    plan_finalize_program(pl, ops_sorted, waves);
-    rc = plan_upload(pl, c.stream, ops_sorted, waves, hst + align_up(in_bytes, 256));
+    if (in_bytes) LHB_CUDA(cudaMemcpyAsync(d_in, in.source(hst), in_bytes, cudaMemcpyDefault, c.stream));
+    rc = plan_upload(pl, c.stream, hst + ho);
     if (rc) return rc;
     rc = plan_enqueue(pl, c.stream);
     if (rc) return rc;
-    if (root & OP_ZERO_FLAG) {
-        LHB_CUDA(cudaStreamSynchronize(c.stream));
-        memcpy(out, c.zero_hashes[root & 0xff], 32);
-        return LHB200_OK;
-    }
-    uint8_t* h_out = hst + stage_bytes - 64;
-    LHB_CUDA(cudaMemcpyAsync(h_out, reinterpret_cast<void*>(root), 32, cudaMemcpyDeviceToHost, c.stream));
+    rc = read_root(root, hst + hr, cudaMemcpyDeviceToHost, hst + hr, c.stream);
+    if (rc) return rc;
     LHB_CUDA(cudaStreamSynchronize(c.stream));
-    memcpy(out, h_out, 32);
+    memcpy(out, hst + hr, 32);
     return LHB200_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Deneb BeaconState (mainnet preset).  Fixed-part offsets: see DESIGN.md §3 / oracle for the derivation.
-namespace deneb {
+// BeaconState (mainnet preset): the fixed-part offsets every post-Altair fork shares, then the later forks' appended
+// fields.  See DESIGN.md §3 / oracle for the derivation.
+namespace state_layout {
 constexpr uint32_t O_GENESIS_TIME = 0, O_GVR = 8, O_SLOT = 40, O_FORK = 48, O_LBH = 64, O_BLOCK_ROOTS = 176,
                    O_STATE_ROOTS = 262320, O_HIST_OFF = 524464, O_ETH1_DATA = 524468, O_VOTES_OFF = 524540,
                    O_DEPOSIT_INDEX = 524544, O_VAL_OFF = 524552, O_BAL_OFF = 524556, O_RANDAO = 524560,
@@ -432,7 +464,7 @@ constexpr uint32_t O_GENESIS_TIME = 0, O_GVR = 8, O_SLOT = 40, O_FORK = 48, O_LB
                    O_NSC = 2712005, O_LEPH_OFF = 2736629, O_NWI = 2736633, O_NWVI = 2736641, O_HS_OFF = 2736649,
                    O_ELECTRA_U64 = 2736653, O_PBD_OFF = 2736701, O_PPW_OFF = 2736705, O_PC_OFF = 2736709;
 constexpr uint32_t SYNC_COMMITTEE_BYTES = 513 * 48;
-}  // namespace deneb
+}  // namespace state_layout
 
 static inline uint32_t rd32(const uint8_t* p) { return p[0] | (p[1] << 8) | (p[2] << 16) | ((uint32_t)p[3] << 24); }
 
@@ -481,11 +513,12 @@ struct lhb200_state {
     lhb200::Plan plan;
     uint64_t field_ops[40];   // MAX_FIELDS (declared below) rounded up
     uint64_t root_op = 0;
+    lhb200::HashOp* d_gather = nullptr;   // operand table: root_op, field_ops, then the sharded lists' local_op
     uint8_t* d_result = nullptr;  // (1 + MAX_FIELDS) * 32 bytes: root + field roots gathered
     cudaEvent_t e_k0 = nullptr, e_k1 = nullptr;  // around k_validator_roots
     lhb200::ShardCfg shard;
     std::vector<lhb200::ShardedList> sharded;
-    uint8_t* d_coll = nullptr;              // lhb200_state_root_sharded: gather ops | own subtree roots | all ranks' roots
+    uint8_t* d_coll = nullptr;              // lhb200_state_root_sharded: own subtree roots | all ranks' roots
     std::vector<lhb200::StageCopy> copies;  // SSZ ranges resident in the arena (for lhb200_state_patch)
     std::vector<uint32_t> copy_order, lit_order;   // offset-sorted indices into copies / plan.lit_src (patch lookups)
     std::vector<int32_t> copy_tree;         // copies[k] -> index of its resident tree (warm path), -1 if none
@@ -537,10 +570,9 @@ static bool fork_spec(int32_t fork, ForkSpec* f) {
     return false;
 }
 
-static int32_t describe_deneb(Plan& p, const uint8_t* s, uint64_t len, std::vector<StageCopy>* copies,
-                              uint64_t* field_ops, uint64_t* root_op, ShardCfg sh = ShardCfg(),
-                              std::vector<ShardedList>* sharded = nullptr) {
-    using namespace deneb;
+static int32_t describe_state(Plan& p, const uint8_t* s, uint64_t len, std::vector<StageCopy>* copies,
+                              uint64_t* field_ops, uint64_t* root_op, ShardCfg sh, std::vector<ShardedList>* sharded) {
+    using namespace state_layout;
     ForkSpec fk;
     if (!fork_spec(sh.fork, &fk)) { set_error("unknown fork id %d", sh.fork); return LHB200_EINVAL; }
     const uint32_t FIXED = fk.fixed;
@@ -583,20 +615,21 @@ static int32_t describe_deneb(Plan& p, const uint8_t* s, uint64_t len, std::vect
     uint64_t* f = field_ops;
     const uint32_t lg_world = ceil_log2(sh.world);
     // Big list with `n_chunks` leaf chunks produced from `n_items` source items of `item_bytes` at `src_off`
-    // (leaf_kind < 0: the bytes already are the chunks).  Unsharded: the full field root.  Sharded: this rank's subtree.
-    auto big_list = [&](int field, size_t src_off, uint64_t n_items, uint32_t item_bytes, int leaf_kind,
+    // (LEAF_NONE: the bytes already are the chunks).  Unsharded: the full field root.  Sharded: this rank's subtree.
+    auto big_list = [&](int field, size_t src_off, uint64_t n_items, uint32_t item_bytes, LeafKind leaf,
                         uint64_t n_chunks, uint32_t limit_depth, uint64_t mix_len) -> uint64_t {
         const uint32_t d0 = ceil_log2(std::max<uint64_t>(n_chunks, 1));
         const bool shard = sh.world > 1 && sharded && d0 >= lg_world + 6;
+        const bool validators = leaf.kernel == LeafKind::VALIDATORS, packed = leaf.kernel == LeafKind::NONE;
         if (!shard) {
             const uint8_t* src = place(src_off, n_items * item_bytes);
-            const uint8_t* chunks = leaf_kind >= 0 ? p.leaf_kernel(leaf_kind, src, n_items) : src;
+            const uint8_t* chunks = packed ? src : p.leaf_kernel(leaf, src, n_items);
             const size_t nt = p.trees.size();
             uint64_t r = p.merkle_list(chunks, n_chunks, limit_depth);
-            if (p.trees.size() > nt && leaf_kind <= 0) {   // warm-path provenance: validators (kind 0) or packed bytes
+            if (p.trees.size() > nt && (validators || packed)) {   // warm-path provenance
                 Plan::TreeSpec& t = p.trees.back();
-                t.src = src; t.kind = leaf_kind == 0 ? 0 : 1; t.src_off = src_off; t.src_bytes = n_items * item_bytes;
-                t.item_bytes = leaf_kind == 0 ? item_bytes : 32;
+                t.src = src; t.kind = validators ? 0 : 1; t.src_off = src_off; t.src_bytes = n_items * item_bytes;
+                t.item_bytes = validators ? item_bytes : 32;
             }
             return mix_len == UINT64_MAX ? r : p.mix_in_length(r, mix_len);
         }
@@ -605,9 +638,9 @@ static int32_t describe_deneb(Plan& p, const uint8_t* s, uint64_t len, std::vect
         const uint64_t c_hi = std::min<uint64_t>(n_chunks, ((uint64_t)sh.rank + 1) << sub);
         const uint64_t cnt = c_hi - c_lo;
         uint64_t op;
-        if (leaf_kind >= 0) {          // one chunk per source item
+        if (!packed) {                 // one chunk per source item
             const uint8_t* src = place(src_off + c_lo * item_bytes, cnt * item_bytes);
-            op = p.merkle_list(p.leaf_kernel(leaf_kind, src, cnt), cnt, sub);
+            op = p.merkle_list(p.leaf_kernel(leaf, src, cnt), cnt, sub);
         } else {                       // packed bytes: chunk c covers bytes [32c, 32c+32) of the field
             const uint64_t total_bytes = n_items * item_bytes;
             const uint64_t b_lo = c_lo * 32, b_hi = std::min<uint64_t>(total_bytes, c_hi * 32);
@@ -616,6 +649,10 @@ static int32_t describe_deneb(Plan& p, const uint8_t* s, uint64_t len, std::vect
         }
         sharded->push_back({field, sub, limit_depth, mix_len, op});
         return Plan::zero_op(0);       // placeholder; the field root is formed in lhb200_state_combine
+    };
+    // list of n fixed-size records (one leaf-kernel root each) with limit 2^depth
+    auto records = [&](LeafKind leaf, uint32_t off, uint64_t n, uint32_t item_bytes, uint32_t depth) {
+        return p.mix_in_length(p.merkle_list(p.leaf_kernel(leaf, place(off, n * item_bytes), n), n, depth), n);
     };
     f[0] = p.literal_bytes(s + O_GENESIS_TIME, 8);
     f[1] = chunk(O_GVR);
@@ -638,21 +675,21 @@ static int32_t describe_deneb(Plan& p, const uint8_t* s, uint64_t len, std::vect
     f[6] = plain_vector(O_STATE_ROOTS, 8192 * 32, 13);
     f[7] = p.mix_in_length(p.merkle_list(place(o_hist, n_hist * 32), n_hist, 24), n_hist);
     f[8] = p.container({chunk(O_ETH1_DATA), p.literal_bytes(s + O_ETH1_DATA + 32, 8), chunk(O_ETH1_DATA + 40)});
-    f[9] = p.mix_in_length(p.merkle_list(p.leaf_kernel(2, place(o_votes, n_votes * 72), n_votes), n_votes, 11), n_votes);
+    f[9] = records(LEAF_ETH1_DATA, o_votes, n_votes, 72, 11);
     f[10] = p.literal_bytes(s + O_DEPOSIT_INDEX, 8);
-    f[11] = big_list(11, o_val, n_val, 121, 0, n_val, 40, n_val);
-    f[12] = big_list(12, o_bal, n_bal, 8, -1, ceil_div(n_bal * 8, 32), 38, n_bal);
-    f[13] = big_list(13, O_RANDAO, 65536, 32, -1, 65536, 16, UINT64_MAX);
+    f[11] = big_list(11, o_val, n_val, 121, LEAF_VALIDATOR, n_val, 40, n_val);
+    f[12] = big_list(12, o_bal, n_bal, 8, LEAF_NONE, ceil_div(n_bal * 8, 32), 38, n_bal);
+    f[13] = big_list(13, O_RANDAO, 65536, 32, LEAF_NONE, 65536, 16, UINT64_MAX);
     f[14] = plain_vector(O_SLASHINGS, 8192 * 8, 11);
-    f[15] = big_list(15, o_pp, n_pp, 1, -1, ceil_div(n_pp, 32), 35, n_pp);
-    f[16] = big_list(16, o_cp, n_cp, 1, -1, ceil_div(n_cp, 32), 35, n_cp);
+    f[15] = big_list(15, o_pp, n_pp, 1, LEAF_NONE, ceil_div(n_pp, 32), 35, n_pp);
+    f[16] = big_list(16, o_cp, n_cp, 1, LEAF_NONE, ceil_div(n_cp, 32), 35, n_cp);
     f[17] = p.literal_bytes(s + O_JUST, 1);
     f[18] = p.container({p.literal_bytes(s + O_PJC, 8), chunk(O_PJC + 8)});
     f[19] = p.container({p.literal_bytes(s + O_CJC, 8), chunk(O_CJC + 8)});
     f[20] = p.container({p.literal_bytes(s + O_FC, 8), chunk(O_FC + 8)});
-    f[21] = big_list(21, o_inact, n_inact, 8, -1, ceil_div(n_inact * 8, 32), 38, n_inact);
+    f[21] = big_list(21, o_inact, n_inact, 8, LEAF_NONE, ceil_div(n_inact * 8, 32), 38, n_inact);
     for (int k = 0; k < 2; k++) {
-        uint8_t* roots = p.leaf_kernel(1, place(k ? O_NSC : O_CSC, SYNC_COMMITTEE_BYTES), 513);
+        uint8_t* roots = p.leaf_kernel(LEAF_PUBKEY, place(k ? O_NSC : O_CSC, SYNC_COMMITTEE_BYTES), 513);
         f[22 + k] = p.container({p.merkle_list(roots, 512, 9), reinterpret_cast<uint64_t>(roots + 512 * 32)});
     }
     if (fk.hdr_fields) {
@@ -673,13 +710,13 @@ static int32_t describe_deneb(Plan& p, const uint8_t* s, uint64_t len, std::vect
     if (fk.n_fields >= 28) {
         f[25] = p.literal_bytes(s + O_NWI, 8);
         f[26] = p.literal_bytes(s + O_NWVI, 8);
-        f[27] = p.mix_in_length(p.merkle_list(p.leaf_kernel(3, place(o_hs, n_hs * 64), n_hs), n_hs, 24), n_hs);
+        f[27] = records(LEAF_CHUNK_PAIR, o_hs, n_hs, 64, 24);
     }
     if (electra) {   // beacon_state.rs:487-525
         for (int k = 0; k < 6; k++) f[28 + k] = p.literal_bytes(s + O_ELECTRA_U64 + 8 * k, 8);
-        f[34] = p.mix_in_length(p.merkle_list(p.leaf_kernel(4, place(o_pbd, n_pbd * 16), n_pbd), n_pbd, 27), n_pbd);
-        f[35] = p.mix_in_length(p.merkle_list(p.leaf_kernel(5, place(o_ppw, n_ppw * 24), n_ppw), n_ppw, 27), n_ppw);
-        f[36] = p.mix_in_length(p.merkle_list(p.leaf_kernel(4, place(o_pc, n_pc * 16), n_pc), n_pc, 18), n_pc);
+        f[34] = records(LEAF_U64_PAIR, o_pbd, n_pbd, 16, 27);
+        f[35] = records(LEAF_U64_TRIPLE, o_ppw, n_ppw, 24, 27);
+        f[36] = records(LEAF_U64_PAIR, o_pc, n_pc, 16, 18);
     }
     for (int k = fk.n_fields; k < MAX_FIELDS; k++) f[k] = Plan::zero_op(0);   // absent in this fork (not part of its container)
     *root_op = p.container(std::vector<uint64_t>(f, f + fk.n_fields));
@@ -692,6 +729,74 @@ __global__ void k_gather_nodes(const HashOp* __restrict__ srcs, int n, uint8_t* 
     uint32_t w[8];
     load_operand(srcs[i].a, w);
     store_chunk(out + 32 * i, w);
+}
+
+// Operand table of k_gather_nodes, staged through the pinned `h` (n * sizeof(HashOp) bytes).
+static int32_t stage_operands(const std::vector<uint64_t>& operands, HashOp* d_tab, uint8_t* h, cudaStream_t s) {
+    HashOp* tab = reinterpret_cast<HashOp*>(h);
+    for (size_t i = 0; i < operands.size(); i++) tab[i] = {0, operands[i], 0};
+    LHB_CUDA(cudaMemcpyAsync(d_tab, tab, operands.size() * sizeof(HashOp), cudaMemcpyHostToDevice, s));
+    return LHB200_OK;
+}
+// The n operands a staged table lists -> n contiguous chunks at `out`.
+static int32_t gather_operands(const HashOp* d_tab, uint32_t n, uint8_t* out, cudaStream_t s) {
+    k_gather_nodes<<<(unsigned)ceil_div(n, 64), 64, 0, s>>>(d_tab, (int)n, out);
+    count_launch();
+    LHB_CUDA(cudaGetLastError());
+    return LHB200_OK;
+}
+
+// The resident parts [a, b) of SSZ bytes [lo, hi) of a staged state: on_copy(copy index, a, b) for staged copies,
+// on_lit(literal source, a, b) for literal chunks, each returning whether to go on; returns whether there were any.
+// Each kind is found by binary search over offset-sorted indices: O(log fields) per edit, so a slot's worth of
+// mutations (tens of thousands of 8-byte edits) costs the host well under a millisecond.  `hint`, the copy of the
+// previous edit, is tried first.
+template <class C, class L>
+static bool visit_resident(const lhb200_state* st, uint64_t lo, uint64_t hi, size_t& hint, C&& on_copy, L&& on_lit) {
+    bool any = false;
+    const std::vector<uint32_t>& co = st->copy_order;
+    auto before = [&](uint32_t ci) { return st->copies[ci].src_off + st->copies[ci].nbytes <= lo; };
+    size_t k = hint < co.size() && st->copies[co[hint]].src_off <= lo && !before(co[hint])
+                   ? hint : std::partition_point(co.begin(), co.end(), before) - co.begin();
+    for (hint = k; k < co.size() && st->copies[co[k]].src_off < hi; k++) {
+        const StageCopy& cp = st->copies[co[k]];
+        const uint64_t a = std::max<uint64_t>(lo, cp.src_off), b = std::min<uint64_t>(hi, cp.src_off + cp.nbytes);
+        if (a >= b) continue;
+        any = true;
+        if (!on_copy(co[k], a, b)) return true;
+    }
+    const std::vector<Plan::LitSrc>& ls = st->plan.lit_src;
+    const std::vector<uint32_t>& lo_order = st->lit_order;
+    size_t m = std::partition_point(lo_order.begin(), lo_order.end(),
+                                    [&](uint32_t li) { return ls[li].src_off + ls[li].n <= lo; }) - lo_order.begin();
+    for (; m < lo_order.size() && ls[lo_order[m]].src_off < hi; m++) {
+        const Plan::LitSrc& l = ls[lo_order[m]];
+        const uint64_t a = std::max<uint64_t>(lo, l.src_off), b = std::min<uint64_t>(hi, l.src_off + l.n);
+        if (a >= b) continue;
+        any = true;
+        if (!on_lit(l, a, b)) return true;
+    }
+    return any;
+}
+// Offset order of a handle's copies and literals (built once), and copy_tree (trees appear with enable_incremental).
+static void index_resident(lhb200_state* st) {
+    if (st->copy_order.empty() && !st->copies.empty()) {
+        st->copy_order.resize(st->copies.size());
+        for (size_t k = 0; k < st->copies.size(); k++) st->copy_order[k] = (uint32_t)k;
+        std::sort(st->copy_order.begin(), st->copy_order.end(),
+                  [&](uint32_t a, uint32_t b) { return st->copies[a].src_off < st->copies[b].src_off; });
+        const std::vector<Plan::LitSrc>& ls = st->plan.lit_src;
+        st->lit_order.resize(ls.size());
+        for (size_t k = 0; k < ls.size(); k++) st->lit_order[k] = (uint32_t)k;
+        std::sort(st->lit_order.begin(), st->lit_order.end(),
+                  [&](uint32_t a, uint32_t b) { return ls[a].src_off < ls[b].src_off; });
+    }
+    if (st->copy_tree.size() == st->copies.size() && st->copy_tree_trees == st->trees.size()) return;
+    st->copy_tree.assign(st->copies.size(), -1);
+    for (size_t k = 0; k < st->copies.size(); k++)
+        for (size_t t = 0; t < st->trees.size(); t++)
+            if (st->trees[t].src_off == st->copies[k].src_off) st->copy_tree[k] = (int32_t)t;
+    st->copy_tree_trees = st->trees.size();
 }
 
 }  // namespace lhb200
@@ -756,31 +861,22 @@ int32_t lhb200_dev_merkleize(const void* d_chunks, uint64_t n_chunks, uint32_t d
     Ctx& c = ctx();
     std::lock_guard<std::recursive_mutex> g(c.mu);
     cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c.stream;
-    Plan dry;
     uint64_t root = 0;
-    auto describe = [&](Plan& p) { root = p.merkle_list(static_cast<const uint8_t*>(d_chunks), n_chunks, depth); };
-    build_plan(dry, nullptr, 0, 256, describe);
-    size_t prog = align_up(dry.ops.size() * sizeof(HashOp), 256) + align_up((dry.ops.size() + 2) * 4, 256) + 512;
-    size_t need = align_up(dry.bump, 256) + prog + 256;
-    uint8_t* arena = static_cast<uint8_t*>(dev_scratch(need));
-    uint8_t* hst = static_cast<uint8_t*>(pinned_scratch(prog + 1024));
-    if (!arena || !hst) return LHB200_ENOMEM;
     Plan pl;
-    int32_t rc = build_plan(pl, arena, need, 256, describe);
+    int32_t rc = build_sized(pl, 256, 256, [&](Plan& p) {
+        root = p.merkle_list(static_cast<const uint8_t*>(d_chunks), n_chunks, depth);
+        return LHB200_OK;
+    }, scratch_arena);
     if (rc) return rc;
-    std::vector<HashOp> ops_sorted;
-    std::vector<int32_t> waves;
-    plan_finalize_program(pl, ops_sorted, waves);
-    rc = plan_upload(pl, s, ops_sorted, waves, hst);
+    const size_t hr = align_up(plan_stage_bytes(pl), 256);
+    uint8_t* hst = static_cast<uint8_t*>(pinned_scratch(hr + 32));
+    if (!hst) return LHB200_ENOMEM;
+    rc = plan_upload(pl, s, hst);
     if (rc) return rc;
     rc = plan_enqueue(pl, s);
     if (rc) return rc;
-    if (root & OP_ZERO_FLAG) {
-        memcpy(hst + prog, c.zero_hashes[root & 0xff], 32);
-        LHB_CUDA(cudaMemcpyAsync(d_out32, hst + prog, 32, cudaMemcpyHostToDevice, s));
-    } else {
-        LHB_CUDA(cudaMemcpyAsync(d_out32, reinterpret_cast<void*>(root), 32, cudaMemcpyDeviceToDevice, s));
-    }
+    rc = read_root(root, d_out32, cudaMemcpyDeviceToDevice, hst + hr, s);
+    if (rc) return rc;
     // the scratch arena and pinned staging are reused by the next call: finish before returning
     LHB_CUDA(cudaStreamSynchronize(s));
     return LHB200_OK;
@@ -805,7 +901,7 @@ int32_t lhb200_validators_root(const uint8_t* ssz, uint64_t n, uint8_t out[32]) 
     LHB_REQUIRE_READY();
     if (!out || (n && !ssz) || n > (1ull << 40)) return LHB200_EINVAL;
     return run_simple(ssz, n * 121, out, [&](Plan& p, uint8_t* d_in) {
-        return p.mix_in_length(p.merkle_list(p.leaf_kernel(0, d_in, n), n, 40), n);
+        return p.mix_in_length(p.merkle_list(p.leaf_kernel(LEAF_VALIDATOR, d_in, n), n, 40), n);
     });
 }
 
@@ -830,7 +926,7 @@ int32_t lhb200_validator_roots(const uint8_t* ssz, uint64_t n, uint8_t* out_root
     return LHB200_OK;
 }
 
-static int32_t stage_deneb(const uint8_t* ssz, uint64_t len, ShardCfg sh, lhb200_state** out) {
+static int32_t stage_state(const uint8_t* ssz, uint64_t len, ShardCfg sh, lhb200_state** out) {
     LHB_REQUIRE_READY();
     if (!ssz || !out) return LHB200_EINVAL;
     if (sh.world == 0 || (sh.world & (sh.world - 1)) || sh.rank >= sh.world) {
@@ -839,83 +935,67 @@ static int32_t stage_deneb(const uint8_t* ssz, uint64_t len, ShardCfg sh, lhb200
     }
     Ctx& c = ctx();
     std::lock_guard<std::recursive_mutex> g(c.mu);
-    const size_t lit_cap = 16384;
-    Plan dry;
-    uint64_t fops[MAX_FIELDS], rop;
-    int32_t rc = LHB200_OK;
-    std::vector<ShardedList> dry_sh;
-    build_plan(dry, nullptr, 0, lit_cap, [&](Plan& p) { rc = describe_deneb(p, ssz, len, nullptr, fops, &rop, sh, &dry_sh); });
-    if (rc) return rc;
-    size_t prog = align_up(dry.ops.size() * sizeof(HashOp), 256) + align_up((dry.ops.size() + 2) * 4, 256) + 512;
-    size_t need = align_up(dry.bump, 256) + prog + (1 + MAX_FIELDS) * 32 + (1 + MAX_FIELDS) * sizeof(HashOp) + 1024;
-    std::unique_ptr<lhb200_state> st(new lhb200_state());
-    if (g_spare_arena && g_spare_bytes >= need) {       // recycled from the last released handle (no cudaMalloc)
-        st->arena = g_spare_arena;
-        st->arena_bytes = g_spare_bytes;
-        g_spare_arena = nullptr;
-        g_spare_bytes = 0;
-    } else {
-        LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->arena), need + (need >> 3)));
-        st->arena_bytes = need + (need >> 3);
-    }
-    std::vector<StageCopy> copies;
-    rc = build_plan(st->plan, st->arena, st->arena_bytes, lit_cap, [&](Plan& p) {
-        st->sharded.clear();
-        rc = describe_deneb(p, ssz, len, &copies, st->field_ops, &st->root_op, sh, &st->sharded);
-    });
+    // a failure releases the handle, which keeps the arena it took as the spare for the next stage call
+    std::unique_ptr<lhb200_state, int32_t (*)(lhb200_state*)> st(new lhb200_state(), lhb200_state_release);
     st->shard = sh;
-    if (rc) { cudaFree(st->arena); return rc; }
-    st->copies = copies;
+    constexpr size_t n_result = 1 + MAX_FIELDS;
+    int32_t rc = build_sized(st->plan, 16384, n_result * 32 + n_result * sizeof(HashOp) + 1024, [&](Plan& p) {
+        st->copies.clear();
+        st->sharded.clear();
+        return describe_state(p, ssz, len, &st->copies, st->field_ops, &st->root_op, sh, &st->sharded);
+    }, [&](size_t need, uint8_t** arena, size_t* bytes) {
+        if (g_spare_arena && g_spare_bytes >= need) {   // recycled from the last released handle (no cudaMalloc)
+            st->arena = g_spare_arena;
+            st->arena_bytes = g_spare_bytes;
+            g_spare_arena = nullptr;
+            g_spare_bytes = 0;
+        } else {
+            uint8_t* a = nullptr;
+            LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&a), need + (need >> 3)));
+            st->arena = a;
+            st->arena_bytes = need + (need >> 3);
+        }
+        *arena = st->arena;
+        *bytes = st->arena_bytes;
+        return LHB200_OK;
+    });
+    if (rc) return rc;
     st->plan.ssz_base = nullptr;  // the caller's buffer is not retained
-    // H2D: per-field copies into the aligned layout.  Pinned caller memory goes straight to the copy engine;
-    // pageable memory is bounced through the pinned staging slab.
-    cudaPointerAttributes at;
-    bool pinned = cudaPointerGetAttributes(&at, ssz) == cudaSuccess && at.type == cudaMemoryTypeHost;
-    cudaGetLastError();
-    const uint8_t* src = ssz;
-    std::vector<HashOp> ops_sorted;
-    std::vector<int32_t> waves;
-    plan_finalize_program(st->plan, ops_sorted, waves);
-    size_t stage_bytes = (pinned ? 0 : len) + lit_cap + prog + (1 + MAX_FIELDS) * sizeof(HashOp) + 2048;
-    uint8_t* hst = static_cast<uint8_t*>(pinned_scratch(stage_bytes));
-    if (!hst) { cudaFree(st->arena); return LHB200_ENOMEM; }
-    size_t ho = 0;
-    if (!pinned) {
-        memcpy(hst, ssz, len);
-        src = hst;
-        ho = align_up(len, 256);
-    }
-    for (const StageCopy& cp : copies) {
+    // allocated before the program blobs, so that plan_upload's arena check covers them too
+    std::vector<uint64_t> gather(1, st->root_op);   // root + field roots -> contiguous result block
+    gather.insert(gather.end(), st->field_ops, st->field_ops + MAX_FIELDS);
+    for (const ShardedList& L : st->sharded) gather.push_back(L.local_op);
+    st->d_gather = reinterpret_cast<HashOp*>(st->plan.alloc(gather.size() * sizeof(HashOp)));
+    st->d_result = st->plan.alloc(n_result * 32);
+    const HostInput in(ssz, len);
+    const size_t hp = in.bounce_bytes(), hg = hp + align_up(plan_stage_bytes(st->plan), 256);
+    uint8_t* hst = static_cast<uint8_t*>(pinned_scratch(hg + gather.size() * sizeof(HashOp)));
+    if (!hst) return LHB200_ENOMEM;
+    // H2D: per-field copies into the aligned layout
+    const uint8_t* src = in.source(hst);
+    for (const StageCopy& cp : st->copies) {
         size_t z0 = cp.nbytes / 256 * 256;
         LHB_CUDA(cudaMemsetAsync(cp.dst + z0, 0, cp.pad_to - z0, c.stream));
         if (cp.nbytes)
             LHB_CUDA(cudaMemcpyAsync(cp.dst, src + cp.src_off, cp.nbytes, cudaMemcpyHostToDevice, c.stream));
     }
-    rc = plan_upload(st->plan, c.stream, ops_sorted, waves, hst + ho);
-    if (rc) { cudaFree(st->arena); return rc; }
-    // gather table: root + field roots -> contiguous result block
-    HashOp gath[1 + MAX_FIELDS];
-    gath[0] = {0, st->root_op, 0};
-    for (int i = 0; i < MAX_FIELDS; i++) gath[i + 1] = {0, st->field_ops[i], 0};
-    uint8_t* h_g = hst + stage_bytes - (1 + MAX_FIELDS) * sizeof(HashOp) - 64;
-    memcpy(h_g, gath, sizeof gath);
-    uint8_t* d_g = st->plan.alloc(sizeof gath);
-    st->d_result = st->plan.alloc((1 + MAX_FIELDS) * 32);
-    LHB_CUDA(cudaMemcpyAsync(d_g, h_g, sizeof gath, cudaMemcpyHostToDevice, c.stream));
-    st->plan.root_addr = reinterpret_cast<uint64_t>(d_g);
+    rc = plan_upload(st->plan, c.stream, hst + hp);
+    if (rc) return rc;
+    rc = stage_operands(gather, st->d_gather, hst + hg, c.stream);
+    if (rc) return rc;
     LHB_CUDA(cudaStreamSynchronize(c.stream));
     *out = st.release();
     return LHB200_OK;
 }
 
 int32_t lhb200_state_stage_deneb(const uint8_t* ssz, uint64_t len, lhb200_state** out) {
-    return stage_deneb(ssz, len, ShardCfg(), out);
+    return stage_state(ssz, len, ShardCfg(), out);
 }
 // Same for any post-Altair fork (LHB200_FORK_*): the describer is table-driven, the kernels are shared.
 int32_t lhb200_state_stage(const uint8_t* ssz, uint64_t len, int32_t fork, lhb200_state** out) {
     ShardCfg sh;
     sh.fork = fork;
-    return stage_deneb(ssz, len, sh, out);
+    return stage_state(ssz, len, sh, out);
 }
 
 int32_t lhb200_state_stage_deneb_shard(const uint8_t* ssz, uint64_t len, uint32_t rank, uint32_t world,
@@ -923,7 +1003,7 @@ int32_t lhb200_state_stage_deneb_shard(const uint8_t* ssz, uint64_t len, uint32_
     ShardCfg sh;
     sh.rank = rank;
     sh.world = world;
-    return stage_deneb(ssz, len, sh, out);
+    return stage_state(ssz, len, sh, out);
 }
 
 // Run this rank's part and return the subtree roots of the sharded lists (n_lists x 32 bytes, fixed list order).
@@ -937,17 +1017,11 @@ int32_t lhb200_state_shard_roots(lhb200_state* st, uint8_t* out, uint32_t* n_lis
     const uint32_t n = (uint32_t)st->sharded.size();
     *n_lists = n;
     if (n == 0) { LHB_CUDA(cudaStreamSynchronize(c.stream)); return LHB200_OK; }
-    std::vector<HashOp> gath(n);
-    for (uint32_t i = 0; i < n; i++) gath[i] = {0, st->sharded[i].local_op, 0};
-    uint8_t* h = static_cast<uint8_t*>(pinned_scratch(n * sizeof(HashOp) + n * 32 + 512));
-    uint8_t* d = static_cast<uint8_t*>(dev_scratch(n * sizeof(HashOp) + n * 32 + 512));
-    if (!h || !d) return LHB200_ENOMEM;
-    memcpy(h, gath.data(), n * sizeof(HashOp));
-    uint8_t* d_res = d + ((n * sizeof(HashOp) + 255) / 256) * 256;
-    LHB_CUDA(cudaMemcpyAsync(d, h, n * sizeof(HashOp), cudaMemcpyHostToDevice, c.stream));
-    k_gather_nodes<<<1, 32, 0, c.stream>>>(reinterpret_cast<const HashOp*>(d), (int)n, d_res);
-    count_launch();
-    uint8_t* h_res = h + ((n * sizeof(HashOp) + 255) / 256) * 256;
+    uint8_t* h_res = static_cast<uint8_t*>(pinned_scratch(n * 32));
+    uint8_t* d_res = static_cast<uint8_t*>(dev_scratch(n * 32));
+    if (!h_res || !d_res) return LHB200_ENOMEM;
+    rc = gather_operands(st->d_gather + 1 + MAX_FIELDS, n, d_res, c.stream);
+    if (rc) return rc;
     LHB_CUDA(cudaMemcpyAsync(h_res, d_res, n * 32, cudaMemcpyDeviceToHost, c.stream));
     LHB_CUDA(cudaStreamSynchronize(c.stream));
     memcpy(out, h_res, n * 32);
@@ -995,21 +1069,13 @@ int32_t lhb200_state_root_sharded(lhb200_state* st, uint8_t out[32]) {
     int32_t rc = lhb200_state_root_enqueue(st, c.stream, nullptr);
     if (rc) return rc;
     if (n == 0) { set_error("handle is not sharded"); return LHB200_EINVAL; }
-    std::vector<HashOp> gath(n);
-    for (uint32_t i = 0; i < n; i++) gath[i] = {0, st->sharded[i].local_op, 0};
-    if (!st->d_coll) {   // [gather ops | my roots | all roots], owned by the handle (dev_scratch is reused by the combine)
-        LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_coll), 4096 + (size_t)(world + 1) * n * 32 + 512));
+    if (!st->d_coll) {   // owned by the handle: dev_scratch is reused by the combine
+        LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_coll), (size_t)(world + 1) * n * 32 + 512));
     }
-    uint8_t* h = static_cast<uint8_t*>(pinned_scratch(n * sizeof(HashOp) + 512));
-    if (!h) return LHB200_ENOMEM;
-    memcpy(h, gath.data(), n * sizeof(HashOp));
-    uint8_t* d_ops = st->d_coll;
-    uint8_t* d_mine = st->d_coll + 4096;
-    uint8_t* d_all = d_mine + ((n * 32 + 255) / 256) * 256;
-    if (n * sizeof(HashOp) > 4096) return LHB200_EINVAL;
-    LHB_CUDA(cudaMemcpyAsync(d_ops, h, n * sizeof(HashOp), cudaMemcpyHostToDevice, c.stream));
-    k_gather_nodes<<<1, 32, 0, c.stream>>>(reinterpret_cast<const HashOp*>(d_ops), (int)n, d_mine);
-    count_launch();
+    uint8_t* d_mine = st->d_coll;
+    uint8_t* d_all = d_mine + align_up(n * 32, 256);
+    rc = gather_operands(st->d_gather + 1 + MAX_FIELDS, n, d_mine, c.stream);
+    if (rc) return rc;
     rc = comm_allgather_bytes(d_mine, d_all, (size_t)n * 32, c.stream);
     if (rc) return rc;
     return state_combine_impl(st, d_all, out, true);
@@ -1034,109 +1100,41 @@ int32_t lhb200_state_patch_batch(lhb200_state* st, const uint64_t* offsets, cons
     std::vector<ScatterOp> ops;
     ops.reserve(n);
     Plan& pl = st->plan;
-    uint64_t blob_off = 0;
     uint32_t lit_lo = ~0u, lit_hi = 0;
-    // Range lookups by binary search over offset-sorted indices (built once per handle): O(log fields) per edit, so a
-    // slot's worth of mutations (tens of thousands of 8-byte edits) costs the host well under a millisecond.
-    if (st->copy_order.empty() && !st->copies.empty()) {
-        st->copy_order.resize(st->copies.size());
-        for (size_t k = 0; k < st->copies.size(); k++) st->copy_order[k] = (uint32_t)k;
-        std::sort(st->copy_order.begin(), st->copy_order.end(),
-                  [&](uint32_t a, uint32_t b) { return st->copies[a].src_off < st->copies[b].src_off; });
-        st->copy_tree.assign(st->copies.size(), -1);
-        for (size_t k = 0; k < st->copies.size(); k++)
-            for (size_t t = 0; t < st->trees.size(); t++)
-                if (st->trees[t].src_off == st->copies[k].src_off) st->copy_tree[k] = (int32_t)t;
-        st->lit_order.resize(pl.lit_src.size());
-        for (size_t k = 0; k < pl.lit_src.size(); k++) st->lit_order[k] = (uint32_t)k;
-        std::sort(st->lit_order.begin(), st->lit_order.end(),
-                  [&](uint32_t a, uint32_t b) { return pl.lit_src[a].src_off < pl.lit_src[b].src_off; });
-    }
-    if (st->incremental && st->copy_tree_trees != st->trees.size()) {   // trees appear with enable_incremental
-        for (size_t k = 0; k < st->copies.size(); k++) {
-            st->copy_tree[k] = -1;
-            for (size_t t = 0; t < st->trees.size(); t++)
-                if (st->trees[t].src_off == st->copies[k].src_off) st->copy_tree[k] = (int32_t)t;
-        }
-        st->copy_tree_trees = st->trees.size();
-    }
+    index_resident(st);
     // pass 1: every edit must hit resident bytes — validated BEFORE anything is modified, so a rejected batch leaves the
     // handle (host literals, dirty lists, device copy) exactly as it was
-    size_t hit = ~(size_t)0;
+    auto stop = [](auto&&...) { return false; };
+    size_t hint = ~(size_t)0;
     for (uint32_t i = 0; i < n; i++) {
         const uint64_t lo = offsets[i], hi = lo + lens[i];
-        if (lens[i] == 0) continue;
-        bool touched = false;
-        if (hit < st->copy_order.size() && st->copies[st->copy_order[hit]].src_off <= lo &&
-            hi <= st->copies[st->copy_order[hit]].src_off + st->copies[st->copy_order[hit]].nbytes) continue;   // same field as the last edit
-        size_t k = std::partition_point(st->copy_order.begin(), st->copy_order.end(), [&](uint32_t ci) {
-                       const StageCopy& cp = st->copies[ci];
-                       return cp.src_off + cp.nbytes <= lo;
-                   }) - st->copy_order.begin();
-        if (k < st->copy_order.size() && st->copies[st->copy_order[k]].src_off < hi) { touched = true; hit = k; }
-        if (!touched) {
-            size_t m = std::partition_point(st->lit_order.begin(), st->lit_order.end(), [&](uint32_t li) {
-                           const Plan::LitSrc& ls = pl.lit_src[li];
-                           return ls.src_off + ls.n <= lo;
-                       }) - st->lit_order.begin();
-            if (m < st->lit_order.size() && pl.lit_src[st->lit_order[m]].src_off < hi) touched = true;
-        }
-        if (!touched) {
+        if (lens[i] && !visit_resident(st, lo, hi, hint, stop, stop)) {
             set_error("state_patch: range [%llu, %llu) is not resident on this handle (offset table or another rank's shard)",
                       (unsigned long long)lo, (unsigned long long)hi);
             return LHB200_EINVAL;
         }
     }
-    size_t last_k = ~(size_t)0;
+    uint64_t blob_off = 0;
     for (uint32_t i = 0; i < n; i++) {
         const uint64_t lo = offsets[i], hi = lo + lens[i];
         const uint8_t* src = data + blob_off;
-        bool touched = lens[i] == 0;
-        // first resident range whose end lies beyond lo (consecutive edits usually hit the same field: try it first)
-        size_t k = last_k;
-        if (!(k < st->copy_order.size() && st->copies[st->copy_order[k]].src_off <= lo &&
-              lo < st->copies[st->copy_order[k]].src_off + st->copies[st->copy_order[k]].nbytes))
-            k = std::partition_point(st->copy_order.begin(), st->copy_order.end(), [&](uint32_t ci) {
-                    const StageCopy& cp = st->copies[ci];
-                    return cp.src_off + cp.nbytes <= lo;
-                }) - st->copy_order.begin();
-        last_k = k;
-        for (; k < st->copy_order.size(); k++) {
-            const uint32_t ci = st->copy_order[k];
+        visit_resident(st, lo, hi, hint, [&](uint32_t ci, uint64_t a, uint64_t b) {
             const StageCopy& cp = st->copies[ci];
-            if (cp.src_off >= hi) break;
-            const uint64_t a = std::max<uint64_t>(lo, cp.src_off), b = std::min<uint64_t>(hi, cp.src_off + cp.nbytes);
-            if (a >= b) continue;
             ops.push_back({cp.dst + (a - cp.src_off), (uint32_t)(b - a), (uint32_t)(blob_off + (a - lo))});
-            touched = true;
-            if (st->incremental && !st->need_full) {   // warm path: which leaves of which tree does this touch?
-                const int32_t ti = st->copy_tree[ci];
-                if (ti < 0) { st->need_full = true; continue; }   // a list without a resident tree (votes, summaries, ...)
-                lhb200_state::Tree& t = st->trees[ti];
-                const uint64_t i0 = (a - t.src_off) / t.item_bytes, i1 = (b - 1 - t.src_off) / t.item_bytes;
-                if (t.n_marks + (i1 - i0 + 1) > 4ull * lhb200_state::DIRTY_CAP) { st->need_full = true; continue; }
-                for (uint64_t q = i0; q <= i1; q++) t.mark(q);
-            }
-        }
-        size_t m = std::partition_point(st->lit_order.begin(), st->lit_order.end(), [&](uint32_t li) {
-                       const Plan::LitSrc& ls = pl.lit_src[li];
-                       return ls.src_off + ls.n <= lo;
-                   }) - st->lit_order.begin();
-        for (; m < st->lit_order.size(); m++) {          // small fixed fields live in host-packed literal chunks
-            const Plan::LitSrc& ls = pl.lit_src[st->lit_order[m]];
-            if (ls.src_off >= hi) break;
-            const uint64_t a = std::max<uint64_t>(lo, ls.src_off), b = std::min<uint64_t>(hi, ls.src_off + ls.n);
-            if (a >= b) continue;
+            if (!st->incremental || st->need_full) return true;   // warm path: which leaves of which tree does this touch?
+            const int32_t ti = st->copy_tree[ci];
+            if (ti < 0) { st->need_full = true; return true; }     // a list without a resident tree (votes, summaries, ...)
+            lhb200_state::Tree& t = st->trees[ti];
+            const uint64_t i0 = (a - t.src_off) / t.item_bytes, i1 = (b - 1 - t.src_off) / t.item_bytes;
+            if (t.n_marks + (i1 - i0 + 1) > 4ull * lhb200_state::DIRTY_CAP) { st->need_full = true; return true; }
+            for (uint64_t q = i0; q <= i1; q++) t.mark(q);
+            return true;
+        }, [&](const Plan::LitSrc& ls, uint64_t a, uint64_t b) {   // small fixed fields live in host-packed literal chunks
             memcpy(&pl.lit[(size_t)ls.lit_index * 32] + (a - ls.src_off), src + (a - lo), b - a);
             lit_lo = std::min(lit_lo, ls.lit_index);
             lit_hi = std::max(lit_hi, ls.lit_index + 1);
-            touched = true;
-        }
-        if (!touched) {
-            set_error("state_patch: range [%llu, %llu) is not resident on this handle (offset table or another rank's shard)",
-                      (unsigned long long)lo, (unsigned long long)hi);
-            return LHB200_EINVAL;
-        }
+            return true;
+        });
         blob_off += lens[i];
     }
     const size_t ob = align_up(ops.size() * sizeof(ScatterOp), 256), bb = align_up(total + 16, 256);
@@ -1311,9 +1309,8 @@ int32_t lhb200_state_root_enqueue(lhb200_state* st, void* stream, const void** d
         if (!rc && st->incremental) rc = state_build_levels(st, s);   // a cold root leaves the level arrays stale
     }
     if (rc) return rc;
-    k_gather_nodes<<<1, 64, 0, s>>>(reinterpret_cast<const HashOp*>(st->plan.root_addr), 1 + MAX_FIELDS, st->d_result);
-    count_launch();
-    LHB_CUDA(cudaGetLastError());
+    rc = gather_operands(st->d_gather, 1 + MAX_FIELDS, st->d_result, s);
+    if (rc) return rc;
     if (d_root) *d_root = st->d_result;
     return LHB200_OK;
 }
@@ -1410,9 +1407,6 @@ int32_t lhb200_merkle_tree_proof(const uint8_t* leaves, uint64_t n, uint32_t dep
         off += align_up(std::max<uint64_t>(cnt[l], 1) * 32, 256);
     }
     for (uint32_t l = 0; l < depth && cnt[l] > 0; l++) {
-        if (cnt[l] == 1 && l > 0 && cnt[l + 1] == 1) {
-            // lone node climbing a zero ladder: still one hash per level
-        }
         MerkleSegTable tab;
         tab.n = 1;
         tab.s[0].in = lvl[l]; tab.s[0].out = lvl[l + 1]; tab.s[0].n_in = cnt[l]; tab.s[0].level_in = l;
@@ -1421,21 +1415,20 @@ int32_t lhb200_merkle_tree_proof(const uint8_t* leaves, uint64_t n, uint32_t dep
         count_launch();
     }
     LHB_CUDA(cudaGetLastError());
-    std::vector<HashOp> gath(depth + 1);
-    gath[0] = {0, n ? reinterpret_cast<uint64_t>(lvl[depth]) : (OP_ZERO_FLAG | depth), 0};
+    std::vector<uint64_t> ops(depth + 1);
+    ops[0] = n ? reinterpret_cast<uint64_t>(lvl[depth]) : (OP_ZERO_FLAG | depth);
     uint64_t idx = index;
     for (uint32_t l = 0; l < depth; l++) {
         uint64_t sib = idx ^ 1;
-        gath[l + 1] = {0, sib < cnt[l] ? reinterpret_cast<uint64_t>(lvl[l] + 32 * sib) : (OP_ZERO_FLAG | l), 0};
+        ops[l + 1] = sib < cnt[l] ? reinterpret_cast<uint64_t>(lvl[l] + 32 * sib) : (OP_ZERO_FLAG | l);
         idx >>= 1;
     }
     uint8_t* h_g = h + align_up(n * 32, 256);
-    memcpy(h_g, gath.data(), gath_bytes);
     uint8_t* d_g = d + total;
     uint8_t* d_res = d_g + align_up(gath_bytes, 256);
-    LHB_CUDA(cudaMemcpyAsync(d_g, h_g, gath_bytes, cudaMemcpyHostToDevice, c.stream));
-    k_gather_nodes<<<(depth + 32) / 32, 32, 0, c.stream>>>(reinterpret_cast<const HashOp*>(d_g), depth + 1, d_res);
-    count_launch();
+    int32_t rc = stage_operands(ops, reinterpret_cast<HashOp*>(d_g), h_g, c.stream);
+    if (!rc) rc = gather_operands(reinterpret_cast<HashOp*>(d_g), depth + 1, d_res, c.stream);
+    if (rc) return rc;
     uint8_t* h_res = h_g + align_up(gath_bytes, 256);
     LHB_CUDA(cudaMemcpyAsync(h_res, d_res, (depth + 1) * 32, cudaMemcpyDeviceToHost, c.stream));
     LHB_CUDA(cudaStreamSynchronize(c.stream));
@@ -1684,10 +1677,10 @@ static int32_t block_roots_attempt(Ctx& c, const uint8_t* ssz, const uint64_t* o
             bd.block(offsets[i] - base, offsets[i + 1] - offsets[i], reinterpret_cast<uint64_t>(d_roots + 32ull * i),
                      reinterpret_cast<uint64_t>(d_body + 32ull * i));
         bad = bd.bad;
+        return LHB200_OK;
     };
     // One planning pass over the bounded arena (host time matters here: a block is only ~10^4 hashes).
-    const size_t prog_bytes = align_up(max_nodes * sizeof(HashOp), 256) + align_up((max_nodes + 2) * 4, 256) +
-                              align_up(max_nodes * sizeof(ByteItem), 256) + 1024;
+    const size_t prog_bytes = program_bytes(max_nodes, max_nodes);
     // literals | node pool (op outputs) | staged blob | roots | item outputs | program blobs
     const size_t need = lit_cap + 32 * max_nodes + in_pad + 64ull * n + 32 * max_nodes + prog_bytes + 8192;
     uint8_t* arena = static_cast<uint8_t*>(dev_scratch(need));
@@ -1695,23 +1688,17 @@ static int32_t block_roots_attempt(Ctx& c, const uint8_t* ssz, const uint64_t* o
     uint8_t* hst = static_cast<uint8_t*>(pinned_scratch(stage_bytes));
     if (!arena || !hst) return LHB200_ENOMEM;
     Plan pl;
-    int32_t rc = build_plan(pl, arena, need, lit_cap, build, max_nodes);
+    int32_t rc = build_plan(pl, arena, need, lit_cap, build, max_nodes);   // fails only on the node or literal cap
     if (bad) { set_error("BeaconBlock SSZ: malformed offsets or lengths for this fork"); return LHB200_EINVAL; }
-    if (pl.node_overflow || pl.lit.size() > lit_cap || pl.ops.size() + pl.items.size() > max_nodes ||
-        pl.bump + prog_bytes > need) {
-        set_error("internal: block plan exceeds its arena bound (%zu ops + %zu items of %zu nodes, %zu of %zu literal bytes, "
-                  "%zu of %zu arena bytes)", pl.ops.size(), pl.items.size(), max_nodes, pl.lit.size(), lit_cap,
-                  pl.bump + prog_bytes, need);
+    if (rc || pl.ops.size() + pl.items.size() > max_nodes) {
+        set_error("internal: block plan exceeds its arena bound (%zu ops + %zu items of %zu nodes, %zu of %zu literal bytes)",
+                  pl.ops.size(), pl.items.size(), max_nodes, pl.lit.size(), lit_cap);
         return LHB200_ERETRY;
     }
-    if (rc) return rc;
     memcpy(hst, ssz + base, total);
     memset(hst + total, 0, align_up(total, 256) - total);
     LHB_CUDA(cudaMemcpyAsync(d_in, hst, align_up(total, 256), cudaMemcpyHostToDevice, c.stream));
-    std::vector<HashOp> ops_sorted;
-    std::vector<int32_t> waves;
-    plan_finalize_program(pl, ops_sorted, waves);
-    rc = plan_upload(pl, c.stream, ops_sorted, waves, hst + align_up(total, 256));
+    rc = plan_upload(pl, c.stream, hst + align_up(total, 256));
     if (rc) return rc;
     rc = plan_enqueue(pl, c.stream);
     if (rc) return rc;
@@ -1724,8 +1711,8 @@ static int32_t block_roots_attempt(Ctx& c, const uint8_t* ssz, const uint64_t* o
     return LHB200_OK;
 }
 
-// n BeaconBlockDeneb SSZ blobs, concatenated; offsets[n+1]; roots n*32; body_roots n*32 or NULL.
-static int32_t block_roots_deneb(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, uint8_t* roots,
+// n BeaconBlock SSZ blobs of `fork`, concatenated; offsets[n+1]; roots n*32; body_roots n*32 or NULL.
+static int32_t block_roots(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, uint8_t* roots,
                                  uint8_t* body_roots, bool blinded, int32_t fork = LHB200_FORK_DENEB) {
     LHB_REQUIRE_READY();
     if (fork < LHB200_FORK_ALTAIR || fork > LHB200_FORK_DENEB || (blinded && fork < LHB200_FORK_BELLATRIX)) {
@@ -1758,22 +1745,22 @@ static int32_t block_roots_deneb(const uint8_t* ssz, const uint64_t* offsets, ui
 }
 int32_t lhb200_beacon_block_roots_deneb(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, uint8_t* roots,
                                         uint8_t* body_roots) {
-    return block_roots_deneb(ssz, offsets, n, roots, body_roots, false);
+    return block_roots(ssz, offsets, n, roots, body_roots, false);
 }
 int32_t lhb200_beacon_block_root_deneb(const uint8_t* ssz, uint64_t len, uint8_t out[32], uint8_t* body_root) {
     const uint64_t offs[2] = {0, len};
-    return block_roots_deneb(ssz, offs, 1, out, body_root, false);
+    return block_roots(ssz, offs, 1, out, body_root, false);
 }
 // The earlier variants of the BeaconBlock superstruct (beacon_block.rs:41-90, beacon_block_body.rs:43-110): fork is
 // LHB200_FORK_ALTAIR .. LHB200_FORK_DENEB; blinded != 0 selects the BlindedBeaconBlock form (Bellatrix and later).
 int32_t lhb200_beacon_block_roots(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, int32_t fork, int32_t blinded,
                                   uint8_t* roots, uint8_t* body_roots) {
-    return block_roots_deneb(ssz, offsets, n, roots, body_roots, blinded != 0, fork);
+    return block_roots(ssz, offsets, n, roots, body_roots, blinded != 0, fork);
 }
 // BlindedBeaconBlock (beacon_block.rs:80): the body carries the ExecutionPayloadHeader; the root equals the full block's.
 int32_t lhb200_blinded_beacon_block_roots_deneb(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, uint8_t* roots,
                                                 uint8_t* body_roots) {
-    return block_roots_deneb(ssz, offsets, n, roots, body_roots, true);
+    return block_roots(ssz, offsets, n, roots, body_roots, true);
 }
 
 // swap_or_not_shuffle::shuffle_list(input, rounds, seed, forwards) (consensus/swap_or_not_shuffle/src/shuffle_list.rs:79).
