@@ -165,9 +165,12 @@ LHB200_API int32_t lhb200_beacon_block_roots_deneb(const uint8_t* ssz, const uin
  * the ExecutionPayloadHeaderDeneb, execution_payload_header.rs:46-87).  The root equals the full block's root. */
 LHB200_API int32_t lhb200_blinded_beacon_block_roots_deneb(const uint8_t* ssz, const uint64_t* offsets, uint32_t n,
                                                            uint8_t* roots, uint8_t* body_roots);
-/* The same for the earlier variants of the BeaconBlock superstruct (consensus/types/src/beacon_block.rs:41-90,
- * beacon_block_body.rs:43-110): fork = LHB200_FORK_ALTAIR (9 body fields, no execution payload), _BELLATRIX (14-field
- * payload), _CAPELLA (+ withdrawals, bls_to_execution_changes), _DENEB (+ blob gas fields, blob_kzg_commitments);
+/* The same for every variant of the BeaconBlock superstruct from Altair on (consensus/types/src/beacon_block.rs:41-90,
+ * beacon_block_body.rs:43-121): fork = LHB200_FORK_ALTAIR (9 body fields, no execution payload), _BELLATRIX (14-field
+ * payload), _CAPELLA (+ withdrawals, bls_to_execution_changes), _DENEB (+ blob gas fields, blob_kzg_commitments),
+ * _ELECTRA (+ consolidations; attestations with committee_bits and up to 131 072 aggregation bits, at most 8 of them
+ * and 1 attester slashing; payload + deposit_requests (<= 8192) and withdrawal_requests (<= 16),
+ * execution_payload.rs:54-101, attestation.rs:76-82, deposit_request.rs:23-29, signed_consolidation.rs:23-24);
  * blinded != 0: BlindedBeaconBlock (the body carries the ExecutionPayloadHeader; Bellatrix and later). */
 LHB200_API int32_t lhb200_beacon_block_roots(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, int32_t fork,
                                              int32_t blinded, uint8_t* roots, uint8_t* body_roots);

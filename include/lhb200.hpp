@@ -282,7 +282,7 @@ inline Hash256 beacon_block_root_deneb(const uint8_t* ssz, size_t len, Hash256* 
     return out;
 }
 
-/// canonical_root of one BeaconBlock / BlindedBeaconBlock of any fork from Altair to Deneb (beacon_block.rs:41-90)
+/// canonical_root of one BeaconBlock / BlindedBeaconBlock of any fork from Altair to Electra (beacon_block.rs:41-90)
 inline Hash256 beacon_block_root(const uint8_t* ssz, size_t len, int32_t fork, bool blinded = false, Hash256* body_root = nullptr) {
     Hash256 out;
     const uint64_t offs[2] = {0, len};

@@ -3,7 +3,7 @@
 // Kernel inventory (SURVEY.md §2d K1-K3):
 //   k_hash_pairs ........ n independent hash32_concat (ethereum_hashing::hash32_concat batch)
 //   k_validator_roots ... 121-byte SSZ Validator -> 32-byte root (8 hashes / validator, validator.rs:25-35)
-//   k_record_roots ...... small fixed records: 48-B pubkey (bls/src/macros.rs:18-25), 72-B Eth1Data
+//   k_record_roots ...... small fixed records: 48-B pubkey (bls/src/macros.rs:18-25), 72-B Eth1Data, 192-B DepositRequest
 //   k_merkle_reduce ..... multi-segment tile reduce: every CTA folds up to 2^11 chunks of one segment
 //                         (up to 11 tree levels) and writes one node; virtual zero padding via ZERO_HASHES
 //   k_hash_program ...... small DAG interpreter (zero ladders, mix_in_length, small containers, top tree)
@@ -116,13 +116,39 @@ __global__ void __launch_bounds__(VAL_PER_CTA) k_validator_roots(const uint8_t* 
 // ---------------------------------------------------------------------------------------------
 // Small fixed-size records -> roots.  kind 0: 48-byte pubkey.  kind 1: 72-byte Eth1Data {H256,u64,H256}.
 // kind 2: 16-byte {u64, u64} (PendingBalanceDeposit, PendingConsolidation).  kind 3: 24-byte {u64, u64, u64}
-// (PendingPartialWithdrawal): the Electra state lists, beacon_state.rs:515-525.
+// (PendingPartialWithdrawal): the Electra state lists, beacon_state.rs:515-525.  kind 4: 192-byte DepositRequest
+// {pubkey, withdrawal_credentials, amount, signature, index} (deposit_request.rs:23-29), 10 hashes.  Loads are
+// bytewise, so `in` may sit at any byte offset (the block path reads the records straight from the staged SSZ blob).
 __global__ void __launch_bounds__(128) k_record_roots(const uint8_t* __restrict__ in, uint64_t n, int kind,
                                                       uint8_t* __restrict__ out) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     uint32_t a[8], b[8];
-    if (kind == 0) {
+    if (kind == 4) {
+        const uint8_t* p = in + 192 * i;
+        uint32_t c[8];
+        for (int k = 0; k < 8; k++) a[k] = be_word(p + 4 * k);
+        for (int k = 0; k < 4; k++) b[k] = be_word(p + 32 + 4 * k);
+        b[4] = b[5] = b[6] = b[7] = 0;
+        hash_pair(a, b, a);                       // pubkey
+        for (int k = 0; k < 8; k++) b[k] = be_word(p + 48 + 4 * k);
+        hash_pair(a, b, a);                       // H(pubkey, withdrawal_credentials)
+        for (int k = 0; k < 8; k++) b[k] = be_word(p + 88 + 4 * k);
+        for (int k = 0; k < 8; k++) c[k] = be_word(p + 120 + 4 * k);
+        hash_pair(b, c, b);                       // signature chunks 0, 1
+        for (int k = 0; k < 8; k++) c[k] = be_word(p + 152 + 4 * k);
+        hash_pair(c, g_zero_words[0], c);         // signature chunk 2, zero chunk
+        hash_pair(b, c, b);                       // signature root
+        for (int k = 0; k < 8; k++) c[k] = 0;
+        le64_words(p + 80, c[0], c[1]);
+        hash_pair(c, b, c);                       // H(amount, signature)
+        hash_pair(a, c, a);                       // fields 0..3
+        for (int k = 0; k < 8; k++) c[k] = 0;
+        le64_words(p + 184, c[0], c[1]);
+        hash_pair(c, g_zero_words[0], c);         // H(index, zero chunk)
+        hash_pair(c, g_zero_words[1], c);         // fields 4..7
+        hash_pair(a, c, a);
+    } else if (kind == 0) {
         const uint8_t* p = in + 48 * i;
         for (int k = 0; k < 8; k++) a[k] = be_word(p + 4 * k);
         for (int k = 0; k < 4; k++) b[k] = be_word(p + 32 + 4 * k);

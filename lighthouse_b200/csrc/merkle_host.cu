@@ -52,7 +52,7 @@ struct LeafKind {
 constexpr LeafKind LEAF_NONE{LeafKind::NONE, 0, 0}, LEAF_VALIDATOR{LeafKind::VALIDATORS, 0, 8},
                    LEAF_PUBKEY{LeafKind::RECORDS, 0, 1}, LEAF_ETH1_DATA{LeafKind::RECORDS, 1, 3},
                    LEAF_U64_PAIR{LeafKind::RECORDS, 2, 1}, LEAF_U64_TRIPLE{LeafKind::RECORDS, 3, 3},
-                   LEAF_CHUNK_PAIR{LeafKind::HASH_PAIRS, 0, 1};
+                   LEAF_DEPOSIT_REQUEST{LeafKind::RECORDS, 4, 10}, LEAF_CHUNK_PAIR{LeafKind::HASH_PAIRS, 0, 1};
 
 struct LeafLaunch {
     LeafKind kind;
@@ -1473,6 +1473,13 @@ int32_t lhb200_verify_merkle_proofs(const uint8_t* leaves, const uint8_t* branch
 // (transactions, signatures, pubkeys, bit lists, index lists, proofs, blooms) is hashed by k_byte_items straight
 // from the staged blob, fixed 8/20/32-byte fields become literal chunks, and the container structure above them is
 // a hash program.  `s` = host bytes, `d` = the same bytes on the device.
+// Electra (beacon_block_body.rs:70-121, limits eth_spec.rs:433-440): 396-byte body fixed part (+ consolidations offset at
+// 392), attestations with up to 131 072 aggregation bits and a committee bitvector before the signature (236-byte fixed
+// part, attestation.rs:76-82), indexed attestations with up to 131 072 indices, a 536-byte payload fixed part (+ offsets
+// of deposit_requests and withdrawal_requests at 528 / 532, execution_payload.rs:54-101).  The up to 8 192 DepositRequest
+// records are the one list of fixed-size containers in a block that can reach thousands of items: past 64 records,
+// k_record_roots kind 4 hashes them straight from the staged blob, the reduce passes fold them, and the host plans no
+// node per record.
 }  // extern "C"
 namespace {
 struct BlockDescriber {
@@ -1482,8 +1489,10 @@ struct BlockDescriber {
     bool bad = false;
     bool blinded = false;   // BlindedBeaconBlock: field 9 of the body is an ExecutionPayloadHeader
     int32_t fork = LHB200_FORK_DENEB;   // beacon_block_body.rs superstruct variant: Altair 9 body fields (no payload),
-                                        // Bellatrix 10 (14-field payload), Capella 11 (+ withdrawals, BLS changes), Deneb 12
+                                        // Bellatrix 10 (14-field payload), Capella 11 (+ withdrawals, BLS changes), Deneb 12,
+                                        // Electra 13 (+ consolidations; 19-field payload, wider attestations)
 
+    bool electra() const { return fork >= LHB200_FORK_ELECTRA; }
     uint64_t u64(uint64_t off) { return p.literal_bytes(s + off, 8); }
     uint64_t h256(uint64_t off) { return p.literal_bytes(s + off, 32); }
     uint64_t addr20(uint64_t off) { return p.literal_bytes(s + off, 20); }
@@ -1499,21 +1508,29 @@ struct BlockDescriber {
         return p.op_hash(h, sig(off + 112));
     }
     uint64_t proposer_slashing(uint64_t off) { return p.op_hash(signed_header(off), signed_header(off + 208)); }
+    // attesting_indices: List[u64, MaxValidatorsPerCommittee = 2048] (depth 9); Electra List[u64, MaxValidatorsPerSlot =
+    // 131072] (depth 15)
     uint64_t indexed_attestation(uint64_t off, uint64_t len) {
-        if (len < 228 || rd32(s + off) != 228 || (len - 228) % 8 || (len - 228) / 8 > 2048) { bad = true; return 0; }
-        uint64_t idx = p.bytes_item(d + off + 228, len - 228, 9, true, (len - 228) / 8);
+        const uint64_t max_idx = electra() ? 131072 : 2048;
+        if (len < 228 || rd32(s + off) != 228 || (len - 228) % 8 || (len - 228) / 8 > max_idx) { bad = true; return 0; }
+        uint64_t idx = p.bytes_item(d + off + 228, len - 228, electra() ? 15 : 9, true, (len - 228) / 8);
         return p.container({idx, att_data(off + 4), sig(off + 132)});
     }
+    // aggregation_bits: Bitlist[2048] (depth 3) behind a 228-byte fixed part; Electra Bitlist[131072] (depth 9) behind
+    // 236 bytes, with committee_bits (Bitvector[64]) between data and signature
     uint64_t attestation(uint64_t off, uint64_t len) {
-        if (len < 229 || rd32(s + off) != 228 || s[off + len - 1] == 0) { bad = true; return 0; }
-        const uint64_t nb = len - 228;
+        const uint32_t fixed = electra() ? 236 : 228;
+        if (len < fixed + 1 || rd32(s + off) != fixed || s[off + len - 1] == 0) { bad = true; return 0; }
+        const uint64_t nb = len - fixed;
         const uint8_t last = s[off + len - 1];
         int top = 7;
         while (!((last >> top) & 1)) top--;
         const uint64_t bitlen = 8 * (nb - 1) + (uint64_t)top;
-        if (bitlen > 2048) { bad = true; return 0; }
+        if (bitlen > (electra() ? 131072u : 2048u)) { bad = true; return 0; }
         // drop the delimiter: either the whole last byte (top == 0) or its top bit
-        uint64_t bits = p.bytes_item(d + off + 228, (bitlen + 7) / 8, 3, true, bitlen, top ? (uint32_t)((1u << top) - 1) : 0xff);
+        uint64_t bits = p.bytes_item(d + off + fixed, (bitlen + 7) / 8, electra() ? 9 : 3, true, bitlen,
+                                     top ? (uint32_t)((1u << top) - 1) : 0xff);
+        if (electra()) return p.container({bits, att_data(off + 4), p.literal_bytes(s + off + 132, 8), sig(off + 140)});
         return p.container({bits, att_data(off + 4), sig(off + 132)});
     }
     uint64_t deposit(uint64_t off) {  // 1240 B
@@ -1525,6 +1542,17 @@ struct BlockDescriber {
         return p.op_hash(p.container({u64(off), pubkey(off + 8), addr20(off + 56)}), sig(off + 76));
     }
     uint64_t withdrawal(uint64_t off) { return p.container({u64(off), u64(off + 8), addr20(off + 16), u64(off + 36)}); }
+    // DepositRequest (deposit_request.rs:23-29): 192 B; k_record_roots kind 4 computes the same root on the device
+    static constexpr uint64_t DEPOSIT_REQUESTS_AS_OPS = 64;
+    uint64_t deposit_request(uint64_t off) {
+        return p.container({pubkey(off), h256(off + 48), u64(off + 80), sig(off + 88), u64(off + 184)});
+    }
+    // ExecutionLayerWithdrawalRequest (execution_layer_withdrawal_request.rs:23-26): 76 B
+    uint64_t withdrawal_request(uint64_t off) { return p.container({addr20(off), pubkey(off + 20), u64(off + 68)}); }
+    // SignedConsolidation (signed_consolidation.rs:23-24, consolidation.rs:24-27): 120 B
+    uint64_t consolidation(uint64_t off) {
+        return p.op_hash(p.container({u64(off), u64(off + 8), u64(off + 16)}), sig(off + 24));
+    }
     uint64_t list_of(std::vector<uint64_t>& roots, uint32_t limit_log) {
         uint64_t n = roots.size();
         uint64_t r = p.small_tree(roots, std::min<uint32_t>(limit_log, ceil_log2(std::max<uint64_t>(n, 1))));
@@ -1553,13 +1581,16 @@ struct BlockDescriber {
         return true;
     }
     uint64_t payload(uint64_t off, uint64_t len) {
-        // fixed part: 508 B (Bellatrix: ... transactions offset), 512 (Capella: + withdrawals offset), 528 (Deneb: + blob gas)
-        const bool has_wd = fork >= LHB200_FORK_CAPELLA, has_blob = fork >= LHB200_FORK_DENEB;
-        const uint32_t fixed = has_blob ? 528 : has_wd ? 512 : 508;
+        // fixed part: 508 B (Bellatrix: ... transactions offset), 512 (Capella: + withdrawals offset), 528 (Deneb: + blob gas),
+        // 536 (Electra: + deposit_requests and withdrawal_requests offsets)
+        const bool has_wd = fork >= LHB200_FORK_CAPELLA, has_blob = fork >= LHB200_FORK_DENEB, has_req = electra();
+        const uint32_t fixed = has_req ? 536 : has_blob ? 528 : has_wd ? 512 : 508;
         if (len < fixed) { bad = true; return 0; }
-        const uint32_t o_extra = rd32(s + off + 436), o_tx = rd32(s + off + 504), o_wd = has_wd ? rd32(s + off + 508) : (uint32_t)len;
-        if (o_extra != fixed || o_tx < o_extra || o_tx - o_extra > 32 || o_wd < o_tx || o_wd > len || (len - o_wd) % 44 ||
-            (len - o_wd) / 44 > 16) { bad = true; return 0; }
+        const uint32_t o_extra = rd32(s + off + 436), o_tx = rd32(s + off + 504), o_wd = has_wd ? rd32(s + off + 508) : (uint32_t)len,
+                       o_dr = has_req ? rd32(s + off + 528) : (uint32_t)len, o_wr = has_req ? rd32(s + off + 532) : (uint32_t)len;
+        if (o_extra != fixed || o_tx < o_extra || o_tx - o_extra > 32 || o_wd < o_tx || o_wd > o_dr || (o_dr - o_wd) % 44 ||
+            (o_dr - o_wd) / 44 > 16 || o_wr < o_dr || o_wr > len || (o_wr - o_dr) % 192 || (o_wr - o_dr) / 192 > 8192 ||
+            (len - o_wr) % 76 || (len - o_wr) / 76 > 16) { bad = true; return 0; }
         std::vector<uint64_t> f(14);
         f[0] = h256(off); f[1] = addr20(off + 32); f[2] = h256(off + 52); f[3] = h256(off + 84);
         f[4] = blob(off + 116, 256, 3);
@@ -1571,15 +1602,27 @@ struct BlockDescriber {
         for (size_t i = 0; i + 1 < b.size(); i++)  // ByteList[2^30]: 2^25 chunks
             roots.push_back(p.bytes_item(d + off + o_tx + b[i], b[i + 1] - b[i], 25, true, b[i + 1] - b[i]));
         f[13] = list_of(roots, 20);
-        if (has_wd) f.push_back(fixed_list(off + o_wd, len - o_wd, 44, 4, [&](uint64_t o) { return withdrawal(o); }));
+        if (has_wd) f.push_back(fixed_list(off + o_wd, o_dr - o_wd, 44, 4, [&](uint64_t o) { return withdrawal(o); }));
         if (has_blob) { f.push_back(u64(off + 512)); f.push_back(u64(off + 520)); }
+        if (has_req) {
+            // List[DepositRequest, 8192]: depth 13.  The record kernel and its reduce pass add two serial launches per
+            // block (k_record_roots is one thread's chain of 10 hashes); host planning costs ~0.7 us per record.  On an
+            // H100 the ops are faster up to 64 records and the kernel past that (DESIGN §3.5).
+            const uint64_t n_dr = (o_wr - o_dr) / 192;
+            if (n_dr <= DEPOSIT_REQUESTS_AS_OPS)
+                f.push_back(fixed_list(off + o_dr, o_wr - o_dr, 192, 13, [&](uint64_t o) { return deposit_request(o); }));
+            else
+                f.push_back(p.mix_in_length(p.merkle_list(p.leaf_kernel(LEAF_DEPOSIT_REQUEST, d + off + o_dr, n_dr), n_dr, 13), n_dr));
+            f.push_back(fixed_list(off + o_wr, len - o_wr, 76, 4, [&](uint64_t o) { return withdrawal_request(o); }));
+        }
         return p.container(f);
     }
     // ExecutionPayloadHeaderDeneb (execution_payload_header.rs:46-87): 584-byte fixed part + extra_data
     uint64_t payload_header(uint64_t off, uint64_t len) {
-        // 536-byte fixed part (Bellatrix, 14 fields), 568 (Capella: + withdrawals_root), 584 (Deneb: + blob gas)
-        const bool has_wd = fork >= LHB200_FORK_CAPELLA, has_blob = fork >= LHB200_FORK_DENEB;
-        const uint32_t fixed = has_blob ? 584 : has_wd ? 568 : 536;
+        // 536-byte fixed part (Bellatrix, 14 fields), 568 (Capella: + withdrawals_root), 584 (Deneb: + blob gas),
+        // 648 (Electra: + deposit_requests_root, withdrawal_requests_root)
+        const bool has_wd = fork >= LHB200_FORK_CAPELLA, has_blob = fork >= LHB200_FORK_DENEB, has_req = electra();
+        const uint32_t fixed = has_req ? 648 : has_blob ? 584 : has_wd ? 568 : 536;
         if (len < fixed || len > fixed + 32 || rd32(s + off + 436) != fixed) { bad = true; return 0; }
         std::vector<uint64_t> f(14);
         f[0] = h256(off); f[1] = addr20(off + 32); f[2] = h256(off + 52); f[3] = h256(off + 84);
@@ -1590,24 +1633,28 @@ struct BlockDescriber {
         f[13] = h256(off + 504);            // transactions_root
         if (has_wd) f.push_back(h256(off + 536));            // withdrawals_root
         if (has_blob) { f.push_back(u64(off + 568)); f.push_back(u64(off + 576)); }
+        if (has_req) { f.push_back(h256(off + 584)); f.push_back(h256(off + 616)); }
         return p.container(f);
     }
     uint64_t body(uint64_t off, uint64_t len, uint64_t dst) {
-        const bool has_ep = fork >= LHB200_FORK_BELLATRIX, has_bc = fork >= LHB200_FORK_CAPELLA, has_kz = fork >= LHB200_FORK_DENEB;
-        const uint32_t fixed = 380 + (has_ep ? 4 : 0) + (has_bc ? 4 : 0) + (has_kz ? 4 : 0);
+        const bool has_ep = fork >= LHB200_FORK_BELLATRIX, has_bc = fork >= LHB200_FORK_CAPELLA, has_kz = fork >= LHB200_FORK_DENEB,
+                   has_cs = electra();
+        const uint32_t fixed = 380 + (has_ep ? 4 : 0) + (has_bc ? 4 : 0) + (has_kz ? 4 : 0) + (has_cs ? 4 : 0);
         if (len < fixed) { bad = true; return 0; }
         const uint32_t o_ps = rd32(s + off + 200), o_as = rd32(s + off + 204), o_at = rd32(s + off + 208),
                        o_dp = rd32(s + off + 212), o_ex = rd32(s + off + 216),
                        o_ep = has_ep ? rd32(s + off + 380) : (uint32_t)len, o_bc = has_bc ? rd32(s + off + 384) : (uint32_t)len,
-                       o_kz = has_kz ? rd32(s + off + 388) : (uint32_t)len;
+                       o_kz = has_kz ? rd32(s + off + 388) : (uint32_t)len, o_cs = has_cs ? rd32(s + off + 392) : (uint32_t)len;
         if (o_ps != fixed || o_as < o_ps || o_at < o_as || o_dp < o_at || o_ex < o_dp || o_ep < o_ex || o_bc < o_ep ||
-            o_kz < o_bc || o_kz > len) { bad = true; return 0; }
+            o_kz < o_bc || o_cs < o_kz || o_cs > len) { bad = true; return 0; }
         std::vector<uint64_t> f(9), b, roots;
         f[0] = sig(off);
         f[1] = p.container({h256(off + 96), u64(off + 128), h256(off + 136)});  // eth1_data.rs:27
         f[2] = h256(off + 168);
         f[3] = fixed_list(off + o_ps, o_as - o_ps, 416, 4, [&](uint64_t o) { return proposer_slashing(o); });
-        if (!var_bounds(off + o_as, o_at - o_as, 2, b)) { bad = true; return 0; }
+        // MaxAttesterSlashings 2, MaxAttestations 128; Electra MaxAttesterSlashingsElectra 1, MaxAttestationsElectra 8
+        const uint32_t as_log = has_cs ? 0 : 1, at_log = has_cs ? 3 : 7;
+        if (!var_bounds(off + o_as, o_at - o_as, 1u << as_log, b)) { bad = true; return 0; }
         for (size_t i = 0; i + 1 < b.size(); i++) {
             const uint64_t q = off + o_as + b[i], ql = b[i + 1] - b[i];
             if (ql < 8) { bad = true; return 0; }
@@ -1617,20 +1664,21 @@ struct BlockDescriber {
             if (bad) return 0;
             roots.push_back(p.op_hash(r1, r2));
         }
-        f[4] = list_of(roots, 1);
+        f[4] = list_of(roots, as_log);
         roots.clear();
-        if (!var_bounds(off + o_at, o_dp - o_at, 128, b)) { bad = true; return 0; }
+        if (!var_bounds(off + o_at, o_dp - o_at, 1u << at_log, b)) { bad = true; return 0; }
         for (size_t i = 0; i + 1 < b.size(); i++) {
             roots.push_back(attestation(off + o_at + b[i], b[i + 1] - b[i]));
             if (bad) return 0;
         }
-        f[5] = list_of(roots, 7);
+        f[5] = list_of(roots, at_log);
         f[6] = fixed_list(off + o_dp, o_ex - o_dp, 1240, 4, [&](uint64_t o) { return deposit(o); });
         f[7] = fixed_list(off + o_ex, o_ep - o_ex, 112, 4, [&](uint64_t o) { return voluntary_exit(o); });
         f[8] = p.op_hash(blob(off + 220, 64, 1), sig(off + 284));  // sync_aggregate.rs:38
         if (has_ep) f.push_back(blinded ? payload_header(off + o_ep, o_bc - o_ep) : payload(off + o_ep, o_bc - o_ep));
         if (has_bc) f.push_back(fixed_list(off + o_bc, o_kz - o_bc, 172, 4, [&](uint64_t o) { return bls_change(o); }));
-        if (has_kz) f.push_back(fixed_list(off + o_kz, len - o_kz, 48, 12, [&](uint64_t o) { return pubkey(o); }));  // kzg_commitment.rs:51
+        if (has_kz) f.push_back(fixed_list(off + o_kz, o_cs - o_kz, 48, 12, [&](uint64_t o) { return pubkey(o); }));  // kzg_commitment.rs:51
+        if (has_cs) f.push_back(fixed_list(off + o_cs, len - o_cs, 120, 0, [&](uint64_t o) { return consolidation(o); }));
         if (bad) return 0;
         return p.container(f, dst);
     }
@@ -1646,7 +1694,9 @@ extern "C" {
 
 constexpr int32_t LHB200_ERETRY = -1000;   // internal: the plan did not fit the arena bound of this attempt
 
-// transactions in one BeaconBlockDeneb blob (0 when the offsets are not plausible — the describer reports that)
+// transactions in one BeaconBlock blob of `fork` (0 when the offsets are not plausible — the describer reports that).
+// The body offsets read here and the payload's transactions / withdrawals offsets sit at the same places from
+// Bellatrix to Electra.
 static uint64_t prescan_transactions(const uint8_t* blk, uint64_t len, int32_t fork) {
     auto rd = [&](uint64_t o) { uint32_t v; memcpy(&v, blk + o, 4); return (uint64_t)v; };
     if (fork < LHB200_FORK_BELLATRIX || len < 84 + 392) return 0;
@@ -1681,7 +1731,8 @@ static int32_t block_roots_attempt(Ctx& c, const uint8_t* ssz, const uint64_t* o
     };
     // One planning pass over the bounded arena (host time matters here: a block is only ~10^4 hashes).
     const size_t prog_bytes = program_bytes(max_nodes, max_nodes);
-    // literals | node pool (op outputs) | staged blob | roots | item outputs | program blobs
+    // literals | node pool (op outputs) | staged blob | roots | item outputs, leaf-kernel roots and reduce outputs
+    // (one 32-byte root per 192-byte DepositRequest, well inside one node per 12 bytes) | program blobs
     const size_t need = lit_cap + 32 * max_nodes + in_pad + 64ull * n + 32 * max_nodes + prog_bytes + 8192;
     uint8_t* arena = static_cast<uint8_t*>(dev_scratch(need));
     const size_t stage_bytes = align_up(total, 256) + lit_cap + prog_bytes + 64ull * n + 1024;
@@ -1690,9 +1741,9 @@ static int32_t block_roots_attempt(Ctx& c, const uint8_t* ssz, const uint64_t* o
     Plan pl;
     int32_t rc = build_plan(pl, arena, need, lit_cap, build, max_nodes);   // fails only on the node or literal cap
     if (bad) { set_error("BeaconBlock SSZ: malformed offsets or lengths for this fork"); return LHB200_EINVAL; }
-    if (rc || pl.ops.size() + pl.items.size() > max_nodes) {
-        set_error("internal: block plan exceeds its arena bound (%zu ops + %zu items of %zu nodes, %zu of %zu literal bytes)",
-                  pl.ops.size(), pl.items.size(), max_nodes, pl.lit.size(), lit_cap);
+    if (rc || pl.ops.size() + pl.items.size() > max_nodes || pl.bump + program_bytes(pl.ops.size(), pl.items.size()) > need) {
+        set_error("internal: block plan exceeds its arena bound (%zu ops + %zu items of %zu nodes, %zu of %zu literal bytes, "
+                  "%zu of %zu arena bytes)", pl.ops.size(), pl.items.size(), max_nodes, pl.lit.size(), lit_cap, pl.bump, need);
         return LHB200_ERETRY;
     }
     memcpy(hst, ssz + base, total);
@@ -1715,8 +1766,8 @@ static int32_t block_roots_attempt(Ctx& c, const uint8_t* ssz, const uint64_t* o
 static int32_t block_roots(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, uint8_t* roots,
                                  uint8_t* body_roots, bool blinded, int32_t fork = LHB200_FORK_DENEB) {
     LHB_REQUIRE_READY();
-    if (fork < LHB200_FORK_ALTAIR || fork > LHB200_FORK_DENEB || (blinded && fork < LHB200_FORK_BELLATRIX)) {
-        set_error("beacon_block_roots: fork id %d not supported (Altair .. Deneb; blinded blocks from Bellatrix)", fork);
+    if (fork < LHB200_FORK_ALTAIR || fork > LHB200_FORK_ELECTRA || (blinded && fork < LHB200_FORK_BELLATRIX)) {
+        set_error("beacon_block_roots: fork id %d not supported (Altair .. Electra; blinded blocks from Bellatrix)", fork);
         return LHB200_EINVAL;
     }
     if (!ssz || !offsets || !roots || n == 0) { set_error("beacon_block_roots: null argument or zero blocks"); return LHB200_EINVAL; }
@@ -1751,8 +1802,8 @@ int32_t lhb200_beacon_block_root_deneb(const uint8_t* ssz, uint64_t len, uint8_t
     const uint64_t offs[2] = {0, len};
     return block_roots(ssz, offs, 1, out, body_root, false);
 }
-// The earlier variants of the BeaconBlock superstruct (beacon_block.rs:41-90, beacon_block_body.rs:43-110): fork is
-// LHB200_FORK_ALTAIR .. LHB200_FORK_DENEB; blinded != 0 selects the BlindedBeaconBlock form (Bellatrix and later).
+// The variants of the BeaconBlock superstruct from Altair on (beacon_block.rs:41-90, beacon_block_body.rs:43-121): fork is
+// LHB200_FORK_ALTAIR .. LHB200_FORK_ELECTRA; blinded != 0 selects the BlindedBeaconBlock form (Bellatrix and later).
 int32_t lhb200_beacon_block_roots(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, int32_t fork, int32_t blinded,
                                   uint8_t* roots, uint8_t* body_roots) {
     return block_roots(ssz, offsets, n, roots, body_roots, blinded != 0, fork);

@@ -192,13 +192,32 @@ ExecutionPayloadCapella = C(*_pf[:15])
 BeaconBlockBodyAltair = C(*_bf[:9])
 BeaconBlockBodyBellatrix = C(*(_bf[:9] + [("execution_payload", ExecutionPayloadBellatrix)]))
 BeaconBlockBodyCapella = C(*(_bf[:9] + [("execution_payload", ExecutionPayloadCapella)] + _bf[10:11]))
+# ---- Electra as in this revision of the reference (beacon_block_body.rs:70-121, attestation.rs:76-82,
+# indexed_attestation.rs:57-62, execution_payload.rs:54-101, deposit_request.rs:23-29,
+# execution_layer_withdrawal_request.rs:23-26, signed_consolidation.rs:23-24, consolidation.rs:24-27; limits
+# eth_spec.rs:395-440: MaxValidatorsPerSlot 131072, MaxCommitteesPerSlot 64)
+IndexedAttestationElectra = C(("attesting_indices", ("list", U64, 131072)), ("data", AttestationData), ("signature", B96))
+AttesterSlashingElectra = C(("attestation_1", IndexedAttestationElectra), ("attestation_2", IndexedAttestationElectra))
+AttestationElectra = C(("aggregation_bits", ("bitlist", 131072)), ("data", AttestationData),
+                       ("committee_bits", ("bitvector", 64)), ("signature", B96))
+DepositRequest = C(("pubkey", B48), ("withdrawal_credentials", B32), ("amount", U64), ("signature", B96), ("index", U64))
+ExecutionLayerWithdrawalRequest = C(("source_address", B20), ("validator_pubkey", B48), ("amount", U64))
+Consolidation = C(("source_index", U64), ("target_index", U64), ("epoch", U64))
+SignedConsolidation = C(("message", Consolidation), ("signature", B96))
+ExecutionPayloadElectra = C(*(_pf + [("deposit_requests", ("list", DepositRequest, 8192)),
+                                     ("withdrawal_requests", ("list", ExecutionLayerWithdrawalRequest, 16))]))
+_electra_body = {"attester_slashings": ("list", AttesterSlashingElectra, 1), "attestations": ("list", AttestationElectra, 8),
+                 "execution_payload": ExecutionPayloadElectra}
+BeaconBlockBodyElectra = C(*([(n, _electra_body.get(n, t)) for n, t in _bf] +
+                             [("consolidations", ("list", SignedConsolidation, 1))]))
 BEACON_BLOCK_BODY_BY_FORK = {"altair": BeaconBlockBodyAltair, "bellatrix": BeaconBlockBodyBellatrix,
-                             "capella": BeaconBlockBodyCapella, "deneb": BeaconBlockBodyDeneb}
+                             "capella": BeaconBlockBodyCapella, "deneb": BeaconBlockBodyDeneb,
+                             "electra": BeaconBlockBodyElectra}
 BEACON_BLOCK_BY_FORK = {k: _block_of(v) for k, v in BEACON_BLOCK_BODY_BY_FORK.items()}
 EXECUTION_PAYLOAD_BY_FORK = {"bellatrix": ExecutionPayloadBellatrix, "capella": ExecutionPayloadCapella,
-                             "deneb": ExecutionPayloadDeneb}
+                             "deneb": ExecutionPayloadDeneb, "electra": ExecutionPayloadElectra}
 EXECUTION_PAYLOAD_HEADER_BY_FORK = {"bellatrix": ExecutionPayloadHeaderBellatrix, "capella": ExecutionPayloadHeaderCapella,
-                                    "deneb": ExecutionPayloadHeaderDeneb}
+                                    "deneb": ExecutionPayloadHeaderDeneb, "electra": ExecutionPayloadHeaderElectra}
 BLINDED_BEACON_BLOCK_BODY_BY_FORK = {
     f: C(*[(n, EXECUTION_PAYLOAD_HEADER_BY_FORK[f]) if n == "execution_payload" else (n, t) for n, t in b[1]])
     for f, b in BEACON_BLOCK_BODY_BY_FORK.items() if f != "altair"}

@@ -335,3 +335,71 @@ def blind_block_deneb(block, transactions_root: bytes, withdrawals_root: bytes, 
     hdr["transactions_root"], hdr["withdrawals_root"] = transactions_root, withdrawals_root
     v["body"]["execution_payload"] = {n: hdr[n] for n, _ in S.EXECUTION_PAYLOAD_HEADER_BY_FORK[fork][1]}
     return v, S.serialize(S.BLINDED_BEACON_BLOCK_BY_FORK[fork], v)
+
+
+# ---------------------------------------------------------------------------------------------------------
+# Synthetic Electra BeaconBlock (mainnet preset, beacon_block_body.rs:70-121).  A generator of its own, so the Deneb
+# generator above keeps its exact byte output (and random stream) for every existing caller.
+def beacon_block_electra(seed=1, n_attestations=8, committees_per_attestation=4, bits_per_committee=500,
+                         n_deposit_requests=4, n_withdrawal_requests=16, n_consolidations=1, n_attester_slashings=1,
+                         slashing_indices=None, bit_lengths=None, **deneb_kw):
+    """-> (value, ssz_bytes) of a BeaconBlockElectra.  The fields Electra shares with Deneb come from
+    beacon_block_deneb(seed, **deneb_kw); the Electra operations from a second seeded stream.  Attestation i covers
+    `committees_per_attestation` committees (committee_bits) of `bits_per_committee` + i % 7 aggregation bits, unless
+    `bit_lengths` gives every attestation's bit count (n_attestations is then len(bit_lengths)).  The first indexed
+    attestation of each attester slashing has `slashing_indices` indices (default: one attestation's bit count)."""
+    from . import ssz_schema as S
+    block, _ = beacon_block_deneb(seed=seed, n_attestations=0, n_attester_slashings=0, **deneb_kw)
+    rng = np.random.default_rng([seed, 5])
+
+    def rb(n):
+        return rng.integers(0, 256, size=n, dtype=np.uint8).tobytes()
+
+    def u64():
+        return int(rng.integers(0, 1 << 62))
+
+    def att_data():  # Electra: the committee index moved to committee_bits, data.index is 0
+        cp = lambda: {"epoch": u64(), "root": rb(32)}
+        return {"slot": u64(), "index": 0, "beacon_block_root": rb(32), "source": cp(), "target": cp()}
+
+    def indexed(n):
+        return {"attesting_indices": sorted(int(x) for x in rng.integers(0, 1 << 20, size=n)), "data": att_data(),
+                "signature": rb(96)}
+
+    k = min(64, committees_per_attestation)
+    if bit_lengths is None:
+        bit_lengths = [k * bits_per_committee + i % 7 for i in range(n_attestations)]
+    if slashing_indices is None:
+        slashing_indices = k * bits_per_committee
+    attestations = []
+    for nb in bit_lengths:
+        committees = {int(c) for c in rng.choice(64, size=k, replace=False)}
+        attestations.append({"aggregation_bits": rng.integers(0, 2, size=nb).astype(bool).tolist(), "data": att_data(),
+                             "committee_bits": [c in committees for c in range(64)], "signature": rb(96)})
+    body = block["body"]
+    body["attester_slashings"] = [{"attestation_1": indexed(slashing_indices),
+                                   "attestation_2": indexed(slashing_indices // 2 + 1)} for _ in range(n_attester_slashings)]
+    body["attestations"] = attestations
+    body["execution_payload"]["deposit_requests"] = [
+        {"pubkey": rb(48), "withdrawal_credentials": rb(32), "amount": u64(), "signature": rb(96), "index": u64()}
+        for _ in range(n_deposit_requests)]
+    body["execution_payload"]["withdrawal_requests"] = [
+        {"source_address": rb(20), "validator_pubkey": rb(48), "amount": u64()} for _ in range(n_withdrawal_requests)]
+    body["consolidations"] = [{"message": {"source_index": u64(), "target_index": u64(), "epoch": u64()},
+                               "signature": rb(96)} for _ in range(n_consolidations)]
+    return block, S.serialize(S.BEACON_BLOCK_BY_FORK["electra"], block)
+
+
+def blind_block_electra(block, transactions_root: bytes, withdrawals_root: bytes, deposit_requests_root: bytes,
+                        withdrawal_requests_root: bytes):
+    """BlindedBeaconBlockElectra value + SSZ of `block` (as produced by beacon_block_electra) given the four list roots
+    of its payload (ExecutionPayloadHeaderElectra, execution_payload_header.rs:88-93)."""
+    import copy
+    from . import ssz_schema as S
+    v = copy.deepcopy(block)
+    p = v["body"]["execution_payload"]
+    hdr = {k: p[k] for k in p if k not in ("transactions", "withdrawals", "deposit_requests", "withdrawal_requests")}
+    hdr.update(transactions_root=transactions_root, withdrawals_root=withdrawals_root,
+               deposit_requests_root=deposit_requests_root, withdrawal_requests_root=withdrawal_requests_root)
+    v["body"]["execution_payload"] = {n: hdr[n] for n, _ in S.ExecutionPayloadHeaderElectra[1]}
+    return v, S.serialize(S.BLINDED_BEACON_BLOCK_BY_FORK["electra"], v)

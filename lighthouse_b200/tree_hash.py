@@ -154,7 +154,7 @@ def beacon_block_roots_deneb(blocks, want_body_roots=False, blinded=False):
 
 def beacon_block_roots(blocks, fork="deneb", want_body_roots=False, blinded=False):
     """canonical_root of a batch of BeaconBlock<fork> (or BlindedBeaconBlock<fork>) SSZ blobs, fork in altair / bellatrix /
-    capella / deneb (beacon_block.rs:41-90): lhb200_beacon_block_roots."""
+    capella / deneb / electra (beacon_block.rs:41-90): lhb200_beacon_block_roots."""
     blocks = [bytes(b) for b in blocks]
     n = len(blocks)
     offs = (C.c_uint64 * (n + 1))()
