@@ -117,7 +117,6 @@ struct Plan {
             lit_src.push_back({(uint32_t)(lit.size() / 32), (uint32_t)n, (uint64_t)(p - ssz_base)});
         return literal_raw(c);
     }
-    uint64_t literal(const uint8_t chunk[32]) { return literal_bytes(chunk, 32); }
     uint64_t literal_u64(uint64_t v) {
         uint8_t c[32] = {0};
         for (int k = 0; k < 8; k++) c[k] = (uint8_t)(v >> (8 * k));
@@ -453,8 +452,9 @@ static int32_t run_simple(const uint8_t* h_in, size_t in_bytes, uint8_t out[32],
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// BeaconState (mainnet preset): the fixed-part offsets every post-Altair fork shares, then the later forks' appended
-// fields.  See DESIGN.md §3 / oracle for the derivation.
+// SSZ layouts (mainnet preset).  Forks only append fields to a container, so every field sits at the same offset in
+// each fork that has it: the positions below hold for all forks, and a fork's row in FORK_LAYOUTS says how many of
+// the fields it has, how large the fixed parts are and which limits apply.
 namespace state_layout {
 constexpr uint32_t O_GENESIS_TIME = 0, O_GVR = 8, O_SLOT = 40, O_FORK = 48, O_LBH = 64, O_BLOCK_ROOTS = 176,
                    O_STATE_ROOTS = 262320, O_HIST_OFF = 524464, O_ETH1_DATA = 524468, O_VOTES_OFF = 524540,
@@ -464,9 +464,78 @@ constexpr uint32_t O_GENESIS_TIME = 0, O_GVR = 8, O_SLOT = 40, O_FORK = 48, O_LB
                    O_NSC = 2712005, O_LEPH_OFF = 2736629, O_NWI = 2736633, O_NWVI = 2736641, O_HS_OFF = 2736649,
                    O_ELECTRA_U64 = 2736653, O_PBD_OFF = 2736701, O_PPW_OFF = 2736705, O_PC_OFF = 2736709;
 constexpr uint32_t SYNC_COMMITTEE_BYTES = 513 * 48;
+// offsets of the variable-size fields, in field order
+constexpr uint32_t VAR_POS[] = {O_HIST_OFF, O_VOTES_OFF, O_VAL_OFF, O_BAL_OFF, O_PP_OFF, O_CP_OFF, O_INACT_OFF,
+                                O_LEPH_OFF, O_HS_OFF, O_PBD_OFF, O_PPW_OFF, O_PC_OFF};
+enum { V_HIST, V_VOTES, V_VAL, V_BAL, V_PP, V_CP, V_INACT, V_LEPH, V_HS, V_PBD, V_PPW, V_PC, N_VAR };
 }  // namespace state_layout
 
+namespace block_layout {
+constexpr uint32_t BLOCK_FIXED = 84, BLOCK_VAR_POS[] = {80};   // body
+// BeaconBlockBody: proposer_slashings, attester_slashings, attestations, deposits, voluntary_exits, execution_payload,
+// bls_to_execution_changes, blob_kzg_commitments, consolidations
+constexpr uint32_t BODY_VAR_POS[] = {200, 204, 208, 212, 216, 380, 384, 388, 392};
+enum { B_PROPOSER_SLASHINGS, B_ATTESTER_SLASHINGS, B_ATTESTATIONS, B_DEPOSITS, B_EXITS, B_PAYLOAD, B_BLS_CHANGES,
+       B_KZG_COMMITMENTS, B_CONSOLIDATIONS, N_BODY_VAR };
+// ExecutionPayload: extra_data, transactions, withdrawals, deposit_requests, withdrawal_requests; the header has the
+// same extra_data offset and no other variable-size field
+constexpr uint32_t PAYLOAD_VAR_POS[] = {436, 504, 508, 528, 532}, HEADER_VAR_POS[] = {436};
+enum { P_EXTRA_DATA, P_TRANSACTIONS, P_WITHDRAWALS, P_DEPOSIT_REQUESTS, P_WITHDRAWAL_REQUESTS, N_PAYLOAD_VAR };
+constexpr uint32_t PAYLOAD_PREFIX_FIELDS = 13;   // parent_hash .. block_hash: the same in payload and header
+// Attestation and IndexedAttestation: the bit or index list is the first field; AttesterSlashing: two
+// IndexedAttestations behind an 8-byte fixed part
+constexpr uint32_t FIRST_VAR_POS[] = {0}, ATTESTER_SLASHING_VAR_POS[] = {0, 4};
+}  // namespace block_layout
+
+// One row per fork from Altair to Electra (beacon_state.rs:224-571, beacon_block_body.rs:43-121,
+// execution_payload.rs:54-101, execution_payload_header.rs:46-93, attestation.rs:76-82; limits eth_spec.rs:389-440).
+struct ForkLayout {
+    int state_fields, body_fields, payload_fields;   // payload_fields: also the header's; 0 before Bellatrix
+    uint32_t state_fixed, header_fixed, body_fixed, payload_fixed, attestation_fixed;
+    // Attestation.aggregation_bits, IndexedAttestation.attesting_indices, BeaconBlockBody.{attestations, attester_slashings}
+    uint64_t max_aggregation_bits, max_attesting_indices, max_attestations, max_attester_slashings;
+};
+constexpr ForkLayout FORK_LAYOUTS[] = {
+    // fields: state, body, payload   fixed parts: state, header, body, payload, attestation   limits
+    {24,  9,  0, 2736629,   0, 380,   0, 228,   2048,   2048, 128, 2},   // Altair
+    {25, 10, 14, 2736633, 536, 384, 508, 228,   2048,   2048, 128, 2},   // Bellatrix
+    {28, 11, 15, 2736653, 568, 388, 512, 228,   2048,   2048, 128, 2},   // Capella
+    {28, 12, 17, 2736653, 584, 392, 528, 228,   2048,   2048, 128, 2},   // Deneb
+    {37, 13, 19, 2736713, 648, 396, 536, 236, 131072, 131072,   8, 1},   // Electra
+};
+static const ForkLayout* fork_layout(int32_t fork) {
+    return fork >= LHB200_FORK_ALTAIR && fork <= LHB200_FORK_ELECTRA ? &FORK_LAYOUTS[fork - LHB200_FORK_ALTAIR] : nullptr;
+}
+constexpr int MAX_FIELDS = FORK_LAYOUTS[LHB200_FORK_ELECTRA - LHB200_FORK_ALTAIR].state_fields;   // the widest state
+// chunk-tree depth of a packed list of at most `nbytes` bytes
+static inline uint32_t packed_depth(uint64_t nbytes) { return ceil_log2(ceil_div(nbytes, 32)); }
+
 static inline uint32_t rd32(const uint8_t* p) { return p[0] | (p[1] << 8) | (p[2] << 16) | ((uint32_t)p[3] << 24); }
+
+// Bytes [off, off + len) of one variable-size field, relative to its container.
+struct Span {
+    uint64_t off, len;
+    // a whole number of `item`-byte items, at most `limit` of them
+    bool fits(uint64_t item, uint64_t limit) const { return len % item == 0 && len / item <= limit; }
+};
+// The variable-size fields of the SSZ container s[0, len) with a `fixed`-byte fixed part: field k's offset is at
+// pos[k].  A field whose offset would lie past the fixed part is one this fork does not have (forks only append), is
+// not read and gets an empty span at the end.  False unless the first offset is the fixed size, the offsets never
+// decrease and the last is at most len.
+template <size_t N>
+static bool read_offsets(const uint8_t* s, uint64_t len, uint32_t fixed, const uint32_t (&pos)[N], Span (&span)[N]) {
+    if (len < fixed) return false;
+    uint64_t at[N + 1];
+    size_t n = 0;
+    for (; n < N && pos[n] + 4 <= fixed; n++) {
+        at[n] = rd32(s + pos[n]);
+        if (n == 0 ? at[0] != fixed : at[n] < at[n - 1]) return false;
+    }
+    if (n && at[n - 1] > len) return false;
+    for (size_t k = n; k <= N; k++) at[k] = len;
+    for (size_t k = 0; k < N; k++) span[k] = {at[k], at[k + 1] - at[k]};
+    return true;
+}
 
 }  // namespace lhb200
 
@@ -483,7 +552,7 @@ struct StageCopy {
 
 struct ShardCfg {
     uint32_t rank = 0, world = 1;
-    int32_t fork = LHB200_FORK_DENEB;   // which BeaconState variant the SSZ is (fork_spec)
+    int32_t fork = LHB200_FORK_DENEB;   // which BeaconState variant the SSZ is (FORK_LAYOUTS)
 };
 struct ShardedList {
     int field;            // index in the state container
@@ -511,7 +580,7 @@ struct lhb200_state {
     uint8_t* arena = nullptr;
     size_t arena_bytes = 0;
     lhb200::Plan plan;
-    uint64_t field_ops[40];   // MAX_FIELDS (declared below) rounded up
+    uint64_t field_ops[lhb200::MAX_FIELDS];
     uint64_t root_op = 0;
     lhb200::HashOp* d_gather = nullptr;   // operand table: root_op, field_ops, then the sharded lists' local_op
     uint8_t* d_result = nullptr;  // (1 + MAX_FIELDS) * 32 bytes: root + field roots gathered
@@ -542,67 +611,85 @@ struct lhb200_state {
 
 namespace lhb200 {
 
-// Describe the whole Deneb state.  `s` = host SSZ (read for offsets and small literal fields only).
-// Big fields are placed in the arena by `place(src_off, nbytes)` which records an H2D copy.
-// The post-Altair BeaconState variants (consensus/types/src/beacon_state.rs:224-571) share the first 24 fields and
-// their fixed-part offsets; later forks APPEND fields and widen the execution payload header:
-//   Altair     24 fields                                                        fixed part 2 736 629 B
-//   Bellatrix  + latest_execution_payload_header (14 fields, 536 B fixed)       2 736 633 B
-//   Capella    header + withdrawals_root (15 fields, 568 B); + next_withdrawal_index, next_withdrawal_validator_index,
-//              historical_summaries                                             2 736 653 B
-//   Deneb      header + blob_gas_used, excess_blob_gas (17 fields, 584 B)       2 736 653 B
-// so one describer covers them all; the kernels are fork-agnostic.
-constexpr int MAX_FIELDS = 37;   // BeaconStateElectra; the field-root block of a handle is root + MAX_FIELDS chunks
-struct ForkSpec {
-    int n_fields;        // 24 / 25 / 28 / 28 / 37
-    uint32_t fixed;      // bytes of the fixed part
-    uint32_t hdr_fixed;  // fixed part of the execution payload header (0: no header)
-    int hdr_fields;
-};
-static bool fork_spec(int32_t fork, ForkSpec* f) {
-    switch (fork) {
-        case LHB200_FORK_ALTAIR: *f = {24, 2736629, 0, 0}; return true;
-        case LHB200_FORK_BELLATRIX: *f = {25, 2736633, 536, 14}; return true;
-        case LHB200_FORK_CAPELLA: *f = {28, 2736653, 568, 15}; return true;
-        case LHB200_FORK_DENEB: *f = {28, 2736653, 584, 17}; return true;
-        case LHB200_FORK_ELECTRA: *f = {37, 2736713, 648, 19}; return true;
-    }
-    return false;
-}
+// The containers a BeaconState and a BeaconBlock share, described into a plan.  `s` = host SSZ bytes; `d` = the same
+// bytes on the device, whose byte strings k_byte_items hashes in place, or null when there is no device copy (a staged
+// state keeps only its big lists there): byte strings then become literal chunks, whose SSZ provenance
+// lhb200_state_patch uses to find edits.  Malformed input sets `bad`.
+struct SszDescriber {
+    Plan& p;
+    const uint8_t* s;
+    const uint8_t* d;
+    const ForkLayout& fl;
+    bool bad = false;
 
+    uint64_t fail() { bad = true; return 0; }
+    uint64_t u64(uint64_t off) { return p.literal_bytes(s + off, 8); }
+    uint64_t h256(uint64_t off) { return p.literal_bytes(s + off, 32); }
+    uint64_t addr20(uint64_t off) { return p.literal_bytes(s + off, 20); }
+    uint64_t checkpoint(uint64_t off) {                                                                  // 40 B
+        const uint64_t epoch = u64(off);
+        return p.op_hash(epoch, h256(off + 8));
+    }
+    uint64_t eth1_data(uint64_t off) { return p.container({h256(off), u64(off + 32), h256(off + 40)}); }  // 72 B
+    uint64_t block_header(uint64_t off) {                                                                // 112 B
+        return p.container({u64(off), u64(off + 8), h256(off + 16), h256(off + 48), h256(off + 80)});
+    }
+    // logs_bloom: ByteVector[256]
+    uint64_t bloom(uint64_t off) {
+        if (d) return p.bytes_item(d + off, 256, 3, false);
+        std::vector<uint64_t> chunks;
+        for (int i = 0; i < 8; i++) chunks.push_back(h256(off + 32 * i));
+        return p.small_tree(chunks, 3);
+    }
+    // extra_data: ByteList[32] at s[off, off + n)
+    uint64_t extra_data(uint64_t off, uint64_t n) {
+        if (d) return p.bytes_item(d + off, n, 0, true, n);
+        return p.mix_in_length(p.literal_bytes(s + off, n), n);
+    }
+    // The first fields of ExecutionPayload and ExecutionPayloadHeader (execution_payload.rs:54-95), extra_data checked
+    // by the caller
+    std::vector<uint64_t> payload_prefix(uint64_t off, Span extra) {
+        return {h256(off), addr20(off + 32), h256(off + 52), h256(off + 84), bloom(off + 116), h256(off + 372),
+                u64(off + 404), u64(off + 412), u64(off + 420), u64(off + 428), extra_data(off + extra.off, extra.len),
+                h256(off + 440), h256(off + 472)};
+    }
+    // ExecutionPayloadHeader (execution_payload_header.rs:46-93): the prefix, then transactions_root, withdrawals_root,
+    // blob_gas_used, excess_blob_gas, deposit_requests_root, withdrawal_requests_root up to the fork's payload field count
+    uint64_t payload_header(uint64_t off, uint64_t len) {
+        static constexpr struct { uint32_t off, n; } TAIL[] = {{504, 32}, {536, 32}, {568, 8}, {576, 8}, {584, 32}, {616, 32}};
+        Span v[1];
+        if (!read_offsets(s + off, len, fl.header_fixed, block_layout::HEADER_VAR_POS, v) || !v[0].fits(1, 32)) return fail();
+        std::vector<uint64_t> f = payload_prefix(off, v[0]);
+        for (int k = block_layout::PAYLOAD_PREFIX_FIELDS; k < fl.payload_fields; k++) {
+            const auto& t = TAIL[k - block_layout::PAYLOAD_PREFIX_FIELDS];
+            f.push_back(p.literal_bytes(s + off + t.off, t.n));
+        }
+        return p.container(f);
+    }
+};
+
+// Describe a whole BeaconState of any fork.  `s` = host SSZ (read for offsets and small literal fields only).
+// Big fields are placed in the arena by `place(src_off, nbytes)` which records an H2D copy.  The fields every fork has
+// come first, then the ones later forks append, up to the fork's field count.
 static int32_t describe_state(Plan& p, const uint8_t* s, uint64_t len, std::vector<StageCopy>* copies,
                               uint64_t* field_ops, uint64_t* root_op, ShardCfg sh, std::vector<ShardedList>* sharded) {
     using namespace state_layout;
-    ForkSpec fk;
-    if (!fork_spec(sh.fork, &fk)) { set_error("unknown fork id %d", sh.fork); return LHB200_EINVAL; }
-    const uint32_t FIXED = fk.fixed;
-    if (len < FIXED) { set_error("BeaconState SSZ shorter than its fixed part"); return LHB200_EINVAL; }
-    const uint32_t o_hist = rd32(s + O_HIST_OFF), o_votes = rd32(s + O_VOTES_OFF), o_val = rd32(s + O_VAL_OFF),
-                   o_bal = rd32(s + O_BAL_OFF), o_pp = rd32(s + O_PP_OFF), o_cp = rd32(s + O_CP_OFF),
-                   o_inact = rd32(s + O_INACT_OFF);
-    const uint32_t o_leph = fk.hdr_fields ? rd32(s + O_LEPH_OFF) : (uint32_t)len;
-    const uint32_t o_hs = fk.n_fields >= 28 ? rd32(s + O_HS_OFF) : (uint32_t)len;
-    const bool electra = fk.n_fields == 37;
-    const uint32_t o_pbd = electra ? rd32(s + O_PBD_OFF) : (uint32_t)len, o_ppw = electra ? rd32(s + O_PPW_OFF) : (uint32_t)len,
-                   o_pc = electra ? rd32(s + O_PC_OFF) : (uint32_t)len;
-    if (o_hist != FIXED || !(o_hist <= o_votes && o_votes <= o_val && o_val <= o_bal && o_bal <= o_pp &&
-                             o_pp <= o_cp && o_cp <= o_inact && o_inact <= o_leph && o_leph <= o_hs && o_hs <= o_pbd &&
-                             o_pbd <= o_ppw && o_ppw <= o_pc && o_pc <= len)) {
-        set_error("BeaconState SSZ: inconsistent variable-part offsets");
+    const ForkLayout* fl = fork_layout(sh.fork);
+    if (!fl) { set_error("unknown fork id %d", sh.fork); return LHB200_EINVAL; }
+    Span v[N_VAR];
+    if (!read_offsets(s, len, fl->state_fixed, VAR_POS, v)) {
+        set_error("BeaconState SSZ: shorter than its fixed part or inconsistent variable-part offsets");
         return LHB200_EINVAL;
     }
-    const uint64_t n_hist = (o_votes - o_hist) / 32, n_votes = (o_val - o_votes) / 72, n_val = (o_bal - o_val) / 121,
-                   n_bal = (o_pp - o_bal) / 8, n_pp = o_cp - o_pp, n_cp = o_inact - o_cp,
-                   n_inact = (o_leph - o_inact) / 8, leph_len = o_hs - o_leph, n_hs = (o_pbd - o_hs) / 64,
-                   n_pbd = (o_ppw - o_pbd) / 16, n_ppw = (o_pc - o_ppw) / 24, n_pc = (len - o_pc) / 16;
-    if ((o_votes - o_hist) % 32 || (o_val - o_votes) % 72 || (o_bal - o_val) % 121 || (o_pp - o_bal) % 8 ||
-        (o_leph - o_inact) % 8 || (o_pbd - o_hs) % 64 || (o_ppw - o_pbd) % 16 || (o_pc - o_ppw) % 24 || (len - o_pc) % 16 ||
-        n_pbd > (1u << 27) || n_ppw > (1u << 27) || n_pc > (1u << 18) ||
-        (fk.hdr_fields && (leph_len < fk.hdr_fixed || leph_len > fk.hdr_fixed + 32 || rd32(s + o_leph + 436) != fk.hdr_fixed)) ||
-        n_votes > 2048 || n_hist > (1u << 24) || n_hs > (1u << 24)) {
+    if (!v[V_HIST].fits(32, 1u << 24) || !v[V_VOTES].fits(72, 2048) || !v[V_VAL].fits(121, 1ull << 40) ||
+        !v[V_BAL].fits(8, 1ull << 40) || !v[V_INACT].fits(8, 1ull << 40) || !v[V_HS].fits(64, 1u << 24) ||
+        !v[V_PBD].fits(16, 1u << 27) || !v[V_PPW].fits(24, 1u << 27) || !v[V_PC].fits(16, 1u << 18)) {
         set_error("BeaconState SSZ: malformed variable part");
         return LHB200_EINVAL;
     }
+    const uint64_t n_hist = v[V_HIST].len / 32, n_val = v[V_VAL].len / 121, n_bal = v[V_BAL].len / 8,
+                   n_pp = v[V_PP].len, n_cp = v[V_CP].len, n_inact = v[V_INACT].len / 8;
+    SszDescriber c{p, s, nullptr, *fl};
     p.ssz_base = s;
     p.ssz_len = len;
     auto place = [&](size_t src_off, size_t nbytes) -> uint8_t* {
@@ -611,7 +698,6 @@ static int32_t describe_state(Plan& p, const uint8_t* s, uint64_t len, std::vect
         if (copies) copies->push_back({src_off, nbytes, d, padded});
         return d;
     };
-    auto chunk = [&](uint32_t off) { return p.literal(s + off); };
     uint64_t* f = field_ops;
     const uint32_t lg_world = ceil_log2(sh.world);
     // Big list with `n_chunks` leaf chunks produced from `n_items` source items of `item_bytes` at `src_off`
@@ -650,17 +736,16 @@ static int32_t describe_state(Plan& p, const uint8_t* s, uint64_t len, std::vect
         sharded->push_back({field, sub, limit_depth, mix_len, op});
         return Plan::zero_op(0);       // placeholder; the field root is formed in lhb200_state_combine
     };
-    // list of n fixed-size records (one leaf-kernel root each) with limit 2^depth
-    auto records = [&](LeafKind leaf, uint32_t off, uint64_t n, uint32_t item_bytes, uint32_t depth) {
-        return p.mix_in_length(p.merkle_list(p.leaf_kernel(leaf, place(off, n * item_bytes), n), n, depth), n);
+    // list of fixed-size records (one leaf-kernel root each) with limit 2^depth
+    auto records = [&](LeafKind leaf, Span x, uint32_t item_bytes, uint32_t depth) {
+        const uint64_t n = x.len / item_bytes;
+        return p.mix_in_length(p.merkle_list(p.leaf_kernel(leaf, place(x.off, x.len), n), n, depth), n);
     };
-    f[0] = p.literal_bytes(s + O_GENESIS_TIME, 8);
-    f[1] = chunk(O_GVR);
-    f[2] = p.literal_bytes(s + O_SLOT, 8);
-    f[3] = p.container({p.literal_bytes(s + O_FORK, 4), p.literal_bytes(s + O_FORK + 4, 4),
-                        p.literal_bytes(s + O_FORK + 8, 8)});
-    f[4] = p.container({p.literal_bytes(s + O_LBH, 8), p.literal_bytes(s + O_LBH + 8, 8), chunk(O_LBH + 16),
-                        chunk(O_LBH + 48), chunk(O_LBH + 80)});
+    f[0] = c.u64(O_GENESIS_TIME);
+    f[1] = c.h256(O_GVR);
+    f[2] = c.u64(O_SLOT);
+    f[3] = p.container({p.literal_bytes(s + O_FORK, 4), p.literal_bytes(s + O_FORK + 4, 4), c.u64(O_FORK + 8)});
+    f[4] = c.block_header(O_LBH);
     auto plain_vector = [&](uint32_t off, uint64_t nbytes, uint32_t depth) {   // fixed vectors of chunks / packed u64
         const uint8_t* src = place(off, nbytes);
         const size_t nt = p.trees.size();
@@ -673,53 +758,40 @@ static int32_t describe_state(Plan& p, const uint8_t* s, uint64_t len, std::vect
     };
     f[5] = plain_vector(O_BLOCK_ROOTS, 8192 * 32, 13);
     f[6] = plain_vector(O_STATE_ROOTS, 8192 * 32, 13);
-    f[7] = p.mix_in_length(p.merkle_list(place(o_hist, n_hist * 32), n_hist, 24), n_hist);
-    f[8] = p.container({chunk(O_ETH1_DATA), p.literal_bytes(s + O_ETH1_DATA + 32, 8), chunk(O_ETH1_DATA + 40)});
-    f[9] = records(LEAF_ETH1_DATA, o_votes, n_votes, 72, 11);
-    f[10] = p.literal_bytes(s + O_DEPOSIT_INDEX, 8);
-    f[11] = big_list(11, o_val, n_val, 121, LEAF_VALIDATOR, n_val, 40, n_val);
-    f[12] = big_list(12, o_bal, n_bal, 8, LEAF_NONE, ceil_div(n_bal * 8, 32), 38, n_bal);
+    f[7] = p.mix_in_length(p.merkle_list(place(v[V_HIST].off, v[V_HIST].len), n_hist, 24), n_hist);
+    f[8] = c.eth1_data(O_ETH1_DATA);
+    f[9] = records(LEAF_ETH1_DATA, v[V_VOTES], 72, 11);
+    f[10] = c.u64(O_DEPOSIT_INDEX);
+    f[11] = big_list(11, v[V_VAL].off, n_val, 121, LEAF_VALIDATOR, n_val, 40, n_val);
+    f[12] = big_list(12, v[V_BAL].off, n_bal, 8, LEAF_NONE, ceil_div(n_bal * 8, 32), 38, n_bal);
     f[13] = big_list(13, O_RANDAO, 65536, 32, LEAF_NONE, 65536, 16, UINT64_MAX);
     f[14] = plain_vector(O_SLASHINGS, 8192 * 8, 11);
-    f[15] = big_list(15, o_pp, n_pp, 1, LEAF_NONE, ceil_div(n_pp, 32), 35, n_pp);
-    f[16] = big_list(16, o_cp, n_cp, 1, LEAF_NONE, ceil_div(n_cp, 32), 35, n_cp);
+    f[15] = big_list(15, v[V_PP].off, n_pp, 1, LEAF_NONE, ceil_div(n_pp, 32), 35, n_pp);
+    f[16] = big_list(16, v[V_CP].off, n_cp, 1, LEAF_NONE, ceil_div(n_cp, 32), 35, n_cp);
     f[17] = p.literal_bytes(s + O_JUST, 1);
-    f[18] = p.container({p.literal_bytes(s + O_PJC, 8), chunk(O_PJC + 8)});
-    f[19] = p.container({p.literal_bytes(s + O_CJC, 8), chunk(O_CJC + 8)});
-    f[20] = p.container({p.literal_bytes(s + O_FC, 8), chunk(O_FC + 8)});
-    f[21] = big_list(21, o_inact, n_inact, 8, LEAF_NONE, ceil_div(n_inact * 8, 32), 38, n_inact);
+    f[18] = c.checkpoint(O_PJC);
+    f[19] = c.checkpoint(O_CJC);
+    f[20] = c.checkpoint(O_FC);
+    f[21] = big_list(21, v[V_INACT].off, n_inact, 8, LEAF_NONE, ceil_div(n_inact * 8, 32), 38, n_inact);
     for (int k = 0; k < 2; k++) {
         uint8_t* roots = p.leaf_kernel(LEAF_PUBKEY, place(k ? O_NSC : O_CSC, SYNC_COMMITTEE_BYTES), 513);
         f[22 + k] = p.container({p.merkle_list(roots, 512, 9), reinterpret_cast<uint64_t>(roots + 512 * 32)});
     }
-    if (fk.hdr_fields) {
-        const uint8_t* h = s + o_leph;
-        std::vector<uint64_t> bloom;
-        for (int i = 0; i < 8; i++) bloom.push_back(p.literal(h + 116 + 32 * i));
-        const uint64_t extra_len = leph_len - fk.hdr_fixed;
-        std::vector<uint64_t> hf = {p.literal(h), p.literal_bytes(h + 32, 20), p.literal(h + 52), p.literal(h + 84),
-                                    p.small_tree(bloom, 3), p.literal(h + 372), p.literal_bytes(h + 404, 8),
-                                    p.literal_bytes(h + 412, 8), p.literal_bytes(h + 420, 8), p.literal_bytes(h + 428, 8),
-                                    p.mix_in_length(p.literal_bytes(h + fk.hdr_fixed, extra_len), extra_len),
-                                    p.literal(h + 440), p.literal(h + 472), p.literal(h + 504)};
-        if (fk.hdr_fields >= 15) hf.push_back(p.literal(h + 536));                       // withdrawals_root (Capella)
-        if (fk.hdr_fields >= 17) { hf.push_back(p.literal_bytes(h + 568, 8)); hf.push_back(p.literal_bytes(h + 576, 8)); }
-        if (fk.hdr_fields >= 19) { hf.push_back(p.literal(h + 584)); hf.push_back(p.literal(h + 616)); }   // request roots (Electra)
-        f[24] = p.container(hf);
+    for (int k = 24; k < fl->state_fields; k++) {   // appended by later forks (beacon_state.rs:339-525)
+        switch (k) {
+            case 24: f[k] = c.payload_header(v[V_LEPH].off, v[V_LEPH].len); break;
+            case 25: f[k] = c.u64(O_NWI); break;
+            case 26: f[k] = c.u64(O_NWVI); break;
+            case 27: f[k] = records(LEAF_CHUNK_PAIR, v[V_HS], 64, 24); break;
+            case 34: f[k] = records(LEAF_U64_PAIR, v[V_PBD], 16, 27); break;
+            case 35: f[k] = records(LEAF_U64_TRIPLE, v[V_PPW], 24, 27); break;
+            case 36: f[k] = records(LEAF_U64_PAIR, v[V_PC], 16, 18); break;
+            default: f[k] = c.u64(O_ELECTRA_U64 + 8 * (k - 28)); break;   // 28 .. 33
+        }
     }
-    if (fk.n_fields >= 28) {
-        f[25] = p.literal_bytes(s + O_NWI, 8);
-        f[26] = p.literal_bytes(s + O_NWVI, 8);
-        f[27] = records(LEAF_CHUNK_PAIR, o_hs, n_hs, 64, 24);
-    }
-    if (electra) {   // beacon_state.rs:487-525
-        for (int k = 0; k < 6; k++) f[28 + k] = p.literal_bytes(s + O_ELECTRA_U64 + 8 * k, 8);
-        f[34] = records(LEAF_U64_PAIR, o_pbd, n_pbd, 16, 27);
-        f[35] = records(LEAF_U64_TRIPLE, o_ppw, n_ppw, 24, 27);
-        f[36] = records(LEAF_U64_PAIR, o_pc, n_pc, 16, 18);
-    }
-    for (int k = fk.n_fields; k < MAX_FIELDS; k++) f[k] = Plan::zero_op(0);   // absent in this fork (not part of its container)
-    *root_op = p.container(std::vector<uint64_t>(f, f + fk.n_fields));
+    if (c.bad) { set_error("BeaconState SSZ: malformed execution payload header"); return LHB200_EINVAL; }
+    for (int k = fl->state_fields; k < MAX_FIELDS; k++) f[k] = Plan::zero_op(0);   // absent in this fork (not part of its container)
+    *root_op = p.container(std::vector<uint64_t>(f, f + fl->state_fields));
     return LHB200_OK;
 }
 
@@ -1467,71 +1539,58 @@ int32_t lhb200_verify_merkle_proofs(const uint8_t* leaves, const uint8_t* branch
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// BeaconBlockDeneb (mainnet preset): BeaconBlock::canonical_root (consensus/types/src/beacon_block.rs:158-160).
-// Layouts: beacon_block.rs:56-78 (84-byte fixed part), beacon_block_body.rs:70-121 (392), execution_payload.rs:54-95
-// (528); operation containers as cited in include/lhb200.h.  The host only walks SSZ offsets: every packed byte string
-// (transactions, signatures, pubkeys, bit lists, index lists, proofs, blooms) is hashed by k_byte_items straight
-// from the staged blob, fixed 8/20/32-byte fields become literal chunks, and the container structure above them is
-// a hash program.  `s` = host bytes, `d` = the same bytes on the device.
-// Electra (beacon_block_body.rs:70-121, limits eth_spec.rs:433-440): 396-byte body fixed part (+ consolidations offset at
-// 392), attestations with up to 131 072 aggregation bits and a committee bitvector before the signature (236-byte fixed
-// part, attestation.rs:76-82), indexed attestations with up to 131 072 indices, a 536-byte payload fixed part (+ offsets
-// of deposit_requests and withdrawal_requests at 528 / 532, execution_payload.rs:54-101).  The up to 8 192 DepositRequest
-// records are the one list of fixed-size containers in a block that can reach thousands of items: past 64 records,
-// k_record_roots kind 4 hashes them straight from the staged blob, the reduce passes fold them, and the host plans no
-// node per record.
+// BeaconBlock (mainnet preset) of any fork from Altair to Electra: BeaconBlock::canonical_root
+// (consensus/types/src/beacon_block.rs:158-160).  Layouts: beacon_block.rs:41-90, beacon_block_body.rs:43-121,
+// execution_payload.rs:54-101, sizes and limits per fork in FORK_LAYOUTS; operation containers as cited in
+// include/lhb200.h.  The host only walks SSZ offsets: every packed byte string (transactions, signatures, pubkeys,
+// bit lists, index lists, proofs, blooms) is hashed by k_byte_items straight from the staged blob, fixed 8/20/32-byte
+// fields become literal chunks, and the container structure above them is a hash program.  The up to 8 192
+// DepositRequest records of an Electra payload are the one list of fixed-size containers in a block that can reach
+// thousands of items: past 64 records, k_record_roots kind 4 hashes them straight from the staged blob, the reduce
+// passes fold them, and the host plans no node per record.
 }  // extern "C"
 namespace {
-struct BlockDescriber {
-    Plan& p;
-    const uint8_t* s;
-    const uint8_t* d;
-    bool bad = false;
-    bool blinded = false;   // BlindedBeaconBlock: field 9 of the body is an ExecutionPayloadHeader
-    int32_t fork = LHB200_FORK_DENEB;   // beacon_block_body.rs superstruct variant: Altair 9 body fields (no payload),
-                                        // Bellatrix 10 (14-field payload), Capella 11 (+ withdrawals, BLS changes), Deneb 12,
-                                        // Electra 13 (+ consolidations; 19-field payload, wider attestations)
+struct BlockDescriber : SszDescriber {
+    bool blinded = false;   // BlindedBeaconBlock: the body carries an ExecutionPayloadHeader
 
-    bool electra() const { return fork >= LHB200_FORK_ELECTRA; }
-    uint64_t u64(uint64_t off) { return p.literal_bytes(s + off, 8); }
-    uint64_t h256(uint64_t off) { return p.literal_bytes(s + off, 32); }
-    uint64_t addr20(uint64_t off) { return p.literal_bytes(s + off, 20); }
     uint64_t blob(uint64_t off, uint64_t n, uint32_t depth) { return p.bytes_item(d + off, n, depth, false); }
     uint64_t sig(uint64_t off) { return blob(off, 96, 2); }
     uint64_t pubkey(uint64_t off) { return blob(off, 48, 1); }
-    uint64_t checkpoint(uint64_t off) { return p.op_hash(u64(off), h256(off + 8)); }
     uint64_t att_data(uint64_t off) {  // 128 B (attestation_data.rs:28)
         return p.container({u64(off), u64(off + 8), h256(off + 16), checkpoint(off + 48), checkpoint(off + 88)});
     }
     uint64_t signed_header(uint64_t off) {  // 208 B
-        uint64_t h = p.container({u64(off), u64(off + 8), h256(off + 16), h256(off + 48), h256(off + 80)});
+        uint64_t h = block_header(off);
         return p.op_hash(h, sig(off + 112));
     }
     uint64_t proposer_slashing(uint64_t off) { return p.op_hash(signed_header(off), signed_header(off + 208)); }
-    // attesting_indices: List[u64, MaxValidatorsPerCommittee = 2048] (depth 9); Electra List[u64, MaxValidatorsPerSlot =
-    // 131072] (depth 15)
+    // IndexedAttestation: attesting_indices (List[u64]) behind a 228-byte fixed part
     uint64_t indexed_attestation(uint64_t off, uint64_t len) {
-        const uint64_t max_idx = electra() ? 131072 : 2048;
-        if (len < 228 || rd32(s + off) != 228 || (len - 228) % 8 || (len - 228) / 8 > max_idx) { bad = true; return 0; }
-        uint64_t idx = p.bytes_item(d + off + 228, len - 228, electra() ? 15 : 9, true, (len - 228) / 8);
+        Span v[1];
+        if (!read_offsets(s + off, len, 228, block_layout::FIRST_VAR_POS, v) || !v[0].fits(8, fl.max_attesting_indices))
+            return fail();
+        uint64_t idx = p.bytes_item(d + off + v[0].off, v[0].len, packed_depth(8 * fl.max_attesting_indices), true,
+                                    v[0].len / 8);
         return p.container({idx, att_data(off + 4), sig(off + 132)});
     }
-    // aggregation_bits: Bitlist[2048] (depth 3) behind a 228-byte fixed part; Electra Bitlist[131072] (depth 9) behind
-    // 236 bytes, with committee_bits (Bitvector[64]) between data and signature
+    // Attestation: aggregation_bits (Bitlist), data, then the signature at the end of the fixed part; Electra puts
+    // committee_bits (Bitvector[64]) between data and signature (attestation.rs:76-82)
     uint64_t attestation(uint64_t off, uint64_t len) {
-        const uint32_t fixed = electra() ? 236 : 228;
-        if (len < fixed + 1 || rd32(s + off) != fixed || s[off + len - 1] == 0) { bad = true; return 0; }
-        const uint64_t nb = len - fixed;
+        const uint32_t fixed = fl.attestation_fixed, o_sig = fixed - 96;
+        Span v[1];
+        if (!read_offsets(s + off, len, fixed, block_layout::FIRST_VAR_POS, v) || v[0].len == 0 || s[off + len - 1] == 0)
+            return fail();
         const uint8_t last = s[off + len - 1];
         int top = 7;
         while (!((last >> top) & 1)) top--;
-        const uint64_t bitlen = 8 * (nb - 1) + (uint64_t)top;
-        if (bitlen > (electra() ? 131072u : 2048u)) { bad = true; return 0; }
+        const uint64_t bitlen = 8 * (v[0].len - 1) + (uint64_t)top;
+        if (bitlen > fl.max_aggregation_bits) return fail();
         // drop the delimiter: either the whole last byte (top == 0) or its top bit
-        uint64_t bits = p.bytes_item(d + off + fixed, (bitlen + 7) / 8, electra() ? 9 : 3, true, bitlen,
-                                     top ? (uint32_t)((1u << top) - 1) : 0xff);
-        if (electra()) return p.container({bits, att_data(off + 4), p.literal_bytes(s + off + 132, 8), sig(off + 140)});
-        return p.container({bits, att_data(off + 4), sig(off + 132)});
+        uint64_t bits = p.bytes_item(d + off + fixed, (bitlen + 7) / 8, packed_depth(fl.max_aggregation_bits / 8), true,
+                                     bitlen, top ? (uint32_t)((1u << top) - 1) : 0xff);
+        const uint64_t data = att_data(off + 4);
+        if (o_sig > 132) return p.container({bits, data, u64(off + 132), sig(off + o_sig)});   // + committee_bits
+        return p.container({bits, data, sig(off + o_sig)});
     }
     uint64_t deposit(uint64_t off) {  // 1240 B
         uint64_t data = p.container({pubkey(off + 1056), h256(off + 1104), u64(off + 1136), sig(off + 1144)});
@@ -1547,6 +1606,15 @@ struct BlockDescriber {
     uint64_t deposit_request(uint64_t off) {
         return p.container({pubkey(off), h256(off + 48), u64(off + 80), sig(off + 88), u64(off + 184)});
     }
+    // List[DepositRequest, 8192] at span x of the payload at `base`: depth 13.  The record kernel and its reduce pass add
+    // two serial launches per block (k_record_roots is one thread's chain of 10 hashes); host planning costs ~0.7 us per
+    // record.  On an H100 the ops are faster up to 64 records and the kernel past that (DESIGN §3.5).
+    uint64_t deposit_requests(uint64_t base, Span x) {
+        const uint64_t n = x.len / 192;
+        if (n <= DEPOSIT_REQUESTS_AS_OPS || !x.fits(192, 8192))   // fixed_list refuses a malformed list
+            return fixed_list(base, x, 192, 13, [&](uint64_t o) { return deposit_request(o); });
+        return p.mix_in_length(p.merkle_list(p.leaf_kernel(LEAF_DEPOSIT_REQUEST, d + base + x.off, n), n, 13), n);
+    }
     // ExecutionLayerWithdrawalRequest (execution_layer_withdrawal_request.rs:23-26): 76 B
     uint64_t withdrawal_request(uint64_t off) { return p.container({addr20(off), pubkey(off + 20), u64(off + 68)}); }
     // SignedConsolidation (signed_consolidation.rs:23-24, consolidation.rs:24-27): 120 B
@@ -1560,11 +1628,12 @@ struct BlockDescriber {
         else for (uint32_t l = ceil_log2(n); l < limit_log; l++) r = p.op_hash(r, Plan::zero_op(l));
         return p.mix_in_length(r, n);
     }
+    // list of `item`-byte containers at span x of the container at `base`, limit 2^limit_log
     template <class F>
-    uint64_t fixed_list(uint64_t off, uint64_t len, uint32_t item, uint32_t limit_log, F&& f) {
-        if (len % item || len / item > (1ull << limit_log)) { bad = true; return 0; }
+    uint64_t fixed_list(uint64_t base, Span x, uint32_t item, uint32_t limit_log, F&& f) {
+        if (!x.fits(item, 1ull << limit_log)) return fail();
         std::vector<uint64_t> roots;
-        for (uint64_t i = 0; i < len / item; i++) roots.push_back(f(off + item * i));
+        for (uint64_t i = 0; i < x.len / item; i++) roots.push_back(f(base + x.off + item * i));
         return list_of(roots, limit_log);
     }
     // offsets table of a list of variable-size items occupying [off, off+len)
@@ -1580,111 +1649,73 @@ struct BlockDescriber {
             if (b[i] > b[i + 1]) return false;
         return true;
     }
+    // ExecutionPayload: the prefix and transactions, then the fields later forks append
     uint64_t payload(uint64_t off, uint64_t len) {
-        // fixed part: 508 B (Bellatrix: ... transactions offset), 512 (Capella: + withdrawals offset), 528 (Deneb: + blob gas),
-        // 536 (Electra: + deposit_requests and withdrawal_requests offsets)
-        const bool has_wd = fork >= LHB200_FORK_CAPELLA, has_blob = fork >= LHB200_FORK_DENEB, has_req = electra();
-        const uint32_t fixed = has_req ? 536 : has_blob ? 528 : has_wd ? 512 : 508;
-        if (len < fixed) { bad = true; return 0; }
-        const uint32_t o_extra = rd32(s + off + 436), o_tx = rd32(s + off + 504), o_wd = has_wd ? rd32(s + off + 508) : (uint32_t)len,
-                       o_dr = has_req ? rd32(s + off + 528) : (uint32_t)len, o_wr = has_req ? rd32(s + off + 532) : (uint32_t)len;
-        if (o_extra != fixed || o_tx < o_extra || o_tx - o_extra > 32 || o_wd < o_tx || o_wd > o_dr || (o_dr - o_wd) % 44 ||
-            (o_dr - o_wd) / 44 > 16 || o_wr < o_dr || o_wr > len || (o_wr - o_dr) % 192 || (o_wr - o_dr) / 192 > 8192 ||
-            (len - o_wr) % 76 || (len - o_wr) / 76 > 16) { bad = true; return 0; }
-        std::vector<uint64_t> f(14);
-        f[0] = h256(off); f[1] = addr20(off + 32); f[2] = h256(off + 52); f[3] = h256(off + 84);
-        f[4] = blob(off + 116, 256, 3);
-        f[5] = h256(off + 372); f[6] = u64(off + 404); f[7] = u64(off + 412); f[8] = u64(off + 420); f[9] = u64(off + 428);
-        f[10] = p.bytes_item(d + off + o_extra, o_tx - o_extra, 0, true, o_tx - o_extra);
-        f[11] = h256(off + 440); f[12] = h256(off + 472);
-        std::vector<uint64_t> b, roots;
-        if (!var_bounds(off + o_tx, o_wd - o_tx, 1u << 20, b)) { bad = true; return 0; }
+        using namespace block_layout;
+        Span v[N_PAYLOAD_VAR];
+        if (!read_offsets(s + off, len, fl.payload_fixed, PAYLOAD_VAR_POS, v) || !v[P_EXTRA_DATA].fits(1, 32)) return fail();
+        std::vector<uint64_t> f = payload_prefix(off, v[P_EXTRA_DATA]), b, roots;
+        const Span tx = v[P_TRANSACTIONS];
+        if (!var_bounds(off + tx.off, tx.len, 1u << 20, b)) return fail();
         for (size_t i = 0; i + 1 < b.size(); i++)  // ByteList[2^30]: 2^25 chunks
-            roots.push_back(p.bytes_item(d + off + o_tx + b[i], b[i + 1] - b[i], 25, true, b[i + 1] - b[i]));
-        f[13] = list_of(roots, 20);
-        if (has_wd) f.push_back(fixed_list(off + o_wd, o_dr - o_wd, 44, 4, [&](uint64_t o) { return withdrawal(o); }));
-        if (has_blob) { f.push_back(u64(off + 512)); f.push_back(u64(off + 520)); }
-        if (has_req) {
-            // List[DepositRequest, 8192]: depth 13.  The record kernel and its reduce pass add two serial launches per
-            // block (k_record_roots is one thread's chain of 10 hashes); host planning costs ~0.7 us per record.  On an
-            // H100 the ops are faster up to 64 records and the kernel past that (DESIGN §3.5).
-            const uint64_t n_dr = (o_wr - o_dr) / 192;
-            if (n_dr <= DEPOSIT_REQUESTS_AS_OPS)
-                f.push_back(fixed_list(off + o_dr, o_wr - o_dr, 192, 13, [&](uint64_t o) { return deposit_request(o); }));
-            else
-                f.push_back(p.mix_in_length(p.merkle_list(p.leaf_kernel(LEAF_DEPOSIT_REQUEST, d + off + o_dr, n_dr), n_dr, 13), n_dr));
-            f.push_back(fixed_list(off + o_wr, len - o_wr, 76, 4, [&](uint64_t o) { return withdrawal_request(o); }));
+            roots.push_back(p.bytes_item(d + off + tx.off + b[i], b[i + 1] - b[i], 25, true, b[i + 1] - b[i]));
+        f.push_back(list_of(roots, 20));
+        for (int k = PAYLOAD_PREFIX_FIELDS + 1; k < fl.payload_fields && !bad; k++) {   // appended by later forks
+            switch (k) {
+                case 14: f.push_back(fixed_list(off, v[P_WITHDRAWALS], 44, 4, [&](uint64_t o) { return withdrawal(o); })); break;
+                case 15: case 16: f.push_back(u64(off + 512 + 8 * (k - 15))); break;   // blob_gas_used, excess_blob_gas
+                case 17: f.push_back(deposit_requests(off, v[P_DEPOSIT_REQUESTS])); break;
+                default: f.push_back(fixed_list(off, v[P_WITHDRAWAL_REQUESTS], 76, 4, [&](uint64_t o) { return withdrawal_request(o); }));
+            }
         }
-        return p.container(f);
-    }
-    // ExecutionPayloadHeaderDeneb (execution_payload_header.rs:46-87): 584-byte fixed part + extra_data
-    uint64_t payload_header(uint64_t off, uint64_t len) {
-        // 536-byte fixed part (Bellatrix, 14 fields), 568 (Capella: + withdrawals_root), 584 (Deneb: + blob gas),
-        // 648 (Electra: + deposit_requests_root, withdrawal_requests_root)
-        const bool has_wd = fork >= LHB200_FORK_CAPELLA, has_blob = fork >= LHB200_FORK_DENEB, has_req = electra();
-        const uint32_t fixed = has_req ? 648 : has_blob ? 584 : has_wd ? 568 : 536;
-        if (len < fixed || len > fixed + 32 || rd32(s + off + 436) != fixed) { bad = true; return 0; }
-        std::vector<uint64_t> f(14);
-        f[0] = h256(off); f[1] = addr20(off + 32); f[2] = h256(off + 52); f[3] = h256(off + 84);
-        f[4] = blob(off + 116, 256, 3);
-        f[5] = h256(off + 372); f[6] = u64(off + 404); f[7] = u64(off + 412); f[8] = u64(off + 420); f[9] = u64(off + 428);
-        f[10] = p.bytes_item(d + off + fixed, len - fixed, 0, true, len - fixed);
-        f[11] = h256(off + 440); f[12] = h256(off + 472);
-        f[13] = h256(off + 504);            // transactions_root
-        if (has_wd) f.push_back(h256(off + 536));            // withdrawals_root
-        if (has_blob) { f.push_back(u64(off + 568)); f.push_back(u64(off + 576)); }
-        if (has_req) { f.push_back(h256(off + 584)); f.push_back(h256(off + 616)); }
-        return p.container(f);
+        return bad ? 0 : p.container(f);
     }
     uint64_t body(uint64_t off, uint64_t len, uint64_t dst) {
-        const bool has_ep = fork >= LHB200_FORK_BELLATRIX, has_bc = fork >= LHB200_FORK_CAPELLA, has_kz = fork >= LHB200_FORK_DENEB,
-                   has_cs = electra();
-        const uint32_t fixed = 380 + (has_ep ? 4 : 0) + (has_bc ? 4 : 0) + (has_kz ? 4 : 0) + (has_cs ? 4 : 0);
-        if (len < fixed) { bad = true; return 0; }
-        const uint32_t o_ps = rd32(s + off + 200), o_as = rd32(s + off + 204), o_at = rd32(s + off + 208),
-                       o_dp = rd32(s + off + 212), o_ex = rd32(s + off + 216),
-                       o_ep = has_ep ? rd32(s + off + 380) : (uint32_t)len, o_bc = has_bc ? rd32(s + off + 384) : (uint32_t)len,
-                       o_kz = has_kz ? rd32(s + off + 388) : (uint32_t)len, o_cs = has_cs ? rd32(s + off + 392) : (uint32_t)len;
-        if (o_ps != fixed || o_as < o_ps || o_at < o_as || o_dp < o_at || o_ex < o_dp || o_ep < o_ex || o_bc < o_ep ||
-            o_kz < o_bc || o_cs < o_kz || o_cs > len) { bad = true; return 0; }
+        using namespace block_layout;
+        Span v[N_BODY_VAR];
+        if (!read_offsets(s + off, len, fl.body_fixed, BODY_VAR_POS, v)) return fail();
         std::vector<uint64_t> f(9), b, roots;
         f[0] = sig(off);
-        f[1] = p.container({h256(off + 96), u64(off + 128), h256(off + 136)});  // eth1_data.rs:27
+        f[1] = eth1_data(off + 96);
         f[2] = h256(off + 168);
-        f[3] = fixed_list(off + o_ps, o_as - o_ps, 416, 4, [&](uint64_t o) { return proposer_slashing(o); });
-        // MaxAttesterSlashings 2, MaxAttestations 128; Electra MaxAttesterSlashingsElectra 1, MaxAttestationsElectra 8
-        const uint32_t as_log = has_cs ? 0 : 1, at_log = has_cs ? 3 : 7;
-        if (!var_bounds(off + o_as, o_at - o_as, 1u << as_log, b)) { bad = true; return 0; }
-        for (size_t i = 0; i + 1 < b.size(); i++) {
-            const uint64_t q = off + o_as + b[i], ql = b[i + 1] - b[i];
-            if (ql < 8) { bad = true; return 0; }
-            const uint32_t a1 = rd32(s + q), a2 = rd32(s + q + 4);
-            if (a1 != 8 || a2 < a1 || a2 > ql) { bad = true; return 0; }
-            uint64_t r1 = indexed_attestation(q + a1, a2 - a1), r2 = indexed_attestation(q + a2, ql - a2);
+        f[3] = fixed_list(off, v[B_PROPOSER_SLASHINGS], 416, 4, [&](uint64_t o) { return proposer_slashing(o); });
+        const Span as = v[B_ATTESTER_SLASHINGS], at = v[B_ATTESTATIONS];
+        if (!var_bounds(off + as.off, as.len, fl.max_attester_slashings, b)) return fail();
+        for (size_t i = 0; i + 1 < b.size(); i++) {   // AttesterSlashing: two IndexedAttestations
+            const uint64_t q = off + as.off + b[i];
+            Span a[2];
+            if (!read_offsets(s + q, b[i + 1] - b[i], 8, ATTESTER_SLASHING_VAR_POS, a)) return fail();
+            uint64_t r1 = indexed_attestation(q + a[0].off, a[0].len), r2 = indexed_attestation(q + a[1].off, a[1].len);
             if (bad) return 0;
             roots.push_back(p.op_hash(r1, r2));
         }
-        f[4] = list_of(roots, as_log);
+        f[4] = list_of(roots, ceil_log2(fl.max_attester_slashings));
         roots.clear();
-        if (!var_bounds(off + o_at, o_dp - o_at, 1u << at_log, b)) { bad = true; return 0; }
+        if (!var_bounds(off + at.off, at.len, fl.max_attestations, b)) return fail();
         for (size_t i = 0; i + 1 < b.size(); i++) {
-            roots.push_back(attestation(off + o_at + b[i], b[i + 1] - b[i]));
+            roots.push_back(attestation(off + at.off + b[i], b[i + 1] - b[i]));
             if (bad) return 0;
         }
-        f[5] = list_of(roots, at_log);
-        f[6] = fixed_list(off + o_dp, o_ex - o_dp, 1240, 4, [&](uint64_t o) { return deposit(o); });
-        f[7] = fixed_list(off + o_ex, o_ep - o_ex, 112, 4, [&](uint64_t o) { return voluntary_exit(o); });
+        f[5] = list_of(roots, ceil_log2(fl.max_attestations));
+        f[6] = fixed_list(off, v[B_DEPOSITS], 1240, 4, [&](uint64_t o) { return deposit(o); });
+        f[7] = fixed_list(off, v[B_EXITS], 112, 4, [&](uint64_t o) { return voluntary_exit(o); });
         f[8] = p.op_hash(blob(off + 220, 64, 1), sig(off + 284));  // sync_aggregate.rs:38
-        if (has_ep) f.push_back(blinded ? payload_header(off + o_ep, o_bc - o_ep) : payload(off + o_ep, o_bc - o_ep));
-        if (has_bc) f.push_back(fixed_list(off + o_bc, o_kz - o_bc, 172, 4, [&](uint64_t o) { return bls_change(o); }));
-        if (has_kz) f.push_back(fixed_list(off + o_kz, o_cs - o_kz, 48, 12, [&](uint64_t o) { return pubkey(o); }));  // kzg_commitment.rs:51
-        if (has_cs) f.push_back(fixed_list(off + o_cs, len - o_cs, 120, 0, [&](uint64_t o) { return consolidation(o); }));
+        for (int k = 9; k < fl.body_fields && !bad; k++) {   // appended by later forks
+            const Span x = v[B_PAYLOAD + (k - 9)];
+            switch (k) {
+                case 9: f.push_back(blinded ? payload_header(off + x.off, x.len) : payload(off + x.off, x.len)); break;
+                case 10: f.push_back(fixed_list(off, x, 172, 4, [&](uint64_t o) { return bls_change(o); })); break;
+                case 11: f.push_back(fixed_list(off, x, 48, 12, [&](uint64_t o) { return pubkey(o); })); break;  // kzg_commitment.rs:51
+                default: f.push_back(fixed_list(off, x, 120, 0, [&](uint64_t o) { return consolidation(o); })); break;  // 12
+            }
+        }
         if (bad) return 0;
         return p.container(f, dst);
     }
     uint64_t block(uint64_t off, uint64_t len, uint64_t dst_root, uint64_t dst_body) {
-        if (len < 84 || rd32(s + off + 80) != 84) { bad = true; return 0; }
-        uint64_t b = body(off + 84, len - 84, dst_body);
+        Span v[1];
+        if (!read_offsets(s + off, len, block_layout::BLOCK_FIXED, block_layout::BLOCK_VAR_POS, v)) return fail();
+        uint64_t b = body(off + v[0].off, v[0].len, dst_body);
         if (bad) return 0;
         return p.container({u64(off), u64(off + 8), h256(off + 16), h256(off + 48), b}, dst_root);
     }
@@ -1694,23 +1725,23 @@ extern "C" {
 
 constexpr int32_t LHB200_ERETRY = -1000;   // internal: the plan did not fit the arena bound of this attempt
 
-// transactions in one BeaconBlock blob of `fork` (0 when the offsets are not plausible — the describer reports that).
-// The body offsets read here and the payload's transactions / withdrawals offsets sit at the same places from
-// Bellatrix to Electra.
-static uint64_t prescan_transactions(const uint8_t* blk, uint64_t len, int32_t fork) {
-    auto rd = [&](uint64_t o) { uint32_t v; memcpy(&v, blk + o, 4); return (uint64_t)v; };
-    if (fork < LHB200_FORK_BELLATRIX || len < 84 + 392) return 0;
-    const uint64_t body = 84, o_ep = rd(body + 380), o_bc = fork >= LHB200_FORK_CAPELLA ? rd(body + 384) : len - body;
-    if (o_ep > o_bc || body + o_bc > len || o_bc - o_ep < 528) return 0;
-    const uint64_t pay = body + o_ep, plen = o_bc - o_ep, o_tx = rd(pay + 504),
-                   o_wd = fork >= LHB200_FORK_CAPELLA ? rd(pay + 508) : plen;
-    if (o_tx > o_wd || o_wd > plen || o_wd - o_tx < 4) return 0;
-    const uint64_t first = rd(pay + o_tx);
-    return first <= o_wd - o_tx ? first / 4 : 0;
+// transactions in one BeaconBlock blob (0 when the offsets are not plausible — the describer reports that)
+static uint64_t prescan_transactions(const uint8_t* blk, uint64_t len, const ForkLayout& fl) {
+    using namespace block_layout;
+    Span block[1], body[N_BODY_VAR], pay[N_PAYLOAD_VAR];
+    if (!fl.payload_fields || !read_offsets(blk, len, BLOCK_FIXED, BLOCK_VAR_POS, block)) return 0;
+    const uint8_t* b = blk + block[0].off;
+    if (!read_offsets(b, block[0].len, fl.body_fixed, BODY_VAR_POS, body)) return 0;
+    const uint8_t* ep = b + body[B_PAYLOAD].off;
+    if (!read_offsets(ep, body[B_PAYLOAD].len, fl.payload_fixed, PAYLOAD_VAR_POS, pay)) return 0;
+    const Span tx = pay[P_TRANSACTIONS];
+    if (tx.len < 4) return 0;
+    const uint64_t first = rd32(ep + tx.off);
+    return first <= tx.len ? first / 4 : 0;
 }
 
 static int32_t block_roots_attempt(Ctx& c, const uint8_t* ssz, const uint64_t* offsets, uint32_t n, uint8_t* roots,
-                                   uint8_t* body_roots, bool blinded, int32_t fork, uint64_t base, uint64_t total, size_t in_pad,
+                                   uint8_t* body_roots, bool blinded, const ForkLayout& fl, uint64_t base, uint64_t total, size_t in_pad,
                                    size_t max_nodes, size_t lit_cap) {
     uint8_t *d_in = nullptr, *d_roots = nullptr, *d_body = nullptr;
     bool bad = false;
@@ -1720,9 +1751,7 @@ static int32_t block_roots_attempt(Ctx& c, const uint8_t* ssz, const uint64_t* o
         d_body = d_roots + 32ull * n;
         p.forced_base = reinterpret_cast<uint64_t>(d_roots);
         p.forced_wave.assign(2ull * n, -1);
-        BlockDescriber bd{p, ssz + base, d_in};
-        bd.blinded = blinded;
-        bd.fork = fork;
+        BlockDescriber bd{{p, ssz + base, d_in, fl}, blinded};
         for (uint32_t i = 0; i < n && !bd.bad; i++)
             bd.block(offsets[i] - base, offsets[i + 1] - offsets[i], reinterpret_cast<uint64_t>(d_roots + 32ull * i),
                      reinterpret_cast<uint64_t>(d_body + 32ull * i));
@@ -1766,7 +1795,8 @@ static int32_t block_roots_attempt(Ctx& c, const uint8_t* ssz, const uint64_t* o
 static int32_t block_roots(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, uint8_t* roots,
                                  uint8_t* body_roots, bool blinded, int32_t fork = LHB200_FORK_DENEB) {
     LHB_REQUIRE_READY();
-    if (fork < LHB200_FORK_ALTAIR || fork > LHB200_FORK_ELECTRA || (blinded && fork < LHB200_FORK_BELLATRIX)) {
+    const ForkLayout* fl = fork_layout(fork);
+    if (!fl || (blinded && !fl->payload_fields)) {
         set_error("beacon_block_roots: fork id %d not supported (Altair .. Electra; blinded blocks from Bellatrix)", fork);
         return LHB200_EINVAL;
     }
@@ -1779,17 +1809,17 @@ static int32_t block_roots(const uint8_t* ssz, const uint64_t* offsets, uint32_t
     const size_t in_pad = align_up(total + 64, 256);
     // Offset pre-scan: the only SSZ shape with more than one tree node per ~14 input bytes is a run of (near-)empty
     // transactions — a 4-byte offset each, one byte item + one list node + one length literal.  Count them per block
-    // (three offset reads) so the arena bound is tight for real blocks and still holds for that shape.
+    // (a walk over its offsets) so the arena bound is tight for real blocks and still holds for that shape.
     uint64_t n_tx = 0;
     if (!blinded)
-        for (uint32_t i = 0; i < n; i++) n_tx += prescan_transactions(ssz + offsets[i], offsets[i + 1] - offsets[i], fork);
+        for (uint32_t i = 0; i < n; i++) n_tx += prescan_transactions(ssz + offsets[i], offsets[i + 1] - offsets[i], *fl);
     int32_t rc = LHB200_OK;
     for (int attempt = 0; attempt < 2; attempt++) {
         // attempt 0: transactions counted, everything else <= one node per 12 bytes and one literal per 8 bytes;
         // attempt 1 (only if a plan ever exceeds that): the unconditional bound of one node and literal per 2 bytes.
         const size_t max_nodes = attempt == 0 ? 2 * n_tx + total / 12 + 512ull * n : total / 2 + 512ull * n;
         const size_t lit_cap = align_up(32 * (attempt == 0 ? n_tx + total / 8 + 128ull * n : total / 2 + 128ull * n), 256);
-        rc = block_roots_attempt(c, ssz, offsets, n, roots, body_roots, blinded, fork, base, total, in_pad, max_nodes, lit_cap);
+        rc = block_roots_attempt(c, ssz, offsets, n, roots, body_roots, blinded, *fl, base, total, in_pad, max_nodes, lit_cap);
         if (rc != LHB200_ERETRY) break;
     }
     return rc == LHB200_ERETRY ? LHB200_EINVAL : rc;

@@ -104,26 +104,25 @@ def validator_roots(ssz: bytes) -> bytes:
     return out.raw[: 32 * n]
 
 
+FORKS = {"altair": 1, "bellatrix": 2, "capella": 3, "deneb": 4, "electra": 5}   # LHB200_FORK_*
+
+
+def _n_field_roots(fork):
+    """Field roots the state entry points write: 28 for every fork before Electra (zero chunks past the fork's own
+    fields), 37 for Electra."""
+    return 37 if fork == "electra" else 28
+
+
 def beacon_state_root_deneb(ssz, want_field_roots=False):
     """BeaconState::update_tree_hash_cache (cold) for BeaconStateDeneb SSZ bytes."""
-    out = C.create_string_buffer(32)
-    fr = C.create_string_buffer(28 * 32) if want_field_roots else None
-    p, keep = buf(ssz)
-    n = len(ssz) if isinstance(ssz, (bytes, bytearray)) else keep.nbytes
-    check(lib.lhb200_beacon_state_root_deneb(p, n, out, fr), "lhb200_beacon_state_root_deneb")
-    if want_field_roots:
-        return out.raw, [fr.raw[32 * i: 32 * i + 32] for i in range(28)]
-    return out.raw
-
-
-FORKS = {"altair": 1, "bellatrix": 2, "capella": 3, "deneb": 4, "electra": 5}   # LHB200_FORK_*
+    return beacon_state_root(ssz, "deneb", want_field_roots)
 
 
 def beacon_state_root(ssz, fork="deneb", want_field_roots=False):
     """BeaconState::update_tree_hash_cache (cold) for any post-Altair variant of the superstruct
     (consensus/types/src/beacon_state.rs:224-571): lhb200_beacon_state_root."""
     out = C.create_string_buffer(32)
-    n_fr = 37 if fork == "electra" else 28
+    n_fr = _n_field_roots(fork)
     fr = C.create_string_buffer(n_fr * 32) if want_field_roots else None
     p, keep = buf(ssz)
     n = len(ssz) if isinstance(ssz, (bytes, bytearray)) else keep.nbytes
@@ -136,20 +135,7 @@ def beacon_state_root(ssz, fork="deneb", want_field_roots=False):
 def beacon_block_roots_deneb(blocks, want_body_roots=False, blinded=False):
     """BeaconBlock::canonical_root (beacon_block.rs:158-160) of a batch of BeaconBlockDeneb SSZ blobs in one pass
     (blinded=True: BlindedBeaconBlockDeneb blobs, whose body carries the payload header)."""
-    blocks = [bytes(b) for b in blocks]
-    n = len(blocks)
-    offs = (C.c_uint64 * (n + 1))()
-    for i, b in enumerate(blocks):
-        offs[i + 1] = offs[i] + len(b)
-    p, keep = buf(b"".join(blocks))
-    out = C.create_string_buffer(32 * max(n, 1))
-    body = C.create_string_buffer(32 * max(n, 1)) if want_body_roots else None
-    fn = lib.lhb200_blinded_beacon_block_roots_deneb if blinded else lib.lhb200_beacon_block_roots_deneb
-    check(fn(p, C.cast(offs, C.c_void_p), n, out, body), "lhb200_beacon_block_roots_deneb")
-    roots = [out.raw[32 * i: 32 * i + 32] for i in range(n)]
-    if want_body_roots:
-        return roots, [body.raw[32 * i: 32 * i + 32] for i in range(n)]
-    return roots
+    return beacon_block_roots(blocks, "deneb", want_body_roots, blinded)
 
 
 def beacon_block_roots(blocks, fork="deneb", want_body_roots=False, blinded=False):
@@ -228,10 +214,11 @@ class ResidentState:
 
     def root(self, want_field_roots=False):
         out = C.create_string_buffer(32)
-        fr = C.create_string_buffer(28 * 32) if want_field_roots else None
+        n_fr = _n_field_roots("deneb")
+        fr = C.create_string_buffer(n_fr * 32) if want_field_roots else None
         check(lib.lhb200_state_root(self._h, out, fr), "lhb200_state_root")
         if want_field_roots:
-            return out.raw, [fr.raw[32 * i: 32 * i + 32] for i in range(28)]
+            return out.raw, [fr.raw[32 * i: 32 * i + 32] for i in range(n_fr)]
         return out.raw
 
     def patch(self, ssz_offset: int, data: bytes):
