@@ -118,6 +118,34 @@ LHB200_API int32_t lhb200_state_patch_batch(lhb200_state* st, const uint64_t* of
  * lhb200_state_last_root_hashes: hash32_concat units the last root actually computed. */
 LHB200_API int32_t lhb200_state_enable_incremental(lhb200_state* st);
 LHB200_API uint64_t lhb200_state_last_root_hashes(const lhb200_state* st);
+/* Resizable lists of an incremental, unsharded handle: what a block and an epoch do to list lengths (eth1 votes,
+ * deposits, historical_summaries, Electra's pending lists) without re-staging.  One edit per field and call:
+ *   append     first = old_len, new_len = old_len + n        truncate / reset   n = 0, new_len < old_len
+ *   front drain  first = 0, n = new_len (the remaining items)  rewrite            new_len = old_len
+ * Items [first, first + n) are written from `data` (SSZ bytes, edit after edit); first + n <= new_len and every item
+ * in [old_len, new_len) must be written.  Fields (container index, item bytes): 9 eth1_data_votes (72), 11 validators
+ * (121), 12 balances (8), 15 / 16 previous_ / current_epoch_participation (1), 21 inactivity_scores (8),
+ * 27 historical_summaries (64, Capella and later), 34 / 35 / 36 pending_balance_deposits / pending_partial_withdrawals /
+ * pending_consolidations (16 / 24 / 16, Electra).  historical_roots is not resizable.  A field the fork does not have,
+ * a limit overrun, reserved != 0, or a non-incremental or sharded handle gives LHB200_EINVAL, and a refused call
+ * changes nothing.  Afterwards roots, field roots, hash units and lhb200_state_patch offsets all refer to the current
+ * encoding; bytes past a list's length are not resident.  Only the dirty paths, the changed lists' zero ladders and
+ * length mix-ins and the tail program are re-hashed; more than 65 536 dirty leaves in one list re-hash its tree from
+ * the resident items. */
+typedef struct lhb200_list_edit {
+    uint32_t field;     /* index in the state container (field_roots order) */
+    uint32_t reserved;  /* 0 */
+    uint64_t new_len;   /* item count after the edit */
+    uint64_t first;     /* first item written */
+    uint64_t n;         /* items written; their SSZ bytes follow in `data`, edit after edit */
+} lhb200_list_edit;
+LHB200_API int32_t lhb200_state_list_edit(lhb200_state* st, const lhb200_list_edit* edits, uint32_t n_edits,
+                                          const uint8_t* data);
+/* Current item count of resizable list `field` (see lhb200_state_list_edit). */
+LHB200_API int32_t lhb200_state_list_len(const lhb200_state* st, uint32_t field, uint64_t* len);
+/* Replace latest_execution_payload_header (Bellatrix and later) with `len` bytes of SSZ of the handle's fork; its
+ * extra_data may change length.  Same handle requirements as lhb200_state_list_edit. */
+LHB200_API int32_t lhb200_state_set_payload_header(lhb200_state* st, const uint8_t* ssz, uint64_t len);
 /* Same as lhb200_state_root but only enqueues; the root lands in device memory (returned pointer valid until
  * the next call on this handle).  Used by bench.py to time kernels with CUDA events. */
 LHB200_API int32_t lhb200_state_root_enqueue(lhb200_state* st, void* stream, const void** d_root);

@@ -140,3 +140,12 @@ _sig("lhb200_verify_signature_set_batches", C.c_int32, vp, vp, vp, vp, vp, C.c_u
 _sig("lhb200_bls_batch_set_segments", C.c_int32, vp, vp, C.c_uint32)
 _sig("lhb200_bls_batch_segment_result", C.c_int32, vp, vp, vp, vp)
 _sig("lhb200_bls_batch_segment_gt", C.c_int32, vp, C.c_uint32, vp)
+_sig("lhb200_state_list_edit", C.c_int32, vp, vp, C.c_uint32, vp)
+_sig("lhb200_state_list_len", C.c_int32, vp, C.c_uint32, C.POINTER(C.c_uint64))
+_sig("lhb200_state_set_payload_header", C.c_int32, vp, vp, C.c_uint64)
+
+
+class ListEdit(C.Structure):
+    """struct lhb200_list_edit"""
+    _fields_ = [("field", C.c_uint32), ("reserved", C.c_uint32), ("new_len", C.c_uint64), ("first", C.c_uint64),
+                ("n", C.c_uint64)]

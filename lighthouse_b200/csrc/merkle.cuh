@@ -117,15 +117,20 @@ __global__ void __launch_bounds__(VAL_PER_CTA) k_validator_roots(const uint8_t* 
 // Small fixed-size records -> roots.  kind 0: 48-byte pubkey.  kind 1: 72-byte Eth1Data {H256,u64,H256}.
 // kind 2: 16-byte {u64, u64} (PendingBalanceDeposit, PendingConsolidation).  kind 3: 24-byte {u64, u64, u64}
 // (PendingPartialWithdrawal): the Electra state lists, beacon_state.rs:515-525.  kind 4: 192-byte DepositRequest
-// {pubkey, withdrawal_credentials, amount, signature, index} (deposit_request.rs:23-29), 10 hashes.  Loads are
-// bytewise, so `in` may sit at any byte offset (the block path reads the records straight from the staged SSZ blob).
-__global__ void __launch_bounds__(128) k_record_roots(const uint8_t* __restrict__ in, uint64_t n, int kind,
-                                                      uint8_t* __restrict__ out) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    uint32_t a[8], b[8];
-    if (kind == 4) {
-        const uint8_t* p = in + 192 * i;
+// {pubkey, withdrawal_credentials, amount, signature, index} (deposit_request.rs:23-29), 10 hashes.  kind 5: 64-byte
+// HistoricalSummary {H256, H256} (historical_summary.rs).  Loads are bytewise, so records may sit at any byte offset
+// (the block path reads them straight from the staged SSZ blob).
+constexpr int REC_PUBKEY = 0, REC_ETH1_DATA = 1, REC_U64_PAIR = 2, REC_U64_TRIPLE = 3, REC_DEPOSIT_REQUEST = 4,
+              REC_HISTORICAL_SUMMARY = 5;
+__host__ __device__ constexpr uint32_t record_bytes(int kind) {
+    return kind == REC_PUBKEY ? 48 : kind == REC_ETH1_DATA ? 72 : kind == REC_U64_PAIR ? 16
+         : kind == REC_U64_TRIPLE ? 24 : kind == REC_DEPOSIT_REQUEST ? 192 : 64;
+}
+
+// hash_tree_root of the record of `kind` at p.  Shared by k_record_roots (cold) and k_tree_update_level (warm).
+__device__ __forceinline__ void record_root_words(const uint8_t* p, int kind, uint32_t a[8]) {
+    uint32_t b[8];
+    if (kind == REC_DEPOSIT_REQUEST) {
         uint32_t c[8];
         for (int k = 0; k < 8; k++) a[k] = be_word(p + 4 * k);
         for (int k = 0; k < 4; k++) b[k] = be_word(p + 32 + 4 * k);
@@ -148,27 +153,28 @@ __global__ void __launch_bounds__(128) k_record_roots(const uint8_t* __restrict_
         hash_pair(c, g_zero_words[0], c);         // H(index, zero chunk)
         hash_pair(c, g_zero_words[1], c);         // fields 4..7
         hash_pair(a, c, a);
-    } else if (kind == 0) {
-        const uint8_t* p = in + 48 * i;
+    } else if (kind == REC_PUBKEY) {
         for (int k = 0; k < 8; k++) a[k] = be_word(p + 4 * k);
         for (int k = 0; k < 4; k++) b[k] = be_word(p + 32 + 4 * k);
         b[4] = b[5] = b[6] = b[7] = 0;
         hash_pair(a, b, a);
-    } else if (kind == 2 || kind == 3) {
-        const uint8_t* p = in + (kind == 2 ? 16 : 24) * i;
+    } else if (kind == REC_U64_PAIR || kind == REC_U64_TRIPLE) {
         for (int k = 0; k < 8; k++) a[k] = b[k] = 0;
         le64_words(p, a[0], a[1]);
         le64_words(p + 8, b[0], b[1]);
         hash_pair(a, b, a);                       // H(field 0, field 1)
-        if (kind == 3) {
+        if (kind == REC_U64_TRIPLE) {
             uint32_t c[8];
             for (int k = 0; k < 8; k++) c[k] = b[k] = 0;
             le64_words(p + 16, c[0], c[1]);
             hash_pair(c, b, c);                   // H(field 2, zero chunk)
             hash_pair(a, c, a);
         }
+    } else if (kind == REC_HISTORICAL_SUMMARY) {
+        for (int k = 0; k < 8; k++) a[k] = be_word(p + 4 * k);
+        for (int k = 0; k < 8; k++) b[k] = be_word(p + 32 + 4 * k);
+        hash_pair(a, b, a);
     } else {
-        const uint8_t* p = in + 72 * i;
         uint32_t c[8];
         for (int k = 0; k < 8; k++) a[k] = be_word(p + 4 * k);
         for (int k = 0; k < 8; k++) b[k] = 0;
@@ -179,6 +185,14 @@ __global__ void __launch_bounds__(128) k_record_roots(const uint8_t* __restrict_
         hash_pair(c, b, c);  // H(block_hash, zero chunk)
         hash_pair(a, c, a);
     }
+}
+
+__global__ void __launch_bounds__(128) k_record_roots(const uint8_t* __restrict__ in, uint64_t n, int kind,
+                                                      uint8_t* __restrict__ out) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t a[8];
+    record_root_words(in + (uint64_t)record_bytes(kind) * i, kind, a);
     store_chunk(out + 32 * i, a);
 }
 
@@ -356,16 +370,19 @@ __global__ void __launch_bounds__(PROG_THREADS) k_hash_ops(const HashOp* __restr
 // Every big list of a resident state keeps ALL its levels; after lhb200_state_patch marks leaves dirty, one CTA per
 // tree re-hashes just the paths above them, level by level.
 struct TreeDev {
-    const uint8_t* src;     // kind 0: the staged 121-byte validator records (leaf roots are recomputed from them)
+    const uint8_t* src;     // kind 0: the 121-byte validator records, kind >= 2: the records (leaf roots are recomputed)
     uint8_t* lvl[41];       // lvl[0] = leaf chunks, lvl[top] = one node
-    uint64_t n_leaves;
+    uint64_t n_leaves;      // current leaf count (a resizable list follows its length)
     uint32_t top;           // ceil_log2(n_leaves)
-    uint32_t kind;          // 0: validators, 1: chunks are the data
-    uint8_t* top_dst;       // where the plan's tail program reads this list's data root
+    uint32_t kind;          // 0: validators, 1: chunks are the data, 2 + k: records of k_record_roots kind k
+    uint8_t* top_dst;       // where the plan's tail program reads this list's data root (null: resizable list)
     const uint32_t* dirty;  // sorted, unique leaf indices
     uint32_t n_dirty;
-    uint32_t pad_;
+    uint32_t limit_depth;   // resizable list: chunk-tree depth of its limit
+    uint64_t length;        // resizable list: item count mixed into its root
+    uint8_t* field_dst;     // resizable list: where k_list_finish writes the field root
 };
+constexpr uint32_t TREE_VALIDATORS = 0, TREE_CHUNKS = 1, TREE_RECORDS = 2;
 
 // out[i] = H(in[2i], in[2i+1] or ZERO[zlevel]) for i < ceil(n_in / 2)   (full build of one level)
 __global__ void __launch_bounds__(256) k_tree_level(const uint8_t* __restrict__ in, uint64_t n_in,
@@ -381,17 +398,19 @@ __global__ void __launch_bounds__(256) k_tree_level(const uint8_t* __restrict__ 
 }
 
 // One level of the dirty-path update for ALL trees of a state: blockIdx.y = tree, one thread per dirty leaf.
-// level < 0: recompute the leaf roots of dirty validators.  Otherwise the first dirty leaf under each parent at
-// `level + 1` hashes that parent from its two children at `level`.
+// level < 0: recompute the leaf roots of dirty validators / records.  Otherwise the first dirty leaf under each parent
+// at `level + 1` hashes that parent from its two children at `level`; a child past the current length is the zero
+// node of its height, so after a truncation the path of the new last leaf rebuilds the right edge.
 __global__ void __launch_bounds__(256) k_tree_update_level(const TreeDev* __restrict__ trees, int level) {
     const TreeDev& t = trees[blockIdx.y];
     const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= t.n_dirty) return;
     if (level < 0) {
-        if (t.kind != 0) return;
+        if (t.kind == TREE_CHUNKS) return;
         const uint32_t i = t.dirty[j];
         uint32_t w[8];
-        validator_root_words(t.src + (uint64_t)VAL_SSZ * i, w);
+        if (t.kind == TREE_VALIDATORS) validator_root_words(t.src + (uint64_t)VAL_SSZ * i, w);
+        else record_root_words(t.src + (uint64_t)record_bytes(t.kind - TREE_RECORDS) * i, t.kind - TREE_RECORDS, w);
         store_chunk(t.lvl[0] + 32ull * i, w);
         return;
     }
@@ -406,7 +425,31 @@ __global__ void __launch_bounds__(256) k_tree_update_level(const TreeDev* __rest
     if (rv) load_operand(reinterpret_cast<uint64_t>(t.lvl[l] + 64ull * p + 32), b);
     fold(a, b, rv, l);
     store_chunk(t.lvl[l + 1] + 32ull * p, a);
-    if (l + 1 == t.top) store_chunk(t.top_dst, a);
+    if (l + 1 == t.top && t.top_dst) store_chunk(t.top_dst, a);
+}
+
+// Finishing step of resizable lists: one thread per list.  Field root = mix_in_length(data root laddered from the
+// current top to the limit depth with ZERO_HASHES, length); an empty list is ZERO_HASHES[limit depth] mixed with 0.
+constexpr int MAX_FINISH = 16;
+struct FinishTable {
+    uint32_t n;
+    uint32_t tree[MAX_FINISH];   // indices into the TreeDev array
+};
+__global__ void __launch_bounds__(32) k_list_finish(const TreeDev* __restrict__ trees,
+                                                    const __grid_constant__ FinishTable tab) {
+    if (threadIdx.x >= tab.n) return;
+    const TreeDev& t = trees[tab.tree[threadIdx.x]];
+    uint32_t r[8];
+    if (t.n_leaves == 0) {
+#pragma unroll
+        for (int i = 0; i < 8; i++) r[i] = g_zero_words[t.limit_depth][i];
+    } else {
+        load_operand(reinterpret_cast<uint64_t>(t.lvl[t.top]), r);
+        for (uint32_t l = t.top; l < t.limit_depth; l++) hash_pair(r, g_zero_words[l], r);
+    }
+    uint32_t len[8] = {bswap32((uint32_t)t.length), bswap32((uint32_t)(t.length >> 32)), 0, 0, 0, 0, 0, 0};
+    hash_pair(r, len, r);
+    store_chunk(t.field_dst, r);
 }
 
 // Scatter a batch of same-length byte patches from one staged blob into resident buffers: one warp per patch.

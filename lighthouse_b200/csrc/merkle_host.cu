@@ -7,6 +7,7 @@
 #include <algorithm>
 #include <array>
 #include <memory>
+#include <unordered_map>
 #include <vector>
 #include "ctx.h"
 #include "merkle.cuh"
@@ -226,8 +227,8 @@ struct Plan {
 };
 
 static int32_t plan_enqueue_tail(Plan& pl, cudaStream_t s);
-// Enqueue a finished plan on `s`.  Literals must already be in the arena.
-static int32_t plan_enqueue(Plan& pl, cudaStream_t s, cudaEvent_t e0 = nullptr, cudaEvent_t e1 = nullptr) {
+// Leaf kernels, reduce passes and byte items of a plan: everything before its tail hash program.
+static void plan_enqueue_body(Plan& pl, cudaStream_t s, cudaEvent_t e0 = nullptr, cudaEvent_t e1 = nullptr) {
     for (const LeafLaunch& L : pl.leaves) {
         switch (L.kind.kernel) {
             case LeafKind::VALIDATORS:
@@ -264,6 +265,10 @@ static int32_t plan_enqueue(Plan& pl, cudaStream_t s, cudaEvent_t e0 = nullptr, 
         k_byte_items<<<(unsigned)pl.items.size(), ITEM_THREADS, 0, s>>>(pl.d_items);
         count_launch();
     }
+}
+// Enqueue a finished plan on `s`.  Literals must already be in the arena.
+static int32_t plan_enqueue(Plan& pl, cudaStream_t s, cudaEvent_t e0 = nullptr, cudaEvent_t e1 = nullptr) {
+    plan_enqueue_body(pl, s, e0, e1);
     return plan_enqueue_tail(pl, s);
 }
 // The tail hash program only (zero ladders, length mix-ins, containers): all a warm root needs after the trees.
@@ -347,6 +352,19 @@ static int32_t scratch_arena(size_t need, uint8_t** arena, size_t* bytes) {
     return *arena ? LHB200_OK : LHB200_ENOMEM;
 }
 
+// The wave table of a plan's ops (h_waves[w]: first op of wave w) and the ops in wave order at h_ops (stable
+// counting sort).
+static void plan_sort_ops(Plan& pl, HashOp* h_ops) {
+    int nw = 0;
+    for (int w : pl.op_wave) nw = std::max(nw, w + 1);
+    pl.n_waves = nw;
+    pl.h_waves.assign(nw + 1, 0);
+    for (int w : pl.op_wave) pl.h_waves[w + 1]++;
+    for (int w = 0; w < nw; w++) pl.h_waves[w + 1] += pl.h_waves[w];
+    std::vector<int32_t> next(pl.h_waves.begin(), pl.h_waves.end() - 1);
+    for (size_t i = 0; i < pl.ops.size(); i++) h_ops[next[pl.op_wave[i]]++] = pl.ops[i];
+}
+
 // Sort the ops by wave and upload literals and program (ops, wave table, byte items) through the pinned `h_stage`
 // (plan_stage_bytes).  The program blobs are allocated from the arena after everything else the plan holds; a plan
 // they would not fit is refused before any copy.
@@ -362,17 +380,9 @@ static int32_t plan_upload(Plan& pl, cudaStream_t s, uint8_t* h_stage) {
         LHB_CUDA(cudaMemcpyAsync(pl.arena + pl.lit_off, h, pl.lit.size(), cudaMemcpyHostToDevice, s));
         h += align_up(pl.lit.size(), 256);
     }
-    int nw = 0;
-    for (int w : pl.op_wave) nw = std::max(nw, w + 1);
-    pl.n_waves = nw;
-    pl.h_waves.assign(nw + 1, 0);   // h_waves[w]: first op of wave w (stable counting sort)
-    for (int w : pl.op_wave) pl.h_waves[w + 1]++;
-    for (int w = 0; w < nw; w++) pl.h_waves[w + 1] += pl.h_waves[w];
+    plan_sort_ops(pl, reinterpret_cast<HashOp*>(h));
     if (!pl.ops.empty()) {
         const size_t nb = pl.ops.size() * sizeof(HashOp), wb = pl.h_waves.size() * sizeof(int32_t);
-        HashOp* h_ops = reinterpret_cast<HashOp*>(h);
-        std::vector<int32_t> next(pl.h_waves.begin(), pl.h_waves.end() - 1);
-        for (size_t i = 0; i < pl.ops.size(); i++) h_ops[next[pl.op_wave[i]]++] = pl.ops[i];
         pl.d_ops = reinterpret_cast<HashOp*>(pl.alloc(nb));
         LHB_CUDA(cudaMemcpyAsync(pl.d_ops, h, nb, cudaMemcpyHostToDevice, s));
         h += align_up(nb, 256);
@@ -596,8 +606,9 @@ struct lhb200_state {
     // dirty leaves since the last root: a host BITMAP per tree (marking is O(1) per edit and dedups for free; the next
     // root extracts the sorted index list with a ctz scan — no sort) plus the number of marks made
     struct Tree {
-        lhb200::TreeDev dev; uint64_t src_off, src_bytes; uint32_t item_bytes;
+        lhb200::TreeDev dev; uint64_t src_off, src_bytes; uint32_t item_bytes;   // item_bytes: SSZ bytes per leaf
         std::vector<uint64_t> dirty_bits; std::vector<uint32_t> dirty; uint64_t n_marks = 0;
+        int list = -1;                   // index into `lists` for a resizable list
         void mark(uint64_t leaf) { dirty_bits[leaf >> 6] |= 1ull << (leaf & 63); n_marks++; }
     };
     bool incremental = false, need_full = false;
@@ -607,6 +618,25 @@ struct lhb200_state {
     uint32_t* d_dirty = nullptr;
     uint64_t last_root_hashes = 0;       // hash32_concat units of the last root (full or incremental)
     static constexpr uint32_t DIRTY_CAP = 1u << 16;
+    // SSZ byte length of each variable-size field of the current encoding (state_layout::VAR_POS order)
+    uint64_t var_len[lhb200::state_layout::N_VAR] = {};
+    // Resizable lists (lhb200_state_list_edit / _set_payload_header convert a handle at its first call): each list owns
+    // device storage for its items, leaf chunks and levels with headroom, and its field root comes from k_list_finish
+    // instead of the tail program.
+    struct List {
+        int spec;                        // index into LIST_SPECS
+        int tree;                        // index into `trees`
+        size_t copy;                     // index into `copies` (patches address the list through it)
+        uint64_t cap = 0;                // items the storage holds
+        uint8_t* d_mem = nullptr;
+        bool resized = false;            // length changed since the last root: the finishing step must run
+    };
+    bool converted = false;
+    std::vector<List> lists;
+    uint64_t units_base = 0;             // hash units of everything but the resizable lists
+    std::vector<std::pair<uint32_t, uint32_t>> hdr_lits;   // payload header literals: (lit_src index, offset in header)
+    int hdr_extra = -1;                  // lit_src index of extra_data
+    uint32_t hdr_len_chunk = 0;          // literal chunk holding extra_data's length
 };
 
 namespace lhb200 {
@@ -1032,6 +1062,11 @@ static int32_t stage_state(const uint8_t* ssz, uint64_t len, ShardCfg sh, lhb200
         return LHB200_OK;
     });
     if (rc) return rc;
+    {   // the describer has checked the offsets
+        Span v[state_layout::N_VAR];
+        read_offsets(ssz, len, fork_layout(sh.fork)->state_fixed, state_layout::VAR_POS, v);
+        for (int k = 0; k < state_layout::N_VAR; k++) st->var_len[k] = v[k].len;
+    }
     st->plan.ssz_base = nullptr;  // the caller's buffer is not retained
     // allocated before the program blobs, so that plan_upload's arena check covers them too
     std::vector<uint64_t> gather(1, st->root_op);   // root + field roots -> contiguous result block
@@ -1237,15 +1272,19 @@ int32_t lhb200_state_patch(lhb200_state* st, uint64_t ssz_offset, const uint8_t*
     return lhb200_state_patch_batch(st, &ssz_offset, &l32, data, len ? 1 : 0);
 }
 
+// (Re)build every level of one resident tree from its leaf chunks.
+static void tree_build_levels(lhb200_state::Tree& t, cudaStream_t s) {
+    uint64_t n = t.dev.n_leaves;
+    for (uint32_t l = 0; l < t.dev.top; l++) {
+        k_tree_level<<<(unsigned)ceil_div(ceil_div(n, 2), 256), 256, 0, s>>>(t.dev.lvl[l], n, t.dev.lvl[l + 1], l);
+        count_launch();
+        n = ceil_div(n, 2);
+    }
+}
 // (Re)build every level of every resident tree from its leaf chunks (which a cold root has just refreshed).
 static int32_t state_build_levels(lhb200_state* st, cudaStream_t s) {
     for (lhb200_state::Tree& t : st->trees) {
-        uint64_t n = t.dev.n_leaves;
-        for (uint32_t l = 0; l < t.dev.top; l++) {
-            k_tree_level<<<(unsigned)ceil_div(ceil_div(n, 2), 256), 256, 0, s>>>(t.dev.lvl[l], n, t.dev.lvl[l + 1], l);
-            count_launch();
-            n = ceil_div(n, 2);
-        }
+        tree_build_levels(t, s);
         t.dirty.clear();
         std::fill(t.dirty_bits.begin(), t.dirty_bits.end(), 0ull);
         t.n_marks = 0;
@@ -1254,7 +1293,69 @@ static int32_t state_build_levels(lhb200_state* st, cudaStream_t s) {
     LHB_CUDA(cudaGetLastError());
     return LHB200_OK;
 }
-// Warm root: re-hash the paths above the dirty leaves (one CTA per tree), then the tail program.
+
+// hash32_concat units of one leaf root of a resident tree (recomputed from its record on the warm path)
+static uint32_t tree_leaf_units(uint32_t kind) {
+    if (kind == TREE_VALIDATORS) return 8;
+    if (kind == TREE_CHUNKS) return 0;
+    const int rec = (int)(kind - TREE_RECORDS);
+    return rec == REC_ETH1_DATA || rec == REC_U64_TRIPLE ? 3 : rec == REC_DEPOSIT_REQUEST ? 10 : 1;
+}
+// Leaf roots of the resizable lists of records and validators, from their items at the current lengths.
+static void lists_enqueue_leaves(lhb200_state* st, cudaStream_t s, cudaEvent_t e0, cudaEvent_t e1) {
+    for (const lhb200_state::List& L : st->lists) {
+        const TreeDev& d = st->trees[L.tree].dev;
+        if (d.n_leaves == 0 || d.kind == TREE_CHUNKS) continue;
+        if (d.kind == TREE_VALIDATORS) {
+            if (e0) cudaEventRecord(e0, s);
+            k_validator_roots<<<(unsigned)ceil_div(d.n_leaves, VAL_PER_CTA), VAL_PER_CTA, 0, s>>>(d.src, d.n_leaves, d.lvl[0]);
+            if (e1) cudaEventRecord(e1, s);
+        } else {
+            k_record_roots<<<(unsigned)ceil_div(d.n_leaves, 128), 128, 0, s>>>(d.src, d.n_leaves, (int)(d.kind - TREE_RECORDS),
+                                                                                d.lvl[0]);
+        }
+        count_launch();
+    }
+}
+// Upload the TreeDev table (through the pinned `h`) and run the finishing step of the lists in `fin`.
+static int32_t lists_enqueue_finish(lhb200_state* st, const FinishTable& fin, cudaStream_t s) {
+    if (fin.n == 0) return LHB200_OK;
+    k_list_finish<<<1, 32, 0, s>>>(st->d_trees, fin);
+    count_launch();
+    LHB_CUDA(cudaGetLastError());
+    for (lhb200_state::List& L : st->lists) L.resized = false;
+    return LHB200_OK;
+}
+static uint64_t finish_units(const TreeDev& d) { return (d.n_leaves ? d.limit_depth - d.top : 0) + 1; }
+
+// Cold root of a handle with resizable lists.  The stage-time plan no longer describes those lists (its leaf launches,
+// reduce passes, ladders and mix-ins carried the old lengths and were dropped at conversion), so their trees are
+// rebuilt from the resident items at the current lengths, then the finishing step, then the tail.
+static int32_t state_converted_cold(lhb200_state* st, cudaStream_t s) {
+    lists_enqueue_leaves(st, s, st->e_k0, st->e_k1);
+    plan_enqueue_body(st->plan, s);
+    int32_t rc = state_build_levels(st, s);
+    if (rc) return rc;
+    const size_t tb = st->trees.size() * sizeof(TreeDev);
+    uint8_t* h = static_cast<uint8_t*>(pinned_scratch(tb));
+    if (!h) return LHB200_ENOMEM;
+    FinishTable fin{};
+    for (size_t k = 0; k < st->trees.size(); k++) {
+        lhb200_state::Tree& t = st->trees[k];
+        t.dev.dirty = st->d_dirty;
+        t.dev.n_dirty = 0;
+        memcpy(h + k * sizeof(TreeDev), &t.dev, sizeof(TreeDev));
+        if (t.list >= 0) fin.tree[fin.n++] = (uint32_t)k;
+    }
+    LHB_CUDA(cudaMemcpyAsync(st->d_trees, h, tb, cudaMemcpyHostToDevice, s));
+    rc = lists_enqueue_finish(st, fin, s);
+    if (rc) return rc;
+    st->last_root_hashes = st->plan.hash_units;
+    return plan_enqueue_tail(st->plan, s);
+}
+
+// Warm root: re-hash the paths above the dirty leaves (one CTA per tree), finish the resizable lists that changed,
+// then the tail program.
 static int32_t state_incremental_enqueue(lhb200_state* st, cudaStream_t s) {
     uint32_t total = 0;
     for (lhb200_state::Tree& t : st->trees) {
@@ -1263,7 +1364,8 @@ static int32_t state_incremental_enqueue(lhb200_state* st, cudaStream_t s) {
             for (size_t w = 0; w < t.dirty_bits.size(); w++) {
                 uint64_t bits = t.dirty_bits[w];
                 while (bits) {
-                    t.dirty.push_back((uint32_t)(w * 64 + (uint32_t)__builtin_ctzll(bits)));
+                    const uint64_t leaf = w * 64 + (uint32_t)__builtin_ctzll(bits);
+                    if (leaf < t.dev.n_leaves) t.dirty.push_back((uint32_t)leaf);   // past a truncation: gone
                     bits &= bits - 1;
                 }
                 t.dirty_bits[w] = 0;
@@ -1277,7 +1379,15 @@ static int32_t state_incremental_enqueue(lhb200_state* st, cudaStream_t s) {
         total += (uint32_t)t.dirty.size();
     }
     uint64_t hashes = st->plan.ops.size();
-    if (total) {
+    FinishTable fin{};
+    for (size_t k = 0; k < st->trees.size(); k++) {
+        const lhb200_state::Tree& t = st->trees[k];
+        if (t.list >= 0 && (!t.dirty.empty() || st->lists[t.list].resized)) {
+            fin.tree[fin.n++] = (uint32_t)k;
+            hashes += finish_units(t.dev);
+        }
+    }
+    if (total || fin.n) {
         const size_t tb = st->trees.size() * sizeof(TreeDev);
         uint8_t* h = static_cast<uint8_t*>(pinned_scratch(tb + (size_t)total * 4 + 256));
         if (!h) return LHB200_ENOMEM;
@@ -1290,32 +1400,36 @@ static int32_t state_incremental_enqueue(lhb200_state* st, cudaStream_t s) {
             if (!t.dirty.empty()) memcpy(hd + off, t.dirty.data(), t.dirty.size() * 4);
             off += t.dev.n_dirty;
             memcpy(h + k * sizeof(TreeDev), &t.dev, sizeof(TreeDev));
-            // hashes = distinct parents per level (+ 8 per dirty validator): neighbours d[j-1] < d[j] have distinct
-            // ancestors exactly at the levels up to the highest bit in which they differ
+            // hashes = distinct parents per level (+ the leaf roots of dirty records): neighbours d[j-1] < d[j] have
+            // distinct ancestors exactly at the levels up to the highest bit in which they differ
             if (!t.dirty.empty()) {
                 uint64_t cnt = t.dev.top;  // the path of the first dirty leaf
                 for (size_t j = 1; j < t.dirty.size(); j++) {
                     const uint32_t hb = 32 - (uint32_t)__builtin_clz(t.dirty[j] ^ t.dirty[j - 1]);  // ancestors equal from level hb up
                     cnt += std::min<uint32_t>(hb - 1, t.dev.top);
                 }
-                hashes += cnt + (t.dev.kind == 0 ? 8ull * t.dirty.size() : 0);
+                hashes += cnt + (uint64_t)tree_leaf_units(t.dev.kind) * t.dirty.size();
             }
             t.dirty.clear();
         }
         LHB_CUDA(cudaMemcpyAsync(st->d_trees, h, tb, cudaMemcpyHostToDevice, s));
-        LHB_CUDA(cudaMemcpyAsync(st->d_dirty, hd, (size_t)total * 4, cudaMemcpyHostToDevice, s));
+        if (total) LHB_CUDA(cudaMemcpyAsync(st->d_dirty, hd, (size_t)total * 4, cudaMemcpyHostToDevice, s));
         // one launch per level covers every tree (blockIdx.y); levels are ordered by the stream
         uint32_t max_nd = 0, max_top = 0;
-        bool any_validators = false;
+        bool any_leaf_roots = false;
         for (const lhb200_state::Tree& t : st->trees) {
             max_nd = std::max(max_nd, t.dev.n_dirty);
-            if (t.dev.n_dirty) { max_top = std::max(max_top, t.dev.top); any_validators |= t.dev.kind == 0; }
+            if (t.dev.n_dirty) { max_top = std::max(max_top, t.dev.top); any_leaf_roots |= t.dev.kind != TREE_CHUNKS; }
         }
-        const dim3 grid((unsigned)ceil_div(max_nd, 256), (unsigned)st->trees.size());
-        for (int l = any_validators ? -1 : 0; l < (int)max_top; l++) {
-            k_tree_update_level<<<grid, 256, 0, s>>>(st->d_trees, l);
-            count_launch();
+        if (total) {
+            const dim3 grid((unsigned)ceil_div(max_nd, 256), (unsigned)st->trees.size());
+            for (int l = any_leaf_roots ? -1 : 0; l < (int)max_top; l++) {
+                k_tree_update_level<<<grid, 256, 0, s>>>(st->d_trees, l);
+                count_launch();
+            }
         }
+        const int32_t rc = lists_enqueue_finish(st, fin, s);
+        if (rc) return rc;
     }
     st->last_root_hashes = hashes;
     return plan_enqueue_tail(st->plan, s);
@@ -1367,6 +1481,419 @@ int32_t lhb200_state_enable_incremental(lhb200_state* st) {
 }
 uint64_t lhb200_state_last_root_hashes(const lhb200_state* st) { return st ? st->last_root_hashes : 0; }
 
+// ---------------------------------------------------------------------------------------------------------
+// Resizable lists (lhb200_state_list_edit, lhb200_state_set_payload_header).  A handle keeps its stage-time plan until
+// the first such call; then each list of the table below moves to storage of its own with headroom (items, leaf
+// chunks, every level), its leaf launches and reduce passes leave the cold plan, and its zero ladder and length mix-in
+// leave the tail program: k_list_finish writes the field root from the list's current top and length instead.
+struct ListSpec {
+    uint32_t field;        // index in the state container
+    int var;               // state_layout::V_*
+    uint32_t item_bytes;
+    uint64_t limit;        // items
+    uint32_t depth;        // chunk-tree depth of the limit
+    uint32_t kind;         // TreeDev kind
+};
+static const ListSpec LIST_SPECS[] = {
+    {9, state_layout::V_VOTES, 72, 2048, 11, TREE_RECORDS + REC_ETH1_DATA},
+    {11, state_layout::V_VAL, 121, 1ull << 40, 40, TREE_VALIDATORS},
+    {12, state_layout::V_BAL, 8, 1ull << 40, 38, TREE_CHUNKS},
+    {15, state_layout::V_PP, 1, 1ull << 40, 35, TREE_CHUNKS},
+    {16, state_layout::V_CP, 1, 1ull << 40, 35, TREE_CHUNKS},
+    {21, state_layout::V_INACT, 8, 1ull << 40, 38, TREE_CHUNKS},
+    {27, state_layout::V_HS, 64, 1ull << 24, 24, TREE_RECORDS + REC_HISTORICAL_SUMMARY},
+    {34, state_layout::V_PBD, 16, 1ull << 27, 27, TREE_RECORDS + REC_U64_PAIR},
+    {35, state_layout::V_PPW, 24, 1ull << 27, 27, TREE_RECORDS + REC_U64_TRIPLE},
+    {36, state_layout::V_PC, 16, 1ull << 18, 18, TREE_RECORDS + REC_U64_PAIR},
+};
+constexpr int N_LIST_SPECS = sizeof(LIST_SPECS) / sizeof(LIST_SPECS[0]);
+static_assert(N_LIST_SPECS <= MAX_FINISH, "one finishing thread per list");
+
+// LIST_SPECS index of the resizable list `field` of the handle's fork, or -1
+static int list_spec_of(const lhb200_state* st, uint32_t field) {
+    const int n_fields = fork_layout(st->shard.fork)->state_fields;
+    for (int k = 0; k < N_LIST_SPECS; k++)
+        if (LIST_SPECS[k].field == field && (int)field < n_fields) return k;
+    return -1;
+}
+static lhb200_state::List& list_of(lhb200_state* st, int spec) {
+    for (lhb200_state::List& L : st->lists)
+        if (L.spec == spec) return L;
+    return st->lists.front();   // not reached: a converted handle has every list of its fork
+}
+static uint64_t list_leaves(const ListSpec& sp, uint64_t len) {
+    return sp.kind == TREE_CHUNKS ? ceil_div(len * sp.item_bytes, 32) : len;
+}
+// Hash units the describer counts for a list of `len` items: leaf roots, data tree, zero ladder, length mix-in.
+static uint64_t list_units(const ListSpec& sp, uint64_t len) {
+    const uint64_t n = list_leaves(sp, len);
+    uint64_t u = (uint64_t)tree_leaf_units(sp.kind) * len + 1;
+    if (n) {
+        const uint32_t top = ceil_log2(n);
+        u += sp.depth - top;
+        for (uint32_t l = 1; l <= top; l++) u += ceil_div(n, 1ull << l);
+    }
+    return u;
+}
+// Lay out the storage of a list of `cap` items at `base` (0: size only): items, leaf chunks (validators and records;
+// packed lists are their own chunks), then one array per level.  Returns the bytes.
+static size_t list_place(TreeDev& d, const ListSpec& sp, uintptr_t base, uint64_t cap) {
+    const uint64_t leaves = std::max<uint64_t>(list_leaves(sp, cap), 1);
+    size_t off = align_up(cap * sp.item_bytes + 32, 256);
+    d.src = reinterpret_cast<const uint8_t*>(base);
+    if (sp.kind == TREE_CHUNKS) {
+        d.lvl[0] = reinterpret_cast<uint8_t*>(base);
+    } else {
+        d.lvl[0] = reinterpret_cast<uint8_t*>(base + off);
+        off += align_up(leaves * 32, 256);
+    }
+    uint64_t n = leaves;
+    for (uint32_t l = 1; l <= ceil_log2(leaves); l++) {
+        n = ceil_div(n, 2);
+        d.lvl[l] = reinterpret_cast<uint8_t*>(base + off);
+        off += align_up(n * 32, 256);
+    }
+    return off;
+}
+// (Re)allocate a list's storage for `cap` items.  Growth copies the items, leaf chunks and levels device to device.
+static int32_t list_alloc(lhb200_state* st, lhb200_state::List& L, uint64_t cap, cudaStream_t s) {
+    const ListSpec& sp = LIST_SPECS[L.spec];
+    lhb200_state::Tree& t = st->trees[L.tree];
+    TreeDev d = t.dev;
+    uint8_t* mem = nullptr;
+    LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&mem), list_place(d, sp, 0, cap)));
+    list_place(d, sp, reinterpret_cast<uintptr_t>(mem), cap);
+    if (L.d_mem) {
+        const uint64_t n = t.dev.n_leaves;
+        const uint64_t item_bytes = sp.kind == TREE_CHUNKS ? n * 32 : t.dev.length * sp.item_bytes;   // with the zero pad
+        if (item_bytes) LHB_CUDA(cudaMemcpyAsync(mem, L.d_mem, item_bytes, cudaMemcpyDeviceToDevice, s));
+        if (sp.kind != TREE_CHUNKS && n) LHB_CUDA(cudaMemcpyAsync(d.lvl[0], t.dev.lvl[0], n * 32, cudaMemcpyDeviceToDevice, s));
+        uint64_t m = n;
+        for (uint32_t l = 1; l <= t.dev.top; l++) {
+            m = ceil_div(m, 2);
+            LHB_CUDA(cudaMemcpyAsync(d.lvl[l], t.dev.lvl[l], m * 32, cudaMemcpyDeviceToDevice, s));
+        }
+        LHB_CUDA(cudaStreamSynchronize(s));
+        LHB_CUDA(cudaFree(L.d_mem));
+    }
+    L.d_mem = mem;
+    L.cap = cap;
+    t.dev = d;
+    t.dirty_bits.resize(ceil_div(std::max<uint64_t>(list_leaves(sp, cap), 1), 64), 0ull);
+    return LHB200_OK;
+}
+
+// SSZ offsets of the variable-size fields of the current encoding follow from their lengths: move the lists' resident
+// copies, the payload header's literal sources and the hash-unit count along, and re-sort the patch lookups.
+static void state_relayout(lhb200_state* st) {
+    using namespace state_layout;
+    uint64_t off[N_VAR];
+    off[0] = fork_layout(st->shard.fork)->state_fixed;
+    for (int k = 1; k < N_VAR; k++) off[k] = off[k - 1] + st->var_len[k - 1];
+    uint64_t units = st->units_base;
+    for (const lhb200_state::List& L : st->lists) {
+        const ListSpec& sp = LIST_SPECS[L.spec];
+        lhb200_state::Tree& t = st->trees[L.tree];
+        t.src_off = off[sp.var];
+        t.src_bytes = t.dev.length * sp.item_bytes;
+        st->copies[L.copy] = {t.src_off, t.src_bytes, L.d_mem, 0};
+        units += list_units(sp, t.dev.length);
+    }
+    st->plan.hash_units = units;
+    for (const auto& h : st->hdr_lits) st->plan.lit_src[h.first].src_off = off[V_LEPH] + h.second;
+    std::vector<uint32_t>& co = st->copy_order;
+    co.resize(st->copies.size());
+    for (size_t k = 0; k < co.size(); k++) co[k] = (uint32_t)k;
+    std::sort(co.begin(), co.end(), [&](uint32_t a, uint32_t b) { return st->copies[a].src_off < st->copies[b].src_off; });
+    const std::vector<Plan::LitSrc>& ls = st->plan.lit_src;
+    std::sort(st->lit_order.begin(), st->lit_order.end(), [&](uint32_t a, uint32_t b) { return ls[a].src_off < ls[b].src_off; });
+    st->copy_tree.assign(st->copies.size(), -1);
+    for (size_t k = 0; k < st->copies.size(); k++)
+        for (size_t t = 0; t < st->trees.size(); t++)
+            if (st->copies[k].nbytes && st->trees[t].src_off == st->copies[k].src_off) st->copy_tree[k] = (int32_t)t;
+    st->copy_tree_trees = st->trees.size();
+}
+
+// Convert an incremental handle to resizable lists (see LIST_SPECS).  Device work only: the lists' bytes move from the
+// stage arena to their own storage and their trees are built there.
+static int32_t state_convert(lhb200_state* st, cudaStream_t s) {
+    using namespace state_layout;
+    const ForkLayout& fl = *fork_layout(st->shard.fork);
+    Plan& pl = st->plan;
+    index_resident(st);
+    uint64_t var_off[N_VAR];
+    var_off[0] = fl.state_fixed;
+    for (int k = 1; k < N_VAR; k++) var_off[k] = var_off[k - 1] + st->var_len[k - 1];
+    // 1. the stage-time copies of the lists (every variable-size field after historical_roots) and everything the
+    //    cold plan derives from them: leaf launches, reduce passes
+    std::vector<StageCopy> staged, keep;
+    staged.swap(st->copies);
+    std::vector<const uint8_t*> owned;
+    bool hist = false;
+    for (const StageCopy& cp : staged) {
+        if (cp.src_off < var_off[V_HIST] || (!hist && cp.src_off == var_off[V_HIST] && cp.nbytes == st->var_len[V_HIST])) {
+            hist |= cp.src_off >= var_off[V_HIST];
+            keep.push_back(cp);
+        } else {
+            owned.push_back(cp.dst);
+        }
+    }
+    auto is_owned = [&](const uint8_t* p) { return std::find(owned.begin(), owned.end(), p) != owned.end(); };
+    std::vector<LeafLaunch> leaves;
+    for (const LeafLaunch& L : pl.leaves) {
+        if (is_owned(L.in)) owned.push_back(L.out);
+        else leaves.push_back(L);
+    }
+    pl.leaves.swap(leaves);
+    for (auto& pass : pl.passes) {
+        std::vector<MerkleSeg> kept;
+        for (const MerkleSeg& sg : pass) {
+            if (is_owned(sg.in)) owned.push_back(sg.out);
+            else kept.push_back(sg);
+        }
+        pass.swap(kept);
+    }
+    pl.passes.erase(std::remove_if(pl.passes.begin(), pl.passes.end(), [](const std::vector<MerkleSeg>& p) { return p.empty(); }),
+                    pl.passes.end());
+    // 2. the tail ops that produce the lists' field roots (small trees, zero ladders, length mix-ins)
+    std::unordered_map<uint64_t, size_t> producer;
+    for (size_t i = 0; i < pl.ops.size(); i++) producer[pl.ops[i].dst] = i;
+    std::vector<char> drop(pl.ops.size(), 0);
+    std::vector<uint64_t> todo;
+    uint64_t stage_units = 0;
+    for (const ListSpec& sp : LIST_SPECS) {
+        if ((int)sp.field >= fl.state_fields) continue;
+        todo.push_back(st->field_ops[sp.field]);
+        stage_units += list_units(sp, st->var_len[sp.var] / sp.item_bytes);
+    }
+    while (!todo.empty()) {
+        const uint64_t x = todo.back();
+        todo.pop_back();
+        const auto it = producer.find(x);
+        if (it == producer.end() || drop[it->second]) continue;
+        drop[it->second] = 1;
+        todo.push_back(pl.ops[it->second].a);
+        todo.push_back(pl.ops[it->second].b);
+    }
+    // 3. the payload header's literal chunks, and the one holding extra_data's length
+    if (fl.payload_fields) {
+        const uint64_t lo = var_off[V_LEPH], hi = lo + st->var_len[V_LEPH];
+        for (size_t k = 0; k < pl.lit_src.size(); k++) {
+            const Plan::LitSrc& ls = pl.lit_src[k];
+            if (ls.src_off < lo || ls.src_off + ls.n > hi) continue;
+            st->hdr_lits.push_back({(uint32_t)k, (uint32_t)(ls.src_off - lo)});
+            if (ls.src_off - lo == fl.header_fixed) st->hdr_extra = (int)k;
+        }
+        const uint64_t lit_base = reinterpret_cast<uint64_t>(pl.arena + pl.lit_off);
+        const uint64_t extra = st->hdr_extra < 0 ? 0 : lit_base + 32ull * pl.lit_src[st->hdr_extra].lit_index;
+        bool found = false;
+        for (const HashOp& op : pl.ops)
+            if (extra && op.a == extra) { st->hdr_len_chunk = (uint32_t)((op.b - lit_base) / 32); found = true; }
+        if (!found) { set_error("internal: payload header literals not found"); return LHB200_EINVAL; }
+    }
+    std::vector<HashOp> ops;
+    std::vector<int> waves;
+    for (size_t i = 0; i < pl.ops.size(); i++)
+        if (!drop[i]) { ops.push_back(pl.ops[i]); waves.push_back(pl.op_wave[i]); }
+    pl.ops.swap(ops);
+    pl.op_wave.swap(waves);
+    {   // the pruned tail goes where the stage-time one was (it is shorter)
+        const size_t nb = align_up(pl.ops.size() * sizeof(HashOp), 256);
+        uint8_t* h = static_cast<uint8_t*>(pinned_scratch(nb + (pl.ops.size() + 2) * 4));
+        if (!h) return LHB200_ENOMEM;
+        plan_sort_ops(pl, reinterpret_cast<HashOp*>(h));
+        memcpy(h + nb, pl.h_waves.data(), pl.h_waves.size() * 4);
+        LHB_CUDA(cudaMemcpyAsync(pl.d_ops, h, pl.ops.size() * sizeof(HashOp), cudaMemcpyHostToDevice, s));
+        LHB_CUDA(cudaMemcpyAsync(pl.d_waves, h + nb, pl.h_waves.size() * 4, cudaMemcpyHostToDevice, s));
+    }
+    st->units_base = pl.hash_units - stage_units;
+    // 4. trees: the fixed-size vectors keep theirs, every list gets a resizable one seeded from its staged bytes
+    std::vector<lhb200_state::Tree> trees;
+    for (lhb200_state::Tree& t : st->trees)
+        if (t.src_off < var_off[V_HIST]) trees.push_back(std::move(t));
+    st->trees.swap(trees);
+    st->copies.swap(keep);
+    for (int k = 0; k < N_LIST_SPECS; k++) {
+        const ListSpec& sp = LIST_SPECS[k];
+        if ((int)sp.field >= fl.state_fields) continue;
+        const uint64_t len = st->var_len[sp.var] / sp.item_bytes;
+        lhb200_state::Tree t;
+        memset(&t.dev, 0, sizeof t.dev);
+        t.dev.kind = sp.kind;
+        t.dev.n_leaves = list_leaves(sp, len);
+        t.dev.top = ceil_log2(t.dev.n_leaves);
+        t.dev.limit_depth = sp.depth;
+        t.dev.length = len;
+        t.dev.field_dst = reinterpret_cast<uint8_t*>(st->field_ops[sp.field]);
+        t.item_bytes = sp.kind == TREE_CHUNKS ? 32 : sp.item_bytes;
+        t.list = (int)st->lists.size();
+        st->trees.push_back(std::move(t));
+        lhb200_state::List L;
+        L.spec = k;
+        L.tree = (int)st->trees.size() - 1;
+        L.copy = st->copies.size();
+        L.resized = true;
+        st->copies.push_back({0, 0, nullptr, 0});
+        st->lists.push_back(L);
+        int32_t rc = list_alloc(st, st->lists.back(), std::max<uint64_t>(2 * len, 16), s);
+        if (rc) return rc;
+        const uint64_t nbytes = sp.kind == TREE_CHUNKS ? 32 * list_leaves(sp, len) : len * sp.item_bytes;
+        for (const StageCopy& cp : staged)   // the staged copy is zero-padded past its bytes
+            if (len && cp.src_off == var_off[sp.var] && cp.nbytes == st->var_len[sp.var])
+                LHB_CUDA(cudaMemcpyAsync(st->lists.back().d_mem, cp.dst, nbytes, cudaMemcpyDeviceToDevice, s));
+    }
+    LHB_CUDA(cudaFree(st->d_trees));
+    LHB_CUDA(cudaFree(st->d_dirty));
+    st->d_trees = nullptr;
+    st->d_dirty = nullptr;
+    LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_trees), st->trees.size() * sizeof(TreeDev) + 256));
+    LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_dirty), (size_t)lhb200_state::DIRTY_CAP * 4 * st->trees.size()));
+    lists_enqueue_leaves(st, s, nullptr, nullptr);
+    for (const lhb200_state::List& L : st->lists) tree_build_levels(st->trees[L.tree], s);
+    LHB_CUDA(cudaGetLastError());
+    st->converted = true;
+    state_relayout(st);
+    LHB_CUDA(cudaStreamSynchronize(s));
+    return LHB200_OK;
+}
+
+static int32_t check_resizable(const lhb200_state* st, const char* what) {
+    if (st->shard.world != 1) { set_error("%s: a sharded handle keeps its list lengths", what); return LHB200_EINVAL; }
+    if (!st->incremental) { set_error("%s: needs an incremental handle (lhb200_state_enable_incremental)", what); return LHB200_EINVAL; }
+    return LHB200_OK;
+}
+
+// New length of one list after its items [first, first + n) were written: zero the packed tail, mark the dirty leaves.
+static int32_t list_set_length(lhb200_state* st, lhb200_state::List& L, uint64_t new_len, uint64_t first, uint64_t n,
+                               cudaStream_t s) {
+    const ListSpec& sp = LIST_SPECS[L.spec];
+    lhb200_state::Tree& t = st->trees[L.tree];
+    const uint64_t old = t.dev.length, nl = list_leaves(sp, new_len), ib = sp.item_bytes;
+    if (sp.kind == TREE_CHUNKS && nl * 32 > new_len * ib)   // SSZ packing pads the last chunk with zeros
+        LHB_CUDA(cudaMemsetAsync(L.d_mem + new_len * ib, 0, nl * 32 - new_len * ib, s));
+    auto mark = [&](uint64_t a, uint64_t b) {
+        if (st->need_full || a >= b) return;
+        if (t.n_marks + (b - a) > 4ull * lhb200_state::DIRTY_CAP) { st->need_full = true; return; }
+        for (uint64_t q = a; q < b; q++) t.mark(q);
+    };
+    if (n) mark(sp.kind == TREE_CHUNKS ? first * ib / 32 : first, list_leaves(sp, first + n));
+    if (new_len < old && nl) mark(nl - 1, nl);   // the new right edge: its path re-hashes with zero siblings
+    L.resized |= new_len != old;
+    t.dev.n_leaves = nl;
+    t.dev.top = ceil_log2(nl);
+    t.dev.length = new_len;
+    st->var_len[sp.var] = new_len * ib;
+    return LHB200_OK;
+}
+
+int32_t lhb200_state_list_edit(lhb200_state* st, const lhb200_list_edit* edits, uint32_t n_edits, const uint8_t* data) {
+    LHB_REQUIRE_READY();
+    if (!st || (n_edits && !edits)) return LHB200_EINVAL;
+    Ctx& c = ctx();
+    std::lock_guard<std::recursive_mutex> g(c.mu);
+    int32_t rc = check_resizable(st, "state_list_edit");
+    if (rc) return rc;
+    // every edit is checked before anything changes: a refused call leaves the handle as it was
+    uint64_t seen = 0, total = 0;
+    for (uint32_t i = 0; i < n_edits; i++) {
+        const lhb200_list_edit& e = edits[i];
+        const int k = list_spec_of(st, e.field);
+        if (k < 0 || e.reserved) {
+            set_error("state_list_edit: field %u is not a resizable list of this fork, or reserved != 0", e.field);
+            return LHB200_EINVAL;
+        }
+        if ((seen >> e.field) & 1) { set_error("state_list_edit: two edits of field %u in one call", e.field); return LHB200_EINVAL; }
+        seen |= 1ull << e.field;
+        const ListSpec& sp = LIST_SPECS[k];
+        const uint64_t old = st->var_len[sp.var] / sp.item_bytes;
+        if (e.new_len > sp.limit || e.first > e.new_len || e.n > e.new_len - e.first) {
+            set_error("state_list_edit: field %u: new_len %llu (limit %llu), first %llu, n %llu", e.field,
+                      (unsigned long long)e.new_len, (unsigned long long)sp.limit, (unsigned long long)e.first,
+                      (unsigned long long)e.n);
+            return LHB200_EINVAL;
+        }
+        if (e.new_len > old && (e.first > old || e.first + e.n < e.new_len)) {
+            set_error("state_list_edit: field %u grows from %llu to %llu items: all new items must be written", e.field,
+                      (unsigned long long)old, (unsigned long long)e.new_len);
+            return LHB200_EINVAL;
+        }
+        total += e.n * sp.item_bytes;
+    }
+    if (total && !data) return LHB200_EINVAL;
+    if (n_edits == 0) return LHB200_OK;
+    if (!st->converted && (rc = state_convert(st, c.stream))) return rc;
+    for (uint32_t i = 0; i < n_edits; i++) {   // capacity first (doubling), device to device
+        lhb200_state::List& L = list_of(st, list_spec_of(st, edits[i].field));
+        if (edits[i].new_len > L.cap && (rc = list_alloc(st, L, std::max(edits[i].new_len, 2 * L.cap), c.stream))) return rc;
+    }
+    uint8_t* h = total ? static_cast<uint8_t*>(pinned_scratch(total)) : nullptr;
+    if (total && !h) return LHB200_ENOMEM;
+    if (total) memcpy(h, data, total);
+    uint64_t off = 0;
+    for (uint32_t i = 0; i < n_edits; i++) {
+        const lhb200_list_edit& e = edits[i];
+        lhb200_state::List& L = list_of(st, list_spec_of(st, e.field));
+        const uint64_t ib = LIST_SPECS[L.spec].item_bytes;
+        if (e.n) LHB_CUDA(cudaMemcpyAsync(L.d_mem + e.first * ib, h + off, e.n * ib, cudaMemcpyHostToDevice, c.stream));
+        off += e.n * ib;
+        if ((rc = list_set_length(st, L, e.new_len, e.first, e.n, c.stream))) return rc;
+    }
+    state_relayout(st);
+    LHB_CUDA(cudaStreamSynchronize(c.stream));   // the staging slab is reused by the next call
+    return LHB200_OK;
+}
+
+int32_t lhb200_state_list_len(const lhb200_state* st, uint32_t field, uint64_t* len) {
+    LHB_REQUIRE_READY();
+    if (!st || !len) return LHB200_EINVAL;
+    const int k = list_spec_of(st, field);
+    if (k < 0) { set_error("state_list_len: field %u is not a resizable list of this fork", field); return LHB200_EINVAL; }
+    *len = st->var_len[LIST_SPECS[k].var] / LIST_SPECS[k].item_bytes;
+    return LHB200_OK;
+}
+
+// The header hashes the same way whatever extra_data's length (one literal chunk and one length literal), so a
+// replacement rewrites literal chunks and moves the offsets of the variable-size fields after it.
+int32_t lhb200_state_set_payload_header(lhb200_state* st, const uint8_t* ssz, uint64_t len) {
+    LHB_REQUIRE_READY();
+    if (!st || (len && !ssz)) return LHB200_EINVAL;
+    Ctx& c = ctx();
+    std::lock_guard<std::recursive_mutex> g(c.mu);
+    int32_t rc = check_resizable(st, "state_set_payload_header");
+    if (rc) return rc;
+    const ForkLayout& fl = *fork_layout(st->shard.fork);
+    if (!fl.payload_fields) { set_error("state_set_payload_header: this fork has no execution payload header"); return LHB200_EINVAL; }
+    Span v[1];
+    if (!read_offsets(ssz, len, fl.header_fixed, block_layout::HEADER_VAR_POS, v) || !v[0].fits(1, 32)) {
+        set_error("state_set_payload_header: malformed ExecutionPayloadHeader SSZ (%llu bytes)", (unsigned long long)len);
+        return LHB200_EINVAL;
+    }
+    if (!st->converted && (rc = state_convert(st, c.stream))) return rc;
+    Plan& pl = st->plan;
+    uint32_t lo = st->hdr_len_chunk, hi = st->hdr_len_chunk + 1;
+    for (const auto& hl : st->hdr_lits) {
+        Plan::LitSrc& ls = pl.lit_src[hl.first];
+        if ((int)hl.first == st->hdr_extra) ls.n = (uint32_t)v[0].len;
+        uint8_t* chunk = &pl.lit[(size_t)ls.lit_index * 32];
+        memset(chunk, 0, 32);
+        memcpy(chunk, ssz + hl.second, ls.n);
+        lo = std::min(lo, ls.lit_index);
+        hi = std::max(hi, ls.lit_index + 1);
+    }
+    uint8_t* lc = &pl.lit[(size_t)st->hdr_len_chunk * 32];
+    memset(lc, 0, 32);
+    for (int k = 0; k < 8; k++) lc[k] = (uint8_t)(v[0].len >> (8 * k));
+    const size_t lb = (size_t)(hi - lo) * 32;
+    uint8_t* h = static_cast<uint8_t*>(pinned_scratch(lb));
+    if (!h) return LHB200_ENOMEM;
+    memcpy(h, &pl.lit[(size_t)lo * 32], lb);
+    LHB_CUDA(cudaMemcpyAsync(pl.arena + pl.lit_off + (size_t)lo * 32, h, lb, cudaMemcpyHostToDevice, c.stream));
+    st->var_len[state_layout::V_LEPH] = len;
+    state_relayout(st);
+    LHB_CUDA(cudaStreamSynchronize(c.stream));
+    return LHB200_OK;
+}
+
 int32_t lhb200_state_root_enqueue(lhb200_state* st, void* stream, const void** d_root) {
     LHB_REQUIRE_READY();
     if (!st) return LHB200_EINVAL;
@@ -1375,7 +1902,9 @@ int32_t lhb200_state_root_enqueue(lhb200_state* st, void* stream, const void** d
     int32_t rc;
     rc = 1;
     if (st->incremental && !st->need_full) rc = state_incremental_enqueue(st, s);
-    if (rc > 0) {
+    if (rc > 0 && st->converted) {
+        rc = state_converted_cold(st, s);
+    } else if (rc > 0) {
         rc = plan_enqueue(st->plan, s, st->e_k0, st->e_k1);
         st->last_root_hashes = st->plan.hash_units;
         if (!rc && st->incremental) rc = state_build_levels(st, s);   // a cold root leaves the level arrays stale
@@ -1419,6 +1948,7 @@ int32_t lhb200_state_release(lhb200_state* st) {
     if (st->d_trees) cudaFree(st->d_trees);
     if (st->d_dirty) cudaFree(st->d_dirty);
     if (st->d_coll) cudaFree(st->d_coll);
+    for (const lhb200_state::List& L : st->lists) cudaFree(L.d_mem);
     delete st;
     return LHB200_OK;
 }

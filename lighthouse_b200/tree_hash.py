@@ -204,17 +204,22 @@ class ShardedState:
 
 
 class ResidentState:
-    """A BeaconStateDeneb staged once into HBM (DESIGN.md §3) and hashed from there."""
+    """A BeaconState staged once into HBM (DESIGN.md §3) and hashed from there.  `fork` in altair / bellatrix / capella /
+    deneb / electra; Deneb stages through lhb200_state_stage_deneb, the others through lhb200_state_stage."""
 
-    def __init__(self, ssz):
+    def __init__(self, ssz, fork="deneb"):
         self._h = C.c_void_p()
+        self.fork = fork
         p, keep = buf(ssz)
         n = len(ssz) if isinstance(ssz, (bytes, bytearray)) else keep.nbytes
-        check(lib.lhb200_state_stage_deneb(p, n, C.byref(self._h)), "lhb200_state_stage_deneb")
+        if fork == "deneb":
+            check(lib.lhb200_state_stage_deneb(p, n, C.byref(self._h)), "lhb200_state_stage_deneb")
+        else:
+            check(lib.lhb200_state_stage(p, n, FORKS[fork], C.byref(self._h)), "lhb200_state_stage")
 
     def root(self, want_field_roots=False):
         out = C.create_string_buffer(32)
-        n_fr = _n_field_roots("deneb")
+        n_fr = _n_field_roots(self.fork)
         fr = C.create_string_buffer(n_fr * 32) if want_field_roots else None
         check(lib.lhb200_state_root(self._h, out, fr), "lhb200_state_root")
         if want_field_roots:
@@ -242,6 +247,51 @@ class ResidentState:
         """Warm path: keep every level of the big lists resident; later root() calls re-hash only the paths above
         the leaves patch() touched (the reference's tree-hash-cache behaviour, beacon_state.rs:2031-2038)."""
         check(lib.lhb200_state_enable_incremental(self._h), "lhb200_state_enable_incremental")
+
+    def _list_field(self, field):
+        """(container index, item bytes) of a resizable list named as in ssz_schema (or given by index)."""
+        from .ssz_schema import BEACON_STATE_BY_FORK, fixed_size
+        fields = BEACON_STATE_BY_FORK[self.fork][1]
+        idx = field if isinstance(field, int) else [name for name, _ in fields].index(field)
+        t = fields[idx][1]
+        return idx, (fixed_size(t[1]) if t[0] == "list" else 0)
+
+    def list_edit(self, edits):
+        """Resize and write lists in one call (lhb200_state_list_edit): [(field, new_len, first, items_ssz), ...], at most
+        one edit per field; items_ssz holds the SSZ bytes of items [first, first + n).  Needs enable_incremental()."""
+        edits = list(edits)
+        arr = (_ffi.ListEdit * max(len(edits), 1))()
+        blobs = []
+        for i, (field, new_len, first, data) in enumerate(edits):
+            idx, item = self._list_field(field)
+            data = bytes(data)
+            if item == 0 or len(data) % item:
+                raise ValueError(f"{field}: not a list of fixed-size items, or {len(data)} bytes is not whole items")
+            arr[i] = _ffi.ListEdit(idx, 0, new_len, first, len(data) // item)
+            blobs.append(data)
+        p, keep = buf(b"".join(blobs))
+        check(lib.lhb200_state_list_edit(self._h, C.cast(arr, C.c_void_p), len(edits), p), "lhb200_state_list_edit")
+
+    def append(self, field, items_ssz):
+        """Append the SSZ items to list `field` (a deposit, an eth1 vote, a historical summary, ...)."""
+        n = self.list_len(field)
+        _, item = self._list_field(field)
+        self.list_edit([(field, n + len(items_ssz) // max(item, 1), n, items_ssz)])
+
+    def truncate(self, field, new_len):
+        """Shorten list `field` to new_len items (0: reset)."""
+        self.list_edit([(field, new_len, new_len, b"")])
+
+    def list_len(self, field):
+        idx, _ = self._list_field(field)
+        n = C.c_uint64(0)
+        check(lib.lhb200_state_list_len(self._h, idx, C.byref(n)), "lhb200_state_list_len")
+        return n.value
+
+    def set_payload_header(self, ssz):
+        """Replace latest_execution_payload_header with SSZ of this fork's header (extra_data may change length)."""
+        p, keep = buf(ssz)
+        check(lib.lhb200_state_set_payload_header(self._h, p, len(ssz)), "lhb200_state_set_payload_header")
 
     @property
     def last_root_hashes(self):
