@@ -7,7 +7,6 @@
 #include <algorithm>
 #include <array>
 #include <memory>
-#include <unordered_map>
 #include <vector>
 #include "ctx.h"
 #include "merkle.cuh"
@@ -45,15 +44,21 @@ int32_t merkle_init() {
 // All device memory a plan touches lives in one arena: [staged inputs | scratch nodes | literals | slots].
 
 // The leaf kernel of a big list turns each fixed-size SSZ item into its 32-byte root, at `units` hash32_concat each.
+// `tree` is the TreeDev kind that recomputes one leaf on the warm path.
 struct LeafKind {
     enum Kernel { NONE, VALIDATORS, RECORDS, HASH_PAIRS } kernel;   // NONE: the items already are the chunks
-    int record;                                                     // k_record_roots kind (RECORDS only)
+    uint32_t tree;                                                  // RECORDS: TREE_RECORDS + its k_record_roots kind
     uint32_t units;
 };
-constexpr LeafKind LEAF_NONE{LeafKind::NONE, 0, 0}, LEAF_VALIDATOR{LeafKind::VALIDATORS, 0, 8},
-                   LEAF_PUBKEY{LeafKind::RECORDS, 0, 1}, LEAF_ETH1_DATA{LeafKind::RECORDS, 1, 3},
-                   LEAF_U64_PAIR{LeafKind::RECORDS, 2, 1}, LEAF_U64_TRIPLE{LeafKind::RECORDS, 3, 3},
-                   LEAF_DEPOSIT_REQUEST{LeafKind::RECORDS, 4, 10}, LEAF_CHUNK_PAIR{LeafKind::HASH_PAIRS, 0, 1};
+constexpr LeafKind LEAF_NONE{LeafKind::NONE, TREE_CHUNKS, 0},
+                   LEAF_VALIDATOR{LeafKind::VALIDATORS, TREE_VALIDATORS, 8},
+                   LEAF_PUBKEY{LeafKind::RECORDS, TREE_RECORDS + REC_PUBKEY, 1},
+                   LEAF_ETH1_DATA{LeafKind::RECORDS, TREE_RECORDS + REC_ETH1_DATA, 3},
+                   LEAF_U64_PAIR{LeafKind::RECORDS, TREE_RECORDS + REC_U64_PAIR, 1},
+                   LEAF_U64_TRIPLE{LeafKind::RECORDS, TREE_RECORDS + REC_U64_TRIPLE, 3},
+                   LEAF_DEPOSIT_REQUEST{LeafKind::RECORDS, TREE_RECORDS + REC_DEPOSIT_REQUEST, 10},
+                   // HistoricalSummary {H256, H256}: one pair hash, which the warm path runs as a record
+                   LEAF_CHUNK_PAIR{LeafKind::HASH_PAIRS, TREE_RECORDS + REC_HISTORICAL_SUMMARY, 1};
 
 struct LeafLaunch {
     LeafKind kind;
@@ -83,10 +88,10 @@ struct Plan {
     ByteItem* d_items = nullptr;
     std::vector<int32_t> h_waves;                      // host copy of the wave table (wide waves get their own launch)
     uint64_t forced_dst = 0;                           // destination of the next op_hash (0 = allocate)
-    // lists big enough for reduce passes: where their leaf chunks live and where the tail program reads their data
-    // root (for the warm path, lhb200_state_enable_incremental)
-    struct TreeSpec { const uint8_t* chunks; uint64_t n_chunks; uint64_t top_addr; const uint8_t* src; int kind;
-                      uint64_t src_off, src_bytes; uint32_t item_bytes; };
+    // big fields of a staged state that keep a tree for the warm path (lhb200_state_enable_incremental): where their
+    // leaf chunks live, where the tail program reads their data root, and the staged copy (SSZ items) they come from
+    struct TreeSpec { const uint8_t* chunks; uint64_t n_chunks; uint64_t top_addr; const uint8_t* src; LeafKind leaf;
+                      size_t copy; uint32_t item_bytes; };
     std::vector<TreeSpec> trees;
     uint64_t hash_units = 0;
     // SSZ provenance of literal chunks (for lhb200_state_patch): chunk index <- n bytes at SSZ offset src_off
@@ -182,8 +187,9 @@ struct Plan {
         hash_units += mix ? 1 : 0;
         return reinterpret_cast<uint64_t>(out);
     }
-    // merkleize n chunks resident at d_in (16-B aligned) with limit 2^depth
-    uint64_t merkle_list(const uint8_t* d_in, uint64_t n, uint32_t depth) {
+    // merkleize n chunks resident at d_in (16-B aligned) with limit 2^depth.  `warm` (optional: src, leaf, copy and
+    // item_bytes) is recorded in `trees` with the chunks and the data root when reduce passes build the tree.
+    uint64_t merkle_list(const uint8_t* d_in, uint64_t n, uint32_t depth, const TreeSpec* warm = nullptr) {
         if (n == 0) return zero_op(depth);
         if (n <= 8) {
             std::vector<uint64_t> nodes;
@@ -214,7 +220,7 @@ struct Plan {
             in = out;
         }
         uint64_t r = reinterpret_cast<uint64_t>(in);
-        trees.push_back({d_in, hash_units_n0, r, nullptr, 1, ~0ull, 0, 32});
+        if (warm) trees.push_back({d_in, hash_units_n0, r, warm->src, warm->leaf, warm->copy, warm->item_bytes});
         for (uint32_t l = level; l < depth; l++) r = op_hash(r, zero_op(l));
         return r;
     }
@@ -227,25 +233,28 @@ struct Plan {
 };
 
 static int32_t plan_enqueue_tail(Plan& pl, cudaStream_t s);
+// Roots of n validators (TREE_VALIDATORS) or records (TREE_RECORDS + kind) at `in` -> chunks at `out`.  e0 / e1
+// (optional) are recorded around k_validator_roots.
+static void enqueue_leaf_roots(uint32_t tree_kind, const uint8_t* in, uint64_t n, uint8_t* out, cudaStream_t s,
+                               cudaEvent_t e0, cudaEvent_t e1) {
+    if (tree_kind == TREE_VALIDATORS) {
+        if (e0) cudaEventRecord(e0, s);
+        k_validator_roots<<<(unsigned)ceil_div(n, VAL_PER_CTA), VAL_PER_CTA, 0, s>>>(in, n, out);
+        if (e1) cudaEventRecord(e1, s);
+    } else {
+        k_record_roots<<<(unsigned)ceil_div(n, 128), 128, 0, s>>>(in, n, (int)(tree_kind - TREE_RECORDS), out);
+    }
+    count_launch();
+}
 // Leaf kernels, reduce passes and byte items of a plan: everything before its tail hash program.
 static void plan_enqueue_body(Plan& pl, cudaStream_t s, cudaEvent_t e0 = nullptr, cudaEvent_t e1 = nullptr) {
-    for (const LeafLaunch& L : pl.leaves) {
-        switch (L.kind.kernel) {
-            case LeafKind::VALIDATORS:
-                if (e0) cudaEventRecord(e0, s);
-                k_validator_roots<<<(unsigned)ceil_div(L.n, VAL_PER_CTA), VAL_PER_CTA, 0, s>>>(L.in, L.n, L.out);
-                if (e1) cudaEventRecord(e1, s);
-                break;
-            case LeafKind::RECORDS:
-                k_record_roots<<<(unsigned)ceil_div(L.n, 128), 128, 0, s>>>(L.in, L.n, L.kind.record, L.out);
-                break;
-            case LeafKind::HASH_PAIRS:
-                k_hash_pairs<<<(unsigned)ceil_div(L.n, 256), 256, 0, s>>>(L.in, L.out, L.n);
-                break;
-            case LeafKind::NONE:
-                break;   // leaf_kernel is never called without a kernel
+    for (const LeafLaunch& L : pl.leaves) {   // leaf_kernel is never called without a kernel
+        if (L.kind.kernel == LeafKind::HASH_PAIRS) {
+            k_hash_pairs<<<(unsigned)ceil_div(L.n, 256), 256, 0, s>>>(L.in, L.out, L.n);
+            count_launch();
+        } else {
+            enqueue_leaf_roots(L.kind.tree, L.in, L.n, L.out, s, e0, e1);
         }
-        count_launch();
     }
     for (auto& pass : pl.passes) {
         for (size_t i = 0; i < pass.size(); i += MAX_SEGS) {
@@ -560,6 +569,14 @@ struct StageCopy {
     size_t pad_to;  // zero-fill up to this many bytes at dst
 };
 
+// Sizes of a staged state's plan and copies when the describer starts a field: field k emitted everything from
+// marks[k] up to marks[k + 1], which is how a conversion to resizable lists drops the lists' share of the plan.
+struct PlanMark {
+    size_t ops, leaves, copies, trees;
+    std::vector<size_t> passes;   // segments of each reduce pass
+    size_t pass(size_t q) const { return q < passes.size() ? passes[q] : 0; }
+};
+
 struct ShardCfg {
     uint32_t rank = 0, world = 1;
     int32_t fork = LHB200_FORK_DENEB;   // which BeaconState variant the SSZ is (FORK_LAYOUTS)
@@ -601,12 +618,13 @@ struct lhb200_state {
     std::vector<lhb200::StageCopy> copies;  // SSZ ranges resident in the arena (for lhb200_state_patch)
     std::vector<uint32_t> copy_order, lit_order;   // offset-sorted indices into copies / plan.lit_src (patch lookups)
     std::vector<int32_t> copy_tree;         // copies[k] -> index of its resident tree (warm path), -1 if none
-    size_t copy_tree_trees = 0;
+    std::vector<lhb200::PlanMark> marks;    // per field, and one past the last (PlanMark)
     // warm path (lhb200_state_enable_incremental): full level arrays per big list + dirty leaves since the last root
     // dirty leaves since the last root: a host BITMAP per tree (marking is O(1) per edit and dedups for free; the next
     // root extracts the sorted index list with a ctz scan — no sort) plus the number of marks made
     struct Tree {
-        lhb200::TreeDev dev; uint64_t src_off, src_bytes; uint32_t item_bytes;   // item_bytes: SSZ bytes per leaf
+        lhb200::TreeDev dev; lhb200::LeafKind leaf;
+        size_t copy; uint32_t item_bytes;   // the copy holding its SSZ bytes, item_bytes of them per leaf
         std::vector<uint64_t> dirty_bits; std::vector<uint32_t> dirty; uint64_t n_marks = 0;
         int list = -1;                   // index into `lists` for a resizable list
         void mark(uint64_t leaf) { dirty_bits[leaf >> 6] |= 1ull << (leaf & 63); n_marks++; }
@@ -626,7 +644,6 @@ struct lhb200_state {
     struct List {
         int spec;                        // index into LIST_SPECS
         int tree;                        // index into `trees`
-        size_t copy;                     // index into `copies` (patches address the list through it)
         uint64_t cap = 0;                // items the storage holds
         uint8_t* d_mem = nullptr;
         bool resized = false;            // length changed since the last root: the finishing step must run
@@ -651,6 +668,8 @@ struct SszDescriber {
     const uint8_t* d;
     const ForkLayout& fl;
     bool bad = false;
+    int extra_lit = -1;             // literal extra_data: its lit_src index and the literal chunk holding its length
+    uint32_t extra_len_chunk = 0;
 
     uint64_t fail() { bad = true; return 0; }
     uint64_t u64(uint64_t off) { return p.literal_bytes(s + off, 8); }
@@ -674,7 +693,10 @@ struct SszDescriber {
     // extra_data: ByteList[32] at s[off, off + n)
     uint64_t extra_data(uint64_t off, uint64_t n) {
         if (d) return p.bytes_item(d + off, n, 0, true, n);
-        return p.mix_in_length(p.literal_bytes(s + off, n), n);
+        extra_lit = (int)p.lit_src.size();
+        const uint64_t chunk = p.literal_bytes(s + off, n);
+        extra_len_chunk = (uint32_t)(p.lit.size() / 32);   // the next literal: mix_in_length's length
+        return p.mix_in_length(chunk, n);
     }
     // The first fields of ExecutionPayload and ExecutionPayloadHeader (execution_payload.rs:54-95), extra_data checked
     // by the caller
@@ -698,12 +720,41 @@ struct SszDescriber {
     }
 };
 
-// Describe a whole BeaconState of any fork.  `s` = host SSZ (read for offsets and small literal fields only).
-// Big fields are placed in the arena by `place(src_off, nbytes)` which records an H2D copy.  The fields every fork has
-// come first, then the ones later forks append, up to the fork's field count.
-static int32_t describe_state(Plan& p, const uint8_t* s, uint64_t len, std::vector<StageCopy>* copies,
-                              uint64_t* field_ops, uint64_t* root_op, ShardCfg sh, std::vector<ShardedList>* sharded) {
+// The resizable lists of a BeaconState, in field order (limits eth_spec.rs:389-440).  Staging checks their lengths
+// against these limits and describes them with these leaf kinds; lhb200_state_list_edit resizes them.
+struct ListSpec {
+    uint32_t field;        // index in the state container
+    int var;               // state_layout::V_*
+    uint32_t item_bytes;
+    uint64_t limit;        // items
+    uint32_t depth;        // chunk-tree depth of the limit
+    LeafKind leaf;
+};
+static const ListSpec LIST_SPECS[] = {
+    {9, state_layout::V_VOTES, 72, 2048, 11, LEAF_ETH1_DATA},
+    {11, state_layout::V_VAL, 121, 1ull << 40, 40, LEAF_VALIDATOR},
+    {12, state_layout::V_BAL, 8, 1ull << 40, 38, LEAF_NONE},
+    {15, state_layout::V_PP, 1, 1ull << 40, 35, LEAF_NONE},
+    {16, state_layout::V_CP, 1, 1ull << 40, 35, LEAF_NONE},
+    {21, state_layout::V_INACT, 8, 1ull << 40, 38, LEAF_NONE},
+    {27, state_layout::V_HS, 64, 1ull << 24, 24, LEAF_CHUNK_PAIR},
+    {34, state_layout::V_PBD, 16, 1ull << 27, 27, LEAF_U64_PAIR},
+    {35, state_layout::V_PPW, 24, 1ull << 27, 27, LEAF_U64_TRIPLE},
+    {36, state_layout::V_PC, 16, 1ull << 18, 18, LEAF_U64_PAIR},
+};
+constexpr int N_LIST_SPECS = sizeof(LIST_SPECS) / sizeof(LIST_SPECS[0]);
+static_assert(N_LIST_SPECS <= MAX_FINISH, "one finishing thread per list");
+static uint64_t list_leaves(const ListSpec& sp, uint64_t len) {
+    return sp.leaf.tree == TREE_CHUNKS ? ceil_div(len * sp.item_bytes, 32) : len;
+}
+
+// Describe a whole BeaconState of any fork into `p` and the handle `st` (its copies, field and root operands, sharded
+// lists, marks and header literals).  `s` = host SSZ (read for offsets and small literal fields only).  Big fields
+// are placed in the arena by `place(src_off, nbytes)` which records an H2D copy.  Fields are described in order, up
+// to the fork's field count, each one's plan after the previous one's (st->marks).
+static int32_t describe_state(Plan& p, const uint8_t* s, uint64_t len, lhb200_state* st) {
     using namespace state_layout;
+    const ShardCfg sh = st->shard;
     const ForkLayout* fl = fork_layout(sh.fork);
     if (!fl) { set_error("unknown fork id %d", sh.fork); return LHB200_EINVAL; }
     Span v[N_VAR];
@@ -711,42 +762,40 @@ static int32_t describe_state(Plan& p, const uint8_t* s, uint64_t len, std::vect
         set_error("BeaconState SSZ: shorter than its fixed part or inconsistent variable-part offsets");
         return LHB200_EINVAL;
     }
-    if (!v[V_HIST].fits(32, 1u << 24) || !v[V_VOTES].fits(72, 2048) || !v[V_VAL].fits(121, 1ull << 40) ||
-        !v[V_BAL].fits(8, 1ull << 40) || !v[V_INACT].fits(8, 1ull << 40) || !v[V_HS].fits(64, 1u << 24) ||
-        !v[V_PBD].fits(16, 1u << 27) || !v[V_PPW].fits(24, 1u << 27) || !v[V_PC].fits(16, 1u << 18)) {
+    bool fits = v[V_HIST].fits(32, 1u << 24);   // historical_roots: a list, but not a resizable one
+    for (const ListSpec& sp : LIST_SPECS) fits = fits && v[sp.var].fits(sp.item_bytes, sp.limit);
+    if (!fits) {
         set_error("BeaconState SSZ: malformed variable part");
         return LHB200_EINVAL;
     }
-    const uint64_t n_hist = v[V_HIST].len / 32, n_val = v[V_VAL].len / 121, n_bal = v[V_BAL].len / 8,
-                   n_pp = v[V_PP].len, n_cp = v[V_CP].len, n_inact = v[V_INACT].len / 8;
+    const uint64_t n_hist = v[V_HIST].len / 32;
     SszDescriber c{p, s, nullptr, *fl};
     p.ssz_base = s;
     p.ssz_len = len;
+    st->copies.clear();
+    st->sharded.clear();
+    st->marks.clear();
+    st->hdr_lits.clear();
     auto place = [&](size_t src_off, size_t nbytes) -> uint8_t* {
         size_t padded = align_up(nbytes + 32, 256);
         uint8_t* d = p.alloc(padded);
-        if (copies) copies->push_back({src_off, nbytes, d, padded});
+        st->copies.push_back({src_off, nbytes, d, padded});
         return d;
     };
-    uint64_t* f = field_ops;
+    uint64_t* f = st->field_ops;
     const uint32_t lg_world = ceil_log2(sh.world);
     // Big list with `n_chunks` leaf chunks produced from `n_items` source items of `item_bytes` at `src_off`
     // (LEAF_NONE: the bytes already are the chunks).  Unsharded: the full field root.  Sharded: this rank's subtree.
     auto big_list = [&](int field, size_t src_off, uint64_t n_items, uint32_t item_bytes, LeafKind leaf,
                         uint64_t n_chunks, uint32_t limit_depth, uint64_t mix_len) -> uint64_t {
         const uint32_t d0 = ceil_log2(std::max<uint64_t>(n_chunks, 1));
-        const bool shard = sh.world > 1 && sharded && d0 >= lg_world + 6;
-        const bool validators = leaf.kernel == LeafKind::VALIDATORS, packed = leaf.kernel == LeafKind::NONE;
+        const bool shard = sh.world > 1 && d0 >= lg_world + 6;
+        const bool packed = leaf.kernel == LeafKind::NONE;
         if (!shard) {
             const uint8_t* src = place(src_off, n_items * item_bytes);
             const uint8_t* chunks = packed ? src : p.leaf_kernel(leaf, src, n_items);
-            const size_t nt = p.trees.size();
-            uint64_t r = p.merkle_list(chunks, n_chunks, limit_depth);
-            if (p.trees.size() > nt && (validators || packed)) {   // warm-path provenance
-                Plan::TreeSpec& t = p.trees.back();
-                t.src = src; t.kind = validators ? 0 : 1; t.src_off = src_off; t.src_bytes = n_items * item_bytes;
-                t.item_bytes = validators ? item_bytes : 32;
-            }
+            const Plan::TreeSpec warm{nullptr, 0, 0, src, leaf, st->copies.size() - 1, packed ? 32 : item_bytes};
+            const uint64_t r = p.merkle_list(chunks, n_chunks, limit_depth, &warm);
             return mix_len == UINT64_MAX ? r : p.mix_in_length(r, mix_len);
         }
         const uint32_t sub = d0 - lg_world;
@@ -763,65 +812,77 @@ static int32_t describe_state(Plan& p, const uint8_t* s, uint64_t len, std::vect
             const uint8_t* src = place(src_off + b_lo, b_hi > b_lo ? b_hi - b_lo : 0);
             op = p.merkle_list(src, cnt, sub);
         }
-        sharded->push_back({field, sub, limit_depth, mix_len, op});
+        st->sharded.push_back({field, sub, limit_depth, mix_len, op});
         return Plan::zero_op(0);       // placeholder; the field root is formed in lhb200_state_combine
     };
-    // list of fixed-size records (one leaf-kernel root each) with limit 2^depth
-    auto records = [&](LeafKind leaf, Span x, uint32_t item_bytes, uint32_t depth) {
-        const uint64_t n = x.len / item_bytes;
-        return p.mix_in_length(p.merkle_list(p.leaf_kernel(leaf, place(x.off, x.len), n), n, depth), n);
+    // a resizable list: validators and packed lists are big lists, records get one leaf-kernel root each
+    auto list = [&](const ListSpec& sp) {
+        const Span x = v[sp.var];
+        const uint64_t n = x.len / sp.item_bytes;
+        if (sp.leaf.kernel == LeafKind::VALIDATORS || sp.leaf.kernel == LeafKind::NONE)
+            return big_list(sp.field, x.off, n, sp.item_bytes, sp.leaf, list_leaves(sp, n), sp.depth, n);
+        return p.mix_in_length(p.merkle_list(p.leaf_kernel(sp.leaf, place(x.off, x.len), n), n, sp.depth), n);
     };
-    f[0] = c.u64(O_GENESIS_TIME);
-    f[1] = c.h256(O_GVR);
-    f[2] = c.u64(O_SLOT);
-    f[3] = p.container({p.literal_bytes(s + O_FORK, 4), p.literal_bytes(s + O_FORK + 4, 4), c.u64(O_FORK + 8)});
-    f[4] = c.block_header(O_LBH);
     auto plain_vector = [&](uint32_t off, uint64_t nbytes, uint32_t depth) {   // fixed vectors of chunks / packed u64
         const uint8_t* src = place(off, nbytes);
-        const size_t nt = p.trees.size();
-        uint64_t r = p.merkle_list(src, nbytes / 32, depth);
-        if (p.trees.size() > nt) {
-            Plan::TreeSpec& t = p.trees.back();
-            t.src = src; t.kind = 1; t.src_off = off; t.src_bytes = nbytes; t.item_bytes = 32;
-        }
-        return r;
+        const Plan::TreeSpec warm{nullptr, 0, 0, src, LEAF_NONE, st->copies.size() - 1, 32};
+        return p.merkle_list(src, nbytes / 32, depth, &warm);
     };
-    f[5] = plain_vector(O_BLOCK_ROOTS, 8192 * 32, 13);
-    f[6] = plain_vector(O_STATE_ROOTS, 8192 * 32, 13);
-    f[7] = p.mix_in_length(p.merkle_list(place(v[V_HIST].off, v[V_HIST].len), n_hist, 24), n_hist);
-    f[8] = c.eth1_data(O_ETH1_DATA);
-    f[9] = records(LEAF_ETH1_DATA, v[V_VOTES], 72, 11);
-    f[10] = c.u64(O_DEPOSIT_INDEX);
-    f[11] = big_list(11, v[V_VAL].off, n_val, 121, LEAF_VALIDATOR, n_val, 40, n_val);
-    f[12] = big_list(12, v[V_BAL].off, n_bal, 8, LEAF_NONE, ceil_div(n_bal * 8, 32), 38, n_bal);
-    f[13] = big_list(13, O_RANDAO, 65536, 32, LEAF_NONE, 65536, 16, UINT64_MAX);
-    f[14] = plain_vector(O_SLASHINGS, 8192 * 8, 11);
-    f[15] = big_list(15, v[V_PP].off, n_pp, 1, LEAF_NONE, ceil_div(n_pp, 32), 35, n_pp);
-    f[16] = big_list(16, v[V_CP].off, n_cp, 1, LEAF_NONE, ceil_div(n_cp, 32), 35, n_cp);
-    f[17] = p.literal_bytes(s + O_JUST, 1);
-    f[18] = c.checkpoint(O_PJC);
-    f[19] = c.checkpoint(O_CJC);
-    f[20] = c.checkpoint(O_FC);
-    f[21] = big_list(21, v[V_INACT].off, n_inact, 8, LEAF_NONE, ceil_div(n_inact * 8, 32), 38, n_inact);
-    for (int k = 0; k < 2; k++) {
-        uint8_t* roots = p.leaf_kernel(LEAF_PUBKEY, place(k ? O_NSC : O_CSC, SYNC_COMMITTEE_BYTES), 513);
-        f[22 + k] = p.container({p.merkle_list(roots, 512, 9), reinterpret_cast<uint64_t>(roots + 512 * 32)});
-    }
-    for (int k = 24; k < fl->state_fields; k++) {   // appended by later forks (beacon_state.rs:339-525)
+    auto mark = [&] {
+        PlanMark m{p.ops.size(), p.leaves.size(), st->copies.size(), p.trees.size(), {}};
+        for (const auto& pass : p.passes) m.passes.push_back(pass.size());
+        st->marks.push_back(std::move(m));
+    };
+    const ListSpec* next_list = LIST_SPECS;   // in field order
+    for (int k = 0; k < fl->state_fields; k++) {   // fields 24 on: appended by later forks (beacon_state.rs:339-525)
+        mark();
+        if (next_list < LIST_SPECS + N_LIST_SPECS && (int)next_list->field == k) {
+            f[k] = list(*next_list++);
+            continue;
+        }
         switch (k) {
-            case 24: f[k] = c.payload_header(v[V_LEPH].off, v[V_LEPH].len); break;
+            case 0: f[k] = c.u64(O_GENESIS_TIME); break;
+            case 1: f[k] = c.h256(O_GVR); break;
+            case 2: f[k] = c.u64(O_SLOT); break;
+            case 3:
+                f[k] = p.container({p.literal_bytes(s + O_FORK, 4), p.literal_bytes(s + O_FORK + 4, 4), c.u64(O_FORK + 8)});
+                break;
+            case 4: f[k] = c.block_header(O_LBH); break;
+            case 5: f[k] = plain_vector(O_BLOCK_ROOTS, 8192 * 32, 13); break;
+            case 6: f[k] = plain_vector(O_STATE_ROOTS, 8192 * 32, 13); break;
+            case 7: f[k] = p.mix_in_length(p.merkle_list(place(v[V_HIST].off, v[V_HIST].len), n_hist, 24), n_hist); break;
+            case 8: f[k] = c.eth1_data(O_ETH1_DATA); break;
+            case 10: f[k] = c.u64(O_DEPOSIT_INDEX); break;
+            case 13: f[k] = big_list(13, O_RANDAO, 65536, 32, LEAF_NONE, 65536, 16, UINT64_MAX); break;
+            case 14: f[k] = plain_vector(O_SLASHINGS, 8192 * 8, 11); break;
+            case 17: f[k] = p.literal_bytes(s + O_JUST, 1); break;
+            case 18: f[k] = c.checkpoint(O_PJC); break;
+            case 19: f[k] = c.checkpoint(O_CJC); break;
+            case 20: f[k] = c.checkpoint(O_FC); break;
+            case 22:
+            case 23: {
+                uint8_t* roots = p.leaf_kernel(LEAF_PUBKEY, place(k == 23 ? O_NSC : O_CSC, SYNC_COMMITTEE_BYTES), 513);
+                f[k] = p.container({p.merkle_list(roots, 512, 9), reinterpret_cast<uint64_t>(roots + 512 * 32)});
+                break;
+            }
+            case 24: {   // its literals move when an earlier list changes length, and are rewritten by a new header
+                const size_t l0 = p.lit_src.size();
+                f[k] = c.payload_header(v[V_LEPH].off, v[V_LEPH].len);
+                for (size_t i = l0; i < p.lit_src.size(); i++)
+                    st->hdr_lits.push_back({(uint32_t)i, (uint32_t)(p.lit_src[i].src_off - v[V_LEPH].off)});
+                break;
+            }
             case 25: f[k] = c.u64(O_NWI); break;
             case 26: f[k] = c.u64(O_NWVI); break;
-            case 27: f[k] = records(LEAF_CHUNK_PAIR, v[V_HS], 64, 24); break;
-            case 34: f[k] = records(LEAF_U64_PAIR, v[V_PBD], 16, 27); break;
-            case 35: f[k] = records(LEAF_U64_TRIPLE, v[V_PPW], 24, 27); break;
-            case 36: f[k] = records(LEAF_U64_PAIR, v[V_PC], 16, 18); break;
             default: f[k] = c.u64(O_ELECTRA_U64 + 8 * (k - 28)); break;   // 28 .. 33
         }
     }
+    mark();
     if (c.bad) { set_error("BeaconState SSZ: malformed execution payload header"); return LHB200_EINVAL; }
+    st->hdr_extra = c.extra_lit;
+    st->hdr_len_chunk = c.extra_len_chunk;
     for (int k = fl->state_fields; k < MAX_FIELDS; k++) f[k] = Plan::zero_op(0);   // absent in this fork (not part of its container)
-    *root_op = p.container(std::vector<uint64_t>(f, f + fl->state_fields));
+    st->root_op = p.container(std::vector<uint64_t>(f, f + fl->state_fields));
     return LHB200_OK;
 }
 
@@ -880,25 +941,25 @@ static bool visit_resident(const lhb200_state* st, uint64_t lo, uint64_t hi, siz
     }
     return any;
 }
-// Offset order of a handle's copies and literals (built once), and copy_tree (trees appear with enable_incremental).
+// Offset order of a handle's copies and literals, and copy_tree: rebuilt whenever offsets move or trees change
+// (staging, lhb200_state_enable_incremental, list and header edits).  An empty range sorts before a range that starts
+// at the same offset (an empty list and the next field), so that the ends ascend too, as visit_resident's binary
+// search needs.
 static void index_resident(lhb200_state* st) {
-    if (st->copy_order.empty() && !st->copies.empty()) {
-        st->copy_order.resize(st->copies.size());
-        for (size_t k = 0; k < st->copies.size(); k++) st->copy_order[k] = (uint32_t)k;
-        std::sort(st->copy_order.begin(), st->copy_order.end(),
-                  [&](uint32_t a, uint32_t b) { return st->copies[a].src_off < st->copies[b].src_off; });
-        const std::vector<Plan::LitSrc>& ls = st->plan.lit_src;
-        st->lit_order.resize(ls.size());
-        for (size_t k = 0; k < ls.size(); k++) st->lit_order[k] = (uint32_t)k;
-        std::sort(st->lit_order.begin(), st->lit_order.end(),
-                  [&](uint32_t a, uint32_t b) { return ls[a].src_off < ls[b].src_off; });
-    }
-    if (st->copy_tree.size() == st->copies.size() && st->copy_tree_trees == st->trees.size()) return;
+    const std::vector<StageCopy>& cp = st->copies;
+    st->copy_order.resize(cp.size());
+    for (size_t k = 0; k < cp.size(); k++) st->copy_order[k] = (uint32_t)k;
+    std::sort(st->copy_order.begin(), st->copy_order.end(), [&](uint32_t a, uint32_t b) {
+        return cp[a].src_off != cp[b].src_off ? cp[a].src_off < cp[b].src_off : cp[a].nbytes < cp[b].nbytes;
+    });
+    const std::vector<Plan::LitSrc>& ls = st->plan.lit_src;
+    st->lit_order.resize(ls.size());
+    for (size_t k = 0; k < ls.size(); k++) st->lit_order[k] = (uint32_t)k;
+    std::sort(st->lit_order.begin(), st->lit_order.end(), [&](uint32_t a, uint32_t b) {
+        return ls[a].src_off != ls[b].src_off ? ls[a].src_off < ls[b].src_off : ls[a].n < ls[b].n;
+    });
     st->copy_tree.assign(st->copies.size(), -1);
-    for (size_t k = 0; k < st->copies.size(); k++)
-        for (size_t t = 0; t < st->trees.size(); t++)
-            if (st->trees[t].src_off == st->copies[k].src_off) st->copy_tree[k] = (int32_t)t;
-    st->copy_tree_trees = st->trees.size();
+    for (size_t t = 0; t < st->trees.size(); t++) st->copy_tree[st->trees[t].copy] = (int32_t)t;
 }
 
 }  // namespace lhb200
@@ -1042,9 +1103,7 @@ static int32_t stage_state(const uint8_t* ssz, uint64_t len, ShardCfg sh, lhb200
     st->shard = sh;
     constexpr size_t n_result = 1 + MAX_FIELDS;
     int32_t rc = build_sized(st->plan, 16384, n_result * 32 + n_result * sizeof(HashOp) + 1024, [&](Plan& p) {
-        st->copies.clear();
-        st->sharded.clear();
-        return describe_state(p, ssz, len, &st->copies, st->field_ops, &st->root_op, sh, &st->sharded);
+        return describe_state(p, ssz, len, st.get());
     }, [&](size_t need, uint8_t** arena, size_t* bytes) {
         if (g_spare_arena && g_spare_bytes >= need) {   // recycled from the last released handle (no cudaMalloc)
             st->arena = g_spare_arena;
@@ -1090,6 +1149,7 @@ static int32_t stage_state(const uint8_t* ssz, uint64_t len, ShardCfg sh, lhb200
     if (rc) return rc;
     rc = stage_operands(gather, st->d_gather, hst + hg, c.stream);
     if (rc) return rc;
+    index_resident(st.get());
     LHB_CUDA(cudaStreamSynchronize(c.stream));
     *out = st.release();
     return LHB200_OK;
@@ -1208,7 +1268,6 @@ int32_t lhb200_state_patch_batch(lhb200_state* st, const uint64_t* offsets, cons
     ops.reserve(n);
     Plan& pl = st->plan;
     uint32_t lit_lo = ~0u, lit_hi = 0;
-    index_resident(st);
     // pass 1: every edit must hit resident bytes — validated BEFORE anything is modified, so a rejected batch leaves the
     // handle (host literals, dirty lists, device copy) exactly as it was
     auto stop = [](auto&&...) { return false; };
@@ -1232,7 +1291,7 @@ int32_t lhb200_state_patch_batch(lhb200_state* st, const uint64_t* offsets, cons
             const int32_t ti = st->copy_tree[ci];
             if (ti < 0) { st->need_full = true; return true; }     // a list without a resident tree (votes, summaries, ...)
             lhb200_state::Tree& t = st->trees[ti];
-            const uint64_t i0 = (a - t.src_off) / t.item_bytes, i1 = (b - 1 - t.src_off) / t.item_bytes;
+            const uint64_t i0 = (a - cp.src_off) / t.item_bytes, i1 = (b - 1 - cp.src_off) / t.item_bytes;
             if (t.n_marks + (i1 - i0 + 1) > 4ull * lhb200_state::DIRTY_CAP) { st->need_full = true; return true; }
             for (uint64_t q = i0; q <= i1; q++) t.mark(q);
             return true;
@@ -1294,27 +1353,11 @@ static int32_t state_build_levels(lhb200_state* st, cudaStream_t s) {
     return LHB200_OK;
 }
 
-// hash32_concat units of one leaf root of a resident tree (recomputed from its record on the warm path)
-static uint32_t tree_leaf_units(uint32_t kind) {
-    if (kind == TREE_VALIDATORS) return 8;
-    if (kind == TREE_CHUNKS) return 0;
-    const int rec = (int)(kind - TREE_RECORDS);
-    return rec == REC_ETH1_DATA || rec == REC_U64_TRIPLE ? 3 : rec == REC_DEPOSIT_REQUEST ? 10 : 1;
-}
 // Leaf roots of the resizable lists of records and validators, from their items at the current lengths.
 static void lists_enqueue_leaves(lhb200_state* st, cudaStream_t s, cudaEvent_t e0, cudaEvent_t e1) {
     for (const lhb200_state::List& L : st->lists) {
         const TreeDev& d = st->trees[L.tree].dev;
-        if (d.n_leaves == 0 || d.kind == TREE_CHUNKS) continue;
-        if (d.kind == TREE_VALIDATORS) {
-            if (e0) cudaEventRecord(e0, s);
-            k_validator_roots<<<(unsigned)ceil_div(d.n_leaves, VAL_PER_CTA), VAL_PER_CTA, 0, s>>>(d.src, d.n_leaves, d.lvl[0]);
-            if (e1) cudaEventRecord(e1, s);
-        } else {
-            k_record_roots<<<(unsigned)ceil_div(d.n_leaves, 128), 128, 0, s>>>(d.src, d.n_leaves, (int)(d.kind - TREE_RECORDS),
-                                                                                d.lvl[0]);
-        }
-        count_launch();
+        if (d.n_leaves && d.kind != TREE_CHUNKS) enqueue_leaf_roots(d.kind, d.src, d.n_leaves, d.lvl[0], s, e0, e1);
     }
 }
 // Upload the TreeDev table (through the pinned `h`) and run the finishing step of the lists in `fin`.
@@ -1328,28 +1371,31 @@ static int32_t lists_enqueue_finish(lhb200_state* st, const FinishTable& fin, cu
 }
 static uint64_t finish_units(const TreeDev& d) { return (d.n_leaves ? d.limit_depth - d.top : 0) + 1; }
 
-// Cold root of a handle with resizable lists.  The stage-time plan no longer describes those lists (its leaf launches,
-// reduce passes, ladders and mix-ins carried the old lengths and were dropped at conversion), so their trees are
-// rebuilt from the resident items at the current lengths, then the finishing step, then the tail.
-static int32_t state_converted_cold(lhb200_state* st, cudaStream_t s) {
+// Cold root: the plan body, every level of the resident trees (incremental handles), then the tail.  A converted
+// handle's plan no longer describes its resizable lists (their leaf launches, reduce passes, ladders and mix-ins
+// carried the stage-time lengths and were dropped at conversion): their leaf roots come first, from the resident items
+// at the current lengths, and the finishing step writes their field roots before the tail.
+static int32_t state_cold_enqueue(lhb200_state* st, cudaStream_t s) {
     lists_enqueue_leaves(st, s, st->e_k0, st->e_k1);
-    plan_enqueue_body(st->plan, s);
+    plan_enqueue_body(st->plan, s, st->e_k0, st->e_k1);
     int32_t rc = state_build_levels(st, s);
     if (rc) return rc;
-    const size_t tb = st->trees.size() * sizeof(TreeDev);
-    uint8_t* h = static_cast<uint8_t*>(pinned_scratch(tb));
-    if (!h) return LHB200_ENOMEM;
-    FinishTable fin{};
-    for (size_t k = 0; k < st->trees.size(); k++) {
-        lhb200_state::Tree& t = st->trees[k];
-        t.dev.dirty = st->d_dirty;
-        t.dev.n_dirty = 0;
-        memcpy(h + k * sizeof(TreeDev), &t.dev, sizeof(TreeDev));
-        if (t.list >= 0) fin.tree[fin.n++] = (uint32_t)k;
+    if (st->converted) {
+        const size_t tb = st->trees.size() * sizeof(TreeDev);
+        uint8_t* h = static_cast<uint8_t*>(pinned_scratch(tb));
+        if (!h) return LHB200_ENOMEM;
+        FinishTable fin{};
+        for (size_t k = 0; k < st->trees.size(); k++) {
+            lhb200_state::Tree& t = st->trees[k];
+            t.dev.dirty = st->d_dirty;
+            t.dev.n_dirty = 0;
+            memcpy(h + k * sizeof(TreeDev), &t.dev, sizeof(TreeDev));
+            if (t.list >= 0) fin.tree[fin.n++] = (uint32_t)k;
+        }
+        LHB_CUDA(cudaMemcpyAsync(st->d_trees, h, tb, cudaMemcpyHostToDevice, s));
+        rc = lists_enqueue_finish(st, fin, s);
+        if (rc) return rc;
     }
-    LHB_CUDA(cudaMemcpyAsync(st->d_trees, h, tb, cudaMemcpyHostToDevice, s));
-    rc = lists_enqueue_finish(st, fin, s);
-    if (rc) return rc;
     st->last_root_hashes = st->plan.hash_units;
     return plan_enqueue_tail(st->plan, s);
 }
@@ -1408,7 +1454,7 @@ static int32_t state_incremental_enqueue(lhb200_state* st, cudaStream_t s) {
                     const uint32_t hb = 32 - (uint32_t)__builtin_clz(t.dirty[j] ^ t.dirty[j - 1]);  // ancestors equal from level hb up
                     cnt += std::min<uint32_t>(hb - 1, t.dev.top);
                 }
-                hashes += cnt + (uint64_t)tree_leaf_units(t.dev.kind) * t.dirty.size();
+                hashes += cnt + (uint64_t)t.leaf.units * t.dirty.size();
             }
             t.dirty.clear();
         }
@@ -1447,18 +1493,15 @@ int32_t lhb200_state_enable_incremental(lhb200_state* st) {
     Ctx& c = ctx();
     std::lock_guard<std::recursive_mutex> g(c.mu);
     size_t bytes = 0;
-    for (const Plan::TreeSpec& ts : st->plan.trees) {
-        if (ts.src_off == ~0ull) continue;
+    for (const Plan::TreeSpec& ts : st->plan.trees)
         for (uint64_t n = ceil_div(ts.n_chunks, 2);; n = ceil_div(n, 2)) { bytes += align_up(n * 32, 256); if (n == 1) break; }
-    }
     LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_levels), bytes + 256));
     size_t off = 0;
     for (const Plan::TreeSpec& ts : st->plan.trees) {
-        if (ts.src_off == ~0ull) continue;
         lhb200_state::Tree t;
         memset(&t.dev, 0, sizeof t.dev);
         t.dev.src = ts.src;
-        t.dev.kind = (uint32_t)ts.kind;
+        t.dev.kind = ts.leaf.tree;
         t.dev.n_leaves = ts.n_chunks;
         t.dev.top = ceil_log2(ts.n_chunks);
         t.dev.top_dst = reinterpret_cast<uint8_t*>(ts.top_addr);
@@ -1469,12 +1512,13 @@ int32_t lhb200_state_enable_incremental(lhb200_state* st) {
             t.dev.lvl[l] = st->d_levels + off;
             off += align_up(n * 32, 256);
         }
-        t.src_off = ts.src_off; t.src_bytes = ts.src_bytes; t.item_bytes = ts.item_bytes;
+        t.leaf = ts.leaf; t.copy = ts.copy; t.item_bytes = ts.item_bytes;
         t.dirty_bits.assign((ts.n_chunks + 63) / 64, 0ull);
         st->trees.push_back(t);
     }
     LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_trees), st->trees.size() * sizeof(TreeDev) + 256));
     LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_dirty), (size_t)lhb200_state::DIRTY_CAP * 4 * st->trees.size()));
+    index_resident(st);
     st->incremental = true;
     st->need_full = true;   // the first root after enabling is cold and builds the levels
     return LHB200_OK;
@@ -1483,31 +1527,9 @@ uint64_t lhb200_state_last_root_hashes(const lhb200_state* st) { return st ? st-
 
 // ---------------------------------------------------------------------------------------------------------
 // Resizable lists (lhb200_state_list_edit, lhb200_state_set_payload_header).  A handle keeps its stage-time plan until
-// the first such call; then each list of the table below moves to storage of its own with headroom (items, leaf
+// the first such call; then each list of LIST_SPECS moves to storage of its own with headroom (items, leaf
 // chunks, every level), its leaf launches and reduce passes leave the cold plan, and its zero ladder and length mix-in
 // leave the tail program: k_list_finish writes the field root from the list's current top and length instead.
-struct ListSpec {
-    uint32_t field;        // index in the state container
-    int var;               // state_layout::V_*
-    uint32_t item_bytes;
-    uint64_t limit;        // items
-    uint32_t depth;        // chunk-tree depth of the limit
-    uint32_t kind;         // TreeDev kind
-};
-static const ListSpec LIST_SPECS[] = {
-    {9, state_layout::V_VOTES, 72, 2048, 11, TREE_RECORDS + REC_ETH1_DATA},
-    {11, state_layout::V_VAL, 121, 1ull << 40, 40, TREE_VALIDATORS},
-    {12, state_layout::V_BAL, 8, 1ull << 40, 38, TREE_CHUNKS},
-    {15, state_layout::V_PP, 1, 1ull << 40, 35, TREE_CHUNKS},
-    {16, state_layout::V_CP, 1, 1ull << 40, 35, TREE_CHUNKS},
-    {21, state_layout::V_INACT, 8, 1ull << 40, 38, TREE_CHUNKS},
-    {27, state_layout::V_HS, 64, 1ull << 24, 24, TREE_RECORDS + REC_HISTORICAL_SUMMARY},
-    {34, state_layout::V_PBD, 16, 1ull << 27, 27, TREE_RECORDS + REC_U64_PAIR},
-    {35, state_layout::V_PPW, 24, 1ull << 27, 27, TREE_RECORDS + REC_U64_TRIPLE},
-    {36, state_layout::V_PC, 16, 1ull << 18, 18, TREE_RECORDS + REC_U64_PAIR},
-};
-constexpr int N_LIST_SPECS = sizeof(LIST_SPECS) / sizeof(LIST_SPECS[0]);
-static_assert(N_LIST_SPECS <= MAX_FINISH, "one finishing thread per list");
 
 // LIST_SPECS index of the resizable list `field` of the handle's fork, or -1
 static int list_spec_of(const lhb200_state* st, uint32_t field) {
@@ -1521,13 +1543,10 @@ static lhb200_state::List& list_of(lhb200_state* st, int spec) {
         if (L.spec == spec) return L;
     return st->lists.front();   // not reached: a converted handle has every list of its fork
 }
-static uint64_t list_leaves(const ListSpec& sp, uint64_t len) {
-    return sp.kind == TREE_CHUNKS ? ceil_div(len * sp.item_bytes, 32) : len;
-}
 // Hash units the describer counts for a list of `len` items: leaf roots, data tree, zero ladder, length mix-in.
 static uint64_t list_units(const ListSpec& sp, uint64_t len) {
     const uint64_t n = list_leaves(sp, len);
-    uint64_t u = (uint64_t)tree_leaf_units(sp.kind) * len + 1;
+    uint64_t u = (uint64_t)sp.leaf.units * len + 1;
     if (n) {
         const uint32_t top = ceil_log2(n);
         u += sp.depth - top;
@@ -1541,7 +1560,7 @@ static size_t list_place(TreeDev& d, const ListSpec& sp, uintptr_t base, uint64_
     const uint64_t leaves = std::max<uint64_t>(list_leaves(sp, cap), 1);
     size_t off = align_up(cap * sp.item_bytes + 32, 256);
     d.src = reinterpret_cast<const uint8_t*>(base);
-    if (sp.kind == TREE_CHUNKS) {
+    if (sp.leaf.tree == TREE_CHUNKS) {
         d.lvl[0] = reinterpret_cast<uint8_t*>(base);
     } else {
         d.lvl[0] = reinterpret_cast<uint8_t*>(base + off);
@@ -1565,9 +1584,9 @@ static int32_t list_alloc(lhb200_state* st, lhb200_state::List& L, uint64_t cap,
     list_place(d, sp, reinterpret_cast<uintptr_t>(mem), cap);
     if (L.d_mem) {
         const uint64_t n = t.dev.n_leaves;
-        const uint64_t item_bytes = sp.kind == TREE_CHUNKS ? n * 32 : t.dev.length * sp.item_bytes;   // with the zero pad
+        const uint64_t item_bytes = sp.leaf.tree == TREE_CHUNKS ? n * 32 : t.dev.length * sp.item_bytes;   // with the zero pad
         if (item_bytes) LHB_CUDA(cudaMemcpyAsync(mem, L.d_mem, item_bytes, cudaMemcpyDeviceToDevice, s));
-        if (sp.kind != TREE_CHUNKS && n) LHB_CUDA(cudaMemcpyAsync(d.lvl[0], t.dev.lvl[0], n * 32, cudaMemcpyDeviceToDevice, s));
+        if (sp.leaf.tree != TREE_CHUNKS && n) LHB_CUDA(cudaMemcpyAsync(d.lvl[0], t.dev.lvl[0], n * 32, cudaMemcpyDeviceToDevice, s));
         uint64_t m = n;
         for (uint32_t l = 1; l <= t.dev.top; l++) {
             m = ceil_div(m, 2);
@@ -1584,7 +1603,7 @@ static int32_t list_alloc(lhb200_state* st, lhb200_state::List& L, uint64_t cap,
 }
 
 // SSZ offsets of the variable-size fields of the current encoding follow from their lengths: move the lists' resident
-// copies, the payload header's literal sources and the hash-unit count along, and re-sort the patch lookups.
+// copies, the payload header's literal sources and the hash-unit count along, and rebuild the patch lookups.
 static void state_relayout(lhb200_state* st) {
     using namespace state_layout;
     uint64_t off[N_VAR];
@@ -1593,110 +1612,36 @@ static void state_relayout(lhb200_state* st) {
     uint64_t units = st->units_base;
     for (const lhb200_state::List& L : st->lists) {
         const ListSpec& sp = LIST_SPECS[L.spec];
-        lhb200_state::Tree& t = st->trees[L.tree];
-        t.src_off = off[sp.var];
-        t.src_bytes = t.dev.length * sp.item_bytes;
-        st->copies[L.copy] = {t.src_off, t.src_bytes, L.d_mem, 0};
+        const lhb200_state::Tree& t = st->trees[L.tree];
+        st->copies[t.copy] = {off[sp.var], t.dev.length * sp.item_bytes, L.d_mem, 0};
         units += list_units(sp, t.dev.length);
     }
     st->plan.hash_units = units;
     for (const auto& h : st->hdr_lits) st->plan.lit_src[h.first].src_off = off[V_LEPH] + h.second;
-    std::vector<uint32_t>& co = st->copy_order;
-    co.resize(st->copies.size());
-    for (size_t k = 0; k < co.size(); k++) co[k] = (uint32_t)k;
-    std::sort(co.begin(), co.end(), [&](uint32_t a, uint32_t b) { return st->copies[a].src_off < st->copies[b].src_off; });
-    const std::vector<Plan::LitSrc>& ls = st->plan.lit_src;
-    std::sort(st->lit_order.begin(), st->lit_order.end(), [&](uint32_t a, uint32_t b) { return ls[a].src_off < ls[b].src_off; });
-    st->copy_tree.assign(st->copies.size(), -1);
-    for (size_t k = 0; k < st->copies.size(); k++)
-        for (size_t t = 0; t < st->trees.size(); t++)
-            if (st->copies[k].nbytes && st->trees[t].src_off == st->copies[k].src_off) st->copy_tree[k] = (int32_t)t;
-    st->copy_tree_trees = st->trees.size();
+    index_resident(st);
 }
 
-// Convert an incremental handle to resizable lists (see LIST_SPECS).  Device work only: the lists' bytes move from the
-// stage arena to their own storage and their trees are built there.
+// Convert an incremental handle to resizable lists (see LIST_SPECS).  Each list's share of the stage-time plan (leaf
+// launches, reduce passes, tail ops and tree; st->marks) is dropped, and its staged copy moves to storage of its own,
+// where its tree is built on the device.
 static int32_t state_convert(lhb200_state* st, cudaStream_t s) {
-    using namespace state_layout;
     const ForkLayout& fl = *fork_layout(st->shard.fork);
     Plan& pl = st->plan;
-    index_resident(st);
-    uint64_t var_off[N_VAR];
-    var_off[0] = fl.state_fixed;
-    for (int k = 1; k < N_VAR; k++) var_off[k] = var_off[k - 1] + st->var_len[k - 1];
-    // 1. the stage-time copies of the lists (every variable-size field after historical_roots) and everything the
-    //    cold plan derives from them: leaf launches, reduce passes
-    std::vector<StageCopy> staged, keep;
-    staged.swap(st->copies);
-    std::vector<const uint8_t*> owned;
-    bool hist = false;
-    for (const StageCopy& cp : staged) {
-        if (cp.src_off < var_off[V_HIST] || (!hist && cp.src_off == var_off[V_HIST] && cp.nbytes == st->var_len[V_HIST])) {
-            hist |= cp.src_off >= var_off[V_HIST];
-            keep.push_back(cp);
-        } else {
-            owned.push_back(cp.dst);
-        }
-    }
-    auto is_owned = [&](const uint8_t* p) { return std::find(owned.begin(), owned.end(), p) != owned.end(); };
-    std::vector<LeafLaunch> leaves;
-    for (const LeafLaunch& L : pl.leaves) {
-        if (is_owned(L.in)) owned.push_back(L.out);
-        else leaves.push_back(L);
-    }
-    pl.leaves.swap(leaves);
-    for (auto& pass : pl.passes) {
-        std::vector<MerkleSeg> kept;
-        for (const MerkleSeg& sg : pass) {
-            if (is_owned(sg.in)) owned.push_back(sg.out);
-            else kept.push_back(sg);
-        }
-        pass.swap(kept);
+    auto cut = [](auto& v, size_t lo, size_t hi) { v.erase(v.begin() + lo, v.begin() + hi); };
+    uint64_t stage_units = 0;
+    for (int k = N_LIST_SPECS - 1; k >= 0; k--) {   // the last field first: earlier fields' marks stay valid
+        const ListSpec& sp = LIST_SPECS[k];
+        if ((int)sp.field >= fl.state_fields) continue;
+        const PlanMark &a = st->marks[sp.field], &b = st->marks[sp.field + 1];
+        cut(pl.leaves, a.leaves, b.leaves);
+        for (size_t q = 0; q < pl.passes.size(); q++) cut(pl.passes[q], a.pass(q), b.pass(q));
+        cut(pl.ops, a.ops, b.ops);
+        cut(pl.op_wave, a.ops, b.ops);
+        cut(st->trees, a.trees, b.trees);
+        stage_units += list_units(sp, st->var_len[sp.var] / sp.item_bytes);
     }
     pl.passes.erase(std::remove_if(pl.passes.begin(), pl.passes.end(), [](const std::vector<MerkleSeg>& p) { return p.empty(); }),
                     pl.passes.end());
-    // 2. the tail ops that produce the lists' field roots (small trees, zero ladders, length mix-ins)
-    std::unordered_map<uint64_t, size_t> producer;
-    for (size_t i = 0; i < pl.ops.size(); i++) producer[pl.ops[i].dst] = i;
-    std::vector<char> drop(pl.ops.size(), 0);
-    std::vector<uint64_t> todo;
-    uint64_t stage_units = 0;
-    for (const ListSpec& sp : LIST_SPECS) {
-        if ((int)sp.field >= fl.state_fields) continue;
-        todo.push_back(st->field_ops[sp.field]);
-        stage_units += list_units(sp, st->var_len[sp.var] / sp.item_bytes);
-    }
-    while (!todo.empty()) {
-        const uint64_t x = todo.back();
-        todo.pop_back();
-        const auto it = producer.find(x);
-        if (it == producer.end() || drop[it->second]) continue;
-        drop[it->second] = 1;
-        todo.push_back(pl.ops[it->second].a);
-        todo.push_back(pl.ops[it->second].b);
-    }
-    // 3. the payload header's literal chunks, and the one holding extra_data's length
-    if (fl.payload_fields) {
-        const uint64_t lo = var_off[V_LEPH], hi = lo + st->var_len[V_LEPH];
-        for (size_t k = 0; k < pl.lit_src.size(); k++) {
-            const Plan::LitSrc& ls = pl.lit_src[k];
-            if (ls.src_off < lo || ls.src_off + ls.n > hi) continue;
-            st->hdr_lits.push_back({(uint32_t)k, (uint32_t)(ls.src_off - lo)});
-            if (ls.src_off - lo == fl.header_fixed) st->hdr_extra = (int)k;
-        }
-        const uint64_t lit_base = reinterpret_cast<uint64_t>(pl.arena + pl.lit_off);
-        const uint64_t extra = st->hdr_extra < 0 ? 0 : lit_base + 32ull * pl.lit_src[st->hdr_extra].lit_index;
-        bool found = false;
-        for (const HashOp& op : pl.ops)
-            if (extra && op.a == extra) { st->hdr_len_chunk = (uint32_t)((op.b - lit_base) / 32); found = true; }
-        if (!found) { set_error("internal: payload header literals not found"); return LHB200_EINVAL; }
-    }
-    std::vector<HashOp> ops;
-    std::vector<int> waves;
-    for (size_t i = 0; i < pl.ops.size(); i++)
-        if (!drop[i]) { ops.push_back(pl.ops[i]); waves.push_back(pl.op_wave[i]); }
-    pl.ops.swap(ops);
-    pl.op_wave.swap(waves);
     {   // the pruned tail goes where the stage-time one was (it is shorter)
         const size_t nb = align_up(pl.ops.size() * sizeof(HashOp), 256);
         uint8_t* h = static_cast<uint8_t*>(pinned_scratch(nb + (pl.ops.size() + 2) * 4));
@@ -1707,40 +1652,35 @@ static int32_t state_convert(lhb200_state* st, cudaStream_t s) {
         LHB_CUDA(cudaMemcpyAsync(pl.d_waves, h + nb, pl.h_waves.size() * 4, cudaMemcpyHostToDevice, s));
     }
     st->units_base = pl.hash_units - stage_units;
-    // 4. trees: the fixed-size vectors keep theirs, every list gets a resizable one seeded from its staged bytes
-    std::vector<lhb200_state::Tree> trees;
-    for (lhb200_state::Tree& t : st->trees)
-        if (t.src_off < var_off[V_HIST]) trees.push_back(std::move(t));
-    st->trees.swap(trees);
-    st->copies.swap(keep);
+    // every list gets a resizable tree, seeded from the list's one staged copy, which then addresses its storage
     for (int k = 0; k < N_LIST_SPECS; k++) {
         const ListSpec& sp = LIST_SPECS[k];
         if ((int)sp.field >= fl.state_fields) continue;
         const uint64_t len = st->var_len[sp.var] / sp.item_bytes;
+        const bool packed = sp.leaf.tree == TREE_CHUNKS;
         lhb200_state::Tree t;
         memset(&t.dev, 0, sizeof t.dev);
-        t.dev.kind = sp.kind;
+        t.dev.kind = sp.leaf.tree;
         t.dev.n_leaves = list_leaves(sp, len);
         t.dev.top = ceil_log2(t.dev.n_leaves);
         t.dev.limit_depth = sp.depth;
         t.dev.length = len;
         t.dev.field_dst = reinterpret_cast<uint8_t*>(st->field_ops[sp.field]);
-        t.item_bytes = sp.kind == TREE_CHUNKS ? 32 : sp.item_bytes;
+        t.leaf = sp.leaf;
+        t.copy = st->marks[sp.field].copies;
+        t.item_bytes = packed ? 32 : sp.item_bytes;
         t.list = (int)st->lists.size();
+        const StageCopy staged = st->copies[t.copy];   // zero-padded past its bytes
         st->trees.push_back(std::move(t));
         lhb200_state::List L;
         L.spec = k;
         L.tree = (int)st->trees.size() - 1;
-        L.copy = st->copies.size();
         L.resized = true;
-        st->copies.push_back({0, 0, nullptr, 0});
         st->lists.push_back(L);
         int32_t rc = list_alloc(st, st->lists.back(), std::max<uint64_t>(2 * len, 16), s);
         if (rc) return rc;
-        const uint64_t nbytes = sp.kind == TREE_CHUNKS ? 32 * list_leaves(sp, len) : len * sp.item_bytes;
-        for (const StageCopy& cp : staged)   // the staged copy is zero-padded past its bytes
-            if (len && cp.src_off == var_off[sp.var] && cp.nbytes == st->var_len[sp.var])
-                LHB_CUDA(cudaMemcpyAsync(st->lists.back().d_mem, cp.dst, nbytes, cudaMemcpyDeviceToDevice, s));
+        const uint64_t nbytes = packed ? 32 * list_leaves(sp, len) : len * sp.item_bytes;
+        if (len) LHB_CUDA(cudaMemcpyAsync(st->lists.back().d_mem, staged.dst, nbytes, cudaMemcpyDeviceToDevice, s));
     }
     LHB_CUDA(cudaFree(st->d_trees));
     LHB_CUDA(cudaFree(st->d_dirty));
@@ -1769,14 +1709,14 @@ static int32_t list_set_length(lhb200_state* st, lhb200_state::List& L, uint64_t
     const ListSpec& sp = LIST_SPECS[L.spec];
     lhb200_state::Tree& t = st->trees[L.tree];
     const uint64_t old = t.dev.length, nl = list_leaves(sp, new_len), ib = sp.item_bytes;
-    if (sp.kind == TREE_CHUNKS && nl * 32 > new_len * ib)   // SSZ packing pads the last chunk with zeros
+    if (sp.leaf.tree == TREE_CHUNKS && nl * 32 > new_len * ib)   // SSZ packing pads the last chunk with zeros
         LHB_CUDA(cudaMemsetAsync(L.d_mem + new_len * ib, 0, nl * 32 - new_len * ib, s));
     auto mark = [&](uint64_t a, uint64_t b) {
         if (st->need_full || a >= b) return;
         if (t.n_marks + (b - a) > 4ull * lhb200_state::DIRTY_CAP) { st->need_full = true; return; }
         for (uint64_t q = a; q < b; q++) t.mark(q);
     };
-    if (n) mark(sp.kind == TREE_CHUNKS ? first * ib / 32 : first, list_leaves(sp, first + n));
+    if (n) mark(sp.leaf.tree == TREE_CHUNKS ? first * ib / 32 : first, list_leaves(sp, first + n));
     if (new_len < old && nl) mark(nl - 1, nl);   // the new right edge: its path re-hashes with zero siblings
     L.resized |= new_len != old;
     t.dev.n_leaves = nl;
@@ -1899,16 +1839,9 @@ int32_t lhb200_state_root_enqueue(lhb200_state* st, void* stream, const void** d
     if (!st) return LHB200_EINVAL;
     cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ctx().stream;
     if (!st->e_k0) { cudaEventCreate(&st->e_k0); cudaEventCreate(&st->e_k1); }
-    int32_t rc;
-    rc = 1;
+    int32_t rc = 1;
     if (st->incremental && !st->need_full) rc = state_incremental_enqueue(st, s);
-    if (rc > 0 && st->converted) {
-        rc = state_converted_cold(st, s);
-    } else if (rc > 0) {
-        rc = plan_enqueue(st->plan, s, st->e_k0, st->e_k1);
-        st->last_root_hashes = st->plan.hash_units;
-        if (!rc && st->incremental) rc = state_build_levels(st, s);   // a cold root leaves the level arrays stale
-    }
+    if (rc > 0) rc = state_cold_enqueue(st, s);
     if (rc) return rc;
     rc = gather_operands(st->d_gather, 1 + MAX_FIELDS, st->d_result, s);
     if (rc) return rc;

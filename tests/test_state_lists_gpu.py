@@ -311,6 +311,92 @@ def test_packed_tails(gpu):
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("fork", ["bellatrix", "capella", "deneb", "electra"])
+def test_conversion_by_payload_header(gpu, fork):
+    """The call that converts the handle replaces the payload header (extra_data changes length); list edits follow
+    on the converted handle."""
+    rng = np.random.default_rng(21)
+    model = StateModel(beacon_state_deneb_ssz(300, seed=12, fork=fork), fork)
+    st = resident(model)
+    hdr = header_bytes(rng, fork, 7)
+    st.set_payload_header(hdr)
+    model.parts["latest_execution_payload_header"][:] = hdr
+    check(st, model, warm=True)
+    apply(st, model, deposits(rng, model, 3))
+    patch(st, model, "latest_execution_payload_header", 0, rb(rng, 32))
+    check(st, model, warm=True)
+    st.release()
+
+
+@pytest.mark.gpu
+def test_conversion_before_the_first_root(gpu):
+    """A list edit straight after enable_incremental: the lists convert before any root has built the levels."""
+    from lighthouse_b200 import tree_hash as T
+    rng = np.random.default_rng(22)
+    model = StateModel(beacon_state_deneb_ssz(1001, seed=13), "deneb")
+    st = T.ResidentState(model.ssz(), "deneb")
+    st.enable_incremental()
+    apply(st, model, deposits(rng, model, 5))
+    check(st, model, warm=False)
+    patch(st, model, "balances", 8 * 3, struct.pack("<Q", 77))
+    patch(st, model, 176 + 32 * 9, 0, rb(rng, 32))                                       # block root
+    check(st, model, warm=True)
+    st.release()
+
+
+@pytest.mark.gpu
+def test_conversion_with_patches_pending(gpu):
+    """Validators and balances are patched with no root in between, then the next call converts: the lists take the
+    patched bytes along."""
+    rng = np.random.default_rng(23)
+    model = StateModel(beacon_state_deneb_ssz(20_000, seed=14, n_votes=5), "deneb")
+    st = resident(model)
+    for vi in rng.choice(20_000, size=50, replace=False):
+        patch(st, model, "validators", 121 * int(vi) + 80, struct.pack("<Q", int(rng.integers(1, 1 << 40))))
+        patch(st, model, "balances", 8 * int(vi), struct.pack("<Q", int(rng.integers(1, 1 << 40))))
+    apply(st, model, [("eth1_data_votes", 6, 5, rb(rng, 72))])
+    check(st, model, warm=True)
+    st.release()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("fork", ["deneb", "electra"])
+def test_conversion_of_a_small_state(gpu, fork):
+    """Every list has at most 8 leaves, so its stage-time field root came from small-tree ops rather than reduce
+    passes; votes, summaries and the pending lists start empty."""
+    rng = np.random.default_rng(24)
+    model = StateModel(beacon_state_deneb_ssz(6, seed=15, fork=fork, n_votes=0, n_summaries=0, n_pending=(0, 0, 0)),
+                       fork)
+    st = resident(model)
+    apply(st, model, deposits(rng, model, 2) + [("eth1_data_votes", 1, 0, rb(rng, 72))])
+    check(st, model, warm=True)
+    apply(st, model, [("historical_summaries", 1, 0, rb(rng, 64))])
+    check(st, model, warm=True)
+    st.release()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("fork", ["capella", "electra"])
+def test_patches_where_an_emptied_list_ends(gpu, fork):
+    """Lists emptied by an epoch end where the next field starts: patches there still find the next field's bytes."""
+    rng = np.random.default_rng(25)
+    model = StateModel(beacon_state_deneb_ssz(37, seed=16, fork=fork, n_votes=5, n_summaries=3), fork)
+    st = resident(model)
+    empty = [("eth1_data_votes", 0, 0, b"")]
+    if fork == "electra":
+        empty += [(n, 0, 0, b"") for n in ("pending_balance_deposits", "pending_partial_withdrawals",
+                                           "pending_consolidations")]
+    apply(st, model, empty)
+    apply(st, model, deposits(rng, model, 70_000))
+    for name in ("validators", "balances"):
+        n = model.length(name)
+        for i in (0, n // 2, n - 3):
+            patch(st, model, name, model.item_bytes(name) * i, rb(rng, 8))
+    check(st, model, warm=False, fresh=False)
+    st.release()
+
+
+@pytest.mark.gpu
 def test_refusals_leave_the_handle_unchanged(gpu):
     from lighthouse_b200 import Lhb200Error, _ffi, tree_hash as T
     rng = np.random.default_rng(13)
