@@ -163,6 +163,20 @@ LHB200_API int32_t lhb200_state_combine(lhb200_state* st, const uint8_t* gathere
  * ncclAllGather, every rank folds the top; only the 32-byte root crosses the host link. */
 LHB200_API int32_t lhb200_state_root_sharded(lhb200_state* st, uint8_t out[32]);
 LHB200_API int32_t lhb200_state_release(lhb200_state* st);
+/* BeaconState::clone of a resident, unsharded handle: a new handle with the same fork, encoding, list lengths and
+ * capacities, payload header, incremental / converted status and pending (not yet rooted) mutations, whose device
+ * memory is its own.  Afterwards the two are independent: edits, roots and release of one never affect the other.
+ * Blocks until the clone is ready; work enqueued on `src` through lhb200_state_root_enqueue on another stream must be
+ * complete.  The live bytes are copied by one kernel launch.  Sharded handle -> LHB200_EINVAL; on failure *out is
+ * untouched and src unchanged. */
+LHB200_API int32_t lhb200_state_clone(const lhb200_state* src, lhb200_state** out);
+/* HBM held by the handle (arena, levels, tree and dirty tables, resizable-list storage), for cache sizing. */
+LHB200_API int32_t lhb200_state_device_bytes(const lhb200_state* st, uint64_t* bytes);
+/* Test hook: *disjoint = 1 iff no device address held by `a` lies in an allocation of `b`. */
+LHB200_API int32_t lhb200_debug_state_disjoint(const lhb200_state* a, const lhb200_state* b, int32_t* disjoint);
+/* Test hook: the live bytes lhb200_state_clone copies for this handle (its arena up to the allocation cursor, its
+ * levels, and each resizable list up to its length). */
+LHB200_API int32_t lhb200_debug_state_live_bytes(const lhb200_state* st, uint64_t* bytes);
 /* Algorithmic work of the last root computed on this handle: number of hash32_concat units. */
 LHB200_API uint64_t lhb200_state_hash_units(const lhb200_state* st);
 /* Device time (ms) of the dominant kernel (k_validator_roots) in the last completed root, from CUDA events on the

@@ -466,6 +466,33 @@ __global__ void __launch_bounds__(256) k_scatter_bytes(const ScatterOp* __restri
     for (uint32_t i = lane; i < op.len; i += 32) op.dst[i] = blob[op.blob_off + i];
 }
 
+// Device-to-device copy of many ranges in one launch (lhb200_state_clone).  Every range is a whole number of 16-byte
+// words at 16-byte aligned addresses; word[k] = 16-byte words of ranges [0, k), word[n] = the total.  Grid-stride over
+// the total: each thread finds the range of its first word by binary search over `word` and walks forward from there,
+// since its later words only lie in the same or later ranges.
+struct CopyRange {
+    uint8_t* dst;
+    const uint8_t* src;
+    uint64_t bytes;   // multiple of 16
+};
+__global__ void __launch_bounds__(256) k_copy_ranges(const CopyRange* __restrict__ ranges,
+                                                     const uint64_t* __restrict__ word, uint32_t n) {
+    const uint64_t total = word[n], stride = (uint64_t)gridDim.x * blockDim.x;
+    uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (w >= total) return;
+    uint32_t lo = 0, hi = n;   // word[lo] <= w < word[hi]
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) / 2;
+        if (word[mid] <= w) lo = mid; else hi = mid;
+    }
+    for (; w < total; w += stride) {
+        while (word[lo + 1] <= w) lo++;
+        const uint64_t o = (w - word[lo]) * 16;
+        const uint4 v = __ldg(reinterpret_cast<const uint4*>(ranges[lo].src + o));
+        *reinterpret_cast<uint4*>(ranges[lo].dst + o) = v;
+    }
+}
+
 // ---------------------------------------------------------------------------------------------
 // Byte items: hash_tree_root of packed byte strings that sit at ARBITRARY byte offsets inside an SSZ blob
 // (transactions, signatures, pubkeys, bitlists, index lists, proofs ... of a BeaconBlock):

@@ -7,6 +7,7 @@
 #include <algorithm>
 #include <array>
 #include <memory>
+#include <type_traits>
 #include <vector>
 #include "ctx.h"
 #include "merkle.cuh"
@@ -632,7 +633,8 @@ struct lhb200_state {
     bool incremental = false, need_full = false;
     std::vector<Tree> trees;
     uint8_t* d_levels = nullptr;
-    lhb200::TreeDev* d_trees = nullptr;
+    size_t levels_bytes = 0;
+    lhb200::TreeDev* d_trees = nullptr;   // trees_bytes() / dirty_bytes(), sized for `trees`
     uint32_t* d_dirty = nullptr;
     uint64_t last_root_hashes = 0;       // hash32_concat units of the last root (full or incremental)
     static constexpr uint32_t DIRTY_CAP = 1u << 16;
@@ -654,6 +656,10 @@ struct lhb200_state {
     std::vector<std::pair<uint32_t, uint32_t>> hdr_lits;   // payload header literals: (lit_src index, offset in header)
     int hdr_extra = -1;                  // lit_src index of extra_data
     uint32_t hdr_len_chunk = 0;          // literal chunk holding extra_data's length
+
+    size_t trees_bytes() const { return trees.size() * sizeof(lhb200::TreeDev) + 256; }
+    size_t dirty_bytes() const { return (size_t)DIRTY_CAP * 4 * trees.size(); }
+    size_t coll_bytes() const { return (size_t)(shard.world + 1) * sharded.size() * 32 + 512; }
 };
 
 namespace lhb200 {
@@ -1237,7 +1243,7 @@ int32_t lhb200_state_root_sharded(lhb200_state* st, uint8_t out[32]) {
     if (rc) return rc;
     if (n == 0) { set_error("handle is not sharded"); return LHB200_EINVAL; }
     if (!st->d_coll) {   // owned by the handle: dev_scratch is reused by the combine
-        LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_coll), (size_t)(world + 1) * n * 32 + 512));
+        LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_coll), st->coll_bytes()));
     }
     uint8_t* d_mine = st->d_coll;
     uint8_t* d_all = d_mine + align_up(n * 32, 256);
@@ -1496,6 +1502,7 @@ int32_t lhb200_state_enable_incremental(lhb200_state* st) {
     for (const Plan::TreeSpec& ts : st->plan.trees)
         for (uint64_t n = ceil_div(ts.n_chunks, 2);; n = ceil_div(n, 2)) { bytes += align_up(n * 32, 256); if (n == 1) break; }
     LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_levels), bytes + 256));
+    st->levels_bytes = bytes + 256;
     size_t off = 0;
     for (const Plan::TreeSpec& ts : st->plan.trees) {
         lhb200_state::Tree t;
@@ -1516,8 +1523,8 @@ int32_t lhb200_state_enable_incremental(lhb200_state* st) {
         t.dirty_bits.assign((ts.n_chunks + 63) / 64, 0ull);
         st->trees.push_back(t);
     }
-    LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_trees), st->trees.size() * sizeof(TreeDev) + 256));
-    LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_dirty), (size_t)lhb200_state::DIRTY_CAP * 4 * st->trees.size()));
+    LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_trees), st->trees_bytes()));
+    LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_dirty), st->dirty_bytes()));
     index_resident(st);
     st->incremental = true;
     st->need_full = true;   // the first root after enabling is cold and builds the levels
@@ -1686,8 +1693,14 @@ static int32_t state_convert(lhb200_state* st, cudaStream_t s) {
     LHB_CUDA(cudaFree(st->d_dirty));
     st->d_trees = nullptr;
     st->d_dirty = nullptr;
-    LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_trees), st->trees.size() * sizeof(TreeDev) + 256));
-    LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_dirty), (size_t)lhb200_state::DIRTY_CAP * 4 * st->trees.size()));
+    LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_trees), st->trees_bytes()));
+    LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&st->d_dirty), st->dirty_bytes()));
+    // a tree's dirty pointer only means something between the upload of the tree table and the kernels that read it;
+    // the old table is gone, so no tree keeps pointing into it (lhb200_state_clone relocates every address it finds)
+    for (lhb200_state::Tree& t : st->trees) {
+        t.dev.dirty = nullptr;
+        t.dev.n_dirty = 0;
+    }
     lists_enqueue_leaves(st, s, nullptr, nullptr);
     for (const lhb200_state::List& L : st->lists) tree_build_levels(st->trees[L.tree], s);
     LHB_CUDA(cudaGetLastError());
@@ -1887,6 +1900,209 @@ int32_t lhb200_state_release(lhb200_state* st) {
 }
 
 uint64_t lhb200_state_hash_units(const lhb200_state* st) { return st ? st->plan.hash_units : 0; }
+
+// ---------------------------------------------------------------------------------------------------------
+// Branches (lhb200_state_clone).  A handle holds absolute device addresses in its plan, its tables and its trees; a
+// clone copies the live bytes of every allocation into allocations of its own and rewrites each address through a map
+// from the source's allocations to the clone's.
+}  // extern "C"
+namespace lhb200 {
+// Every device address a handle holds, as f(address, bytes): bytes > 0 for the base of an allocation the handle owns
+// (the arena first), 0 for an address into one.  Null addresses and zero-hash operands (OP_ZERO_FLAG) are passed too.
+// f may rewrite the address.  The clone and lhb200_debug_state_disjoint both walk a handle through this one function.
+template <class F>
+static void visit_device_addresses(lhb200_state* st, F&& f) {
+    auto at = [&](auto*& p, size_t bytes = 0) {
+        uint64_t a = reinterpret_cast<uint64_t>(p);
+        f(a, bytes);
+        p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(a);
+    };
+    at(st->arena, st->arena_bytes);
+    if (st->d_levels) at(st->d_levels, st->levels_bytes);
+    if (st->d_trees) at(st->d_trees, st->trees_bytes());
+    if (st->d_dirty) at(st->d_dirty, st->dirty_bytes());
+    if (st->d_coll) at(st->d_coll, st->coll_bytes());
+    for (lhb200_state::List& L : st->lists) {
+        TreeDev d;
+        at(L.d_mem, list_place(d, LIST_SPECS[L.spec], 0, L.cap));
+    }
+    Plan& pl = st->plan;
+    at(pl.arena);
+    for (LeafLaunch& L : pl.leaves) { at(L.in); at(L.out); }
+    for (auto& pass : pl.passes)
+        for (MerkleSeg& sg : pass) { at(sg.in); at(sg.out); }
+    for (HashOp& op : pl.ops) { f(op.dst, 0); f(op.a, 0); f(op.b, 0); }
+    for (ByteItem& it : pl.items) { at(it.src); at(it.out); }
+    for (Plan::TreeSpec& ts : pl.trees) { at(ts.chunks); f(ts.top_addr, 0); at(ts.src); }
+    at(pl.d_ops); at(pl.d_waves); at(pl.d_items);
+    for (StageCopy& cp : st->copies) at(cp.dst);
+    for (uint64_t& op : st->field_ops) f(op, 0);
+    f(st->root_op, 0);
+    at(st->d_gather); at(st->d_result);
+    for (ShardedList& L : st->sharded) f(L.local_op, 0);
+    for (lhb200_state::Tree& t : st->trees) {
+        at(t.dev.src);
+        for (uint8_t*& l : t.dev.lvl) at(l);
+        at(t.dev.top_dst); at(t.dev.dirty); at(t.dev.field_dst);
+    }
+}
+static bool is_device_address(uint64_t a) { return a && !(a & OP_ZERO_FLAG); }
+
+// An allocation of a source handle and where the clone's copy of it starts.
+struct Relocation {
+    uint64_t from, bytes, to;
+};
+// Sorted by `from`: the address a moves to, or 0 if it lies in no allocation.
+static uint64_t relocate(const std::vector<Relocation>& map, uint64_t a) {
+    auto r = std::upper_bound(map.begin(), map.end(), a, [](uint64_t x, const Relocation& m) { return x < m.from; });
+    if (r == map.begin()) return 0;
+    --r;
+    return a - r->from < r->bytes ? a - r->from + r->to : 0;
+}
+// The bytes of a handle that a clone copies, as g(address, bytes), each range rounded up to 16 inside its allocation:
+// the arena up to its allocation cursor, the levels, and per resizable list its items, leaf chunks and each level up
+// to the current length (list_alloc relies on the same: nothing past the length is read before it is written).
+template <class G>
+static void visit_live_ranges(const lhb200_state* st, G&& g) {
+    auto live = [&](const void* p, uint64_t bytes) {
+        if (bytes) g(static_cast<const uint8_t*>(p), align_up(bytes, 16));
+    };
+    live(st->arena, st->plan.bump);
+    live(st->d_levels, st->levels_bytes);
+    for (const lhb200_state::List& L : st->lists) {
+        const TreeDev& d = st->trees[L.tree].dev;
+        if (d.kind != TREE_CHUNKS) live(d.src, d.length * LIST_SPECS[L.spec].item_bytes);
+        uint64_t n = d.n_leaves;
+        live(d.lvl[0], n * 32);
+        for (uint32_t l = 1; l <= d.top; l++) live(d.lvl[l], (n = ceil_div(n, 2)) * 32);
+    }
+}
+}  // namespace lhb200
+extern "C" {
+
+int32_t lhb200_state_device_bytes(const lhb200_state* st, uint64_t* bytes) {
+    LHB_REQUIRE_READY();
+    if (!st || !bytes) return LHB200_EINVAL;
+    std::lock_guard<std::recursive_mutex> g(ctx().mu);
+    uint64_t sum = 0;
+    visit_device_addresses(const_cast<lhb200_state*>(st), [&](uint64_t&, size_t n) { sum += n; });
+    *bytes = sum;
+    return LHB200_OK;
+}
+
+int32_t lhb200_debug_state_live_bytes(const lhb200_state* st, uint64_t* bytes) {
+    LHB_REQUIRE_READY();
+    if (!st || !bytes) return LHB200_EINVAL;
+    std::lock_guard<std::recursive_mutex> g(ctx().mu);
+    uint64_t sum = 0;
+    visit_live_ranges(st, [&](const uint8_t*, uint64_t n) { sum += n; });
+    *bytes = sum;
+    return LHB200_OK;
+}
+
+int32_t lhb200_debug_state_disjoint(const lhb200_state* a, const lhb200_state* b, int32_t* disjoint) {
+    LHB_REQUIRE_READY();
+    if (!a || !b || !disjoint) return LHB200_EINVAL;
+    std::lock_guard<std::recursive_mutex> g(ctx().mu);
+    std::vector<Relocation> allocs;   // b's allocations (`to` unused)
+    visit_device_addresses(const_cast<lhb200_state*>(b), [&](uint64_t& p, size_t n) {
+        if (n && p) allocs.push_back({p, n, p});
+    });
+    std::sort(allocs.begin(), allocs.end(), [](const Relocation& x, const Relocation& y) { return x.from < y.from; });
+    bool hit = false;
+    visit_device_addresses(const_cast<lhb200_state*>(a), [&](uint64_t& p, size_t) {
+        hit |= is_device_address(p) && relocate(allocs, p) != 0;
+    });
+    *disjoint = hit ? 0 : 1;
+    return LHB200_OK;
+}
+
+int32_t lhb200_state_clone(const lhb200_state* src, lhb200_state** out) {
+    LHB_REQUIRE_READY();
+    if (!src || !out) return LHB200_EINVAL;
+    if (src->shard.world != 1) { set_error("state_clone: a sharded handle cannot be cloned"); return LHB200_EINVAL; }
+    Ctx& c = ctx();
+    std::lock_guard<std::recursive_mutex> g(c.mu);
+    // The host state as it is (plan, literals, dirty bitmaps, lengths, patch lookups).  Before anything can fail, the
+    // copy forgets the source's allocations and events, so that releasing a failed clone frees only its own.
+    std::unique_ptr<lhb200_state, int32_t (*)(lhb200_state*)> st(new lhb200_state(*src), lhb200_state_release);
+    st->e_k0 = st->e_k1 = nullptr;
+    // Allocations of the same sizes as the source's; the arena may be the spare one a released handle left behind.
+    std::vector<Relocation> map;
+    int32_t rc = LHB200_OK;
+    visit_device_addresses(st.get(), [&](uint64_t& p, size_t n) {
+        if (!n || !p) return;
+        const uint64_t from = p;
+        p = 0;
+        if (rc) return;
+        void* mem = nullptr;
+        if (map.empty() && g_spare_arena && g_spare_bytes >= n) {
+            mem = g_spare_arena;
+            st->arena_bytes = g_spare_bytes;
+            g_spare_arena = nullptr;
+            g_spare_bytes = 0;
+        } else {
+            const cudaError_t e = cudaMalloc(&mem, n);
+            if (e != cudaSuccess) { rc = cuda_fail(e, "cudaMalloc(state_clone)"); return; }
+        }
+        p = reinterpret_cast<uint64_t>(mem);
+        map.push_back({from, n, p});
+    });
+    if (rc) return rc;
+    std::sort(map.begin(), map.end(), [](const Relocation& x, const Relocation& y) { return x.from < y.from; });
+    std::vector<CopyRange> ranges;
+    visit_live_ranges(src, [&](const uint8_t* p, uint64_t bytes) {
+        ranges.push_back({reinterpret_cast<uint8_t*>(relocate(map, reinterpret_cast<uint64_t>(p))), p, bytes});
+    });
+    // Every address the clone holds moves into its own allocations; one that lies in none is refused rather than
+    // left pointing into the source.
+    bool missed = false;
+    visit_device_addresses(st.get(), [&](uint64_t& p, size_t n) {
+        if (n || !is_device_address(p)) return;
+        const uint64_t q = relocate(map, p);
+        missed |= q == 0;
+        p = q;
+    });
+    for (const CopyRange& r : ranges) missed |= r.dst == nullptr;
+    if (missed) { set_error("internal: state_clone found a device address outside the source's allocations"); return LHB200_EINVAL; }
+    // The tables that hold addresses are uploaded again from the relocated host copies: the tail program, the byte
+    // items and the gather table.  The tree and dirty tables need nothing: every root uploads them.
+    Plan& pl = st->plan;
+    std::vector<uint64_t> gather(1, st->root_op);
+    gather.insert(gather.end(), st->field_ops, st->field_ops + MAX_FIELDS);
+    const size_t n_ranges = ranges.size();
+    const size_t rb = align_up(n_ranges * sizeof(CopyRange), 256), wb = align_up((n_ranges + 1) * 8, 256);
+    const size_t ob = align_up(pl.ops.size() * sizeof(HashOp), 256), ib = align_up(pl.items.size() * sizeof(ByteItem), 256);
+    uint8_t* h = static_cast<uint8_t*>(pinned_scratch(rb + wb + ob + ib + gather.size() * sizeof(HashOp)));
+    uint8_t* d = static_cast<uint8_t*>(dev_scratch(rb + wb));
+    if (!h || !d) return LHB200_ENOMEM;
+    memcpy(h, ranges.data(), n_ranges * sizeof(CopyRange));
+    uint64_t* word = reinterpret_cast<uint64_t*>(h + rb);
+    word[0] = 0;
+    for (size_t i = 0; i < n_ranges; i++) word[i + 1] = word[i] + ranges[i].bytes / 16;
+    LHB_CUDA(cudaMemcpyAsync(d, h, rb + (n_ranges + 1) * 8, cudaMemcpyHostToDevice, c.stream));
+    int n_sm = 0;
+    LHB_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, c.device));
+    const unsigned grid = (unsigned)std::min<uint64_t>(ceil_div(word[n_ranges], 256), 8ull * n_sm);
+    k_copy_ranges<<<grid, 256, 0, c.stream>>>(reinterpret_cast<const CopyRange*>(d), reinterpret_cast<const uint64_t*>(d + rb),
+                                             (uint32_t)n_ranges);
+    count_launch();
+    LHB_CUDA(cudaGetLastError());
+    if (!pl.ops.empty()) {
+        plan_sort_ops(pl, reinterpret_cast<HashOp*>(h + rb + wb));
+        LHB_CUDA(cudaMemcpyAsync(pl.d_ops, h + rb + wb, pl.ops.size() * sizeof(HashOp), cudaMemcpyHostToDevice, c.stream));
+    }
+    if (!pl.items.empty()) {
+        memcpy(h + rb + wb + ob, pl.items.data(), pl.items.size() * sizeof(ByteItem));
+        LHB_CUDA(cudaMemcpyAsync(pl.d_items, h + rb + wb + ob, pl.items.size() * sizeof(ByteItem), cudaMemcpyHostToDevice,
+                                 c.stream));
+    }
+    rc = stage_operands(gather, st->d_gather, h + rb + wb + ob + ib, c.stream);
+    if (rc) return rc;
+    LHB_CUDA(cudaStreamSynchronize(c.stream));   // the staging slabs are reused by the next call
+    *out = st.release();
+    return LHB200_OK;
+}
 
 float lhb200_state_dominant_kernel_ms(const lhb200_state* st) {
     float ms = -1.f;

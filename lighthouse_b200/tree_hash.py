@@ -293,6 +293,22 @@ class ResidentState:
         p, keep = buf(ssz)
         check(lib.lhb200_state_set_payload_header(self._h, p, len(ssz)), "lhb200_state_set_payload_header")
 
+    def clone(self):
+        """BeaconState::clone on the device (lhb200_state_clone): a new handle of the same fork whose device memory is
+        its own, with this one's pending mutations; edits, roots and release of either never affect the other."""
+        new = ResidentState.__new__(ResidentState)
+        new._h = C.c_void_p()
+        new.fork = self.fork
+        check(lib.lhb200_state_clone(self._h, C.byref(new._h)), "lhb200_state_clone")
+        return new
+
+    @property
+    def device_bytes(self):
+        """HBM the handle holds (lhb200_state_device_bytes)."""
+        n = C.c_uint64(0)
+        check(lib.lhb200_state_device_bytes(self._h, C.byref(n)), "lhb200_state_device_bytes")
+        return n.value
+
     @property
     def last_root_hashes(self):
         """hash32_concat units the last root() actually computed (cold: all of them; warm: dirty paths + tail)."""
