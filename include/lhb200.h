@@ -191,6 +191,26 @@ LHB200_API int32_t lhb200_merkle_tree_proof(const uint8_t* leaves, uint64_t n, u
  * ok[i] = (fold(leaf_i, branch_i, depth, index_i) == root_i).  branches: n * depth * 32 bytes. */
 LHB200_API int32_t lhb200_verify_merkle_proofs(const uint8_t* leaves, const uint8_t* branches, uint32_t depth,
                                     const uint64_t* indices, const uint8_t* roots, uint64_t n, uint8_t* ok);
+/* Branches of generalized indices of a resident BeaconState (spec compute_merkle_proof, consensus-specs
+ * ssz/merkle-proofs.md; beacon_state.rs:2483).  Roots the handle first, warm or cold exactly as lhb200_state_root
+ * would, consuming pending mutations the same way.  Proof i has depth_i = floor(log2(gindices[i])) siblings, bottom-up
+ * (the leaf's sibling first), at branches + 32 * sum_{j<i} depth_j.  root: the state root every branch verifies
+ * against.  Unsharded handles of every fork, incremental or not, converted or not.  LHB200_EINVAL, with the handle
+ * left as it was: gindex 0, a gindex below a leaf (a u64 field, a packed chunk, a validator, record or byte-string
+ * root), a sharded handle.  One gather launch per call, plus one k_tree_level launch per level the call rebuilds for a
+ * list without resident levels. */
+LHB200_API int32_t lhb200_state_proofs(lhb200_state* st, const uint64_t* gindices, uint32_t n, uint8_t* branches,
+                                       uint8_t root[32]);
+/* Same for the BeaconBlockBody of n_blocks blocks (SSZ and layout of lhb200_beacon_block_roots): gindices relative to
+ * the BODY root, proof i taken in block block_of[i]; body_roots n_blocks x 32.  block_of[i] >= n_blocks, malformed
+ * SSZ or a gindex below a leaf (a transaction, a signature, a commitment root) -> LHB200_EINVAL. */
+LHB200_API int32_t lhb200_beacon_block_body_proofs(const uint8_t* ssz, const uint64_t* offsets, uint32_t n_blocks,
+                                                   int32_t fork, int32_t blinded, const uint32_t* block_of,
+                                                   const uint64_t* gindices, uint32_t n, uint8_t* branches,
+                                                   uint8_t* body_roots);
+/* Benchmark hook: device time (ms) of the last k_proof_branches launch of either call above, from CUDA events recorded
+ * around it; < 0 if unavailable. */
+LHB200_API float lhb200_debug_proof_gather_ms(void);
 
 /* BeaconBlock::canonical_root for BeaconBlockDeneb SSZ bytes, mainnet preset (consensus/types/src/beacon_block.rs:
  * 56-78,158-160; body beacon_block_body.rs:70-121,145-176; payload execution_payload.rs:54-95; operations

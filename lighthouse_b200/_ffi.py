@@ -147,6 +147,9 @@ _sig("lhb200_state_clone", C.c_int32, vp, C.POINTER(vp))
 _sig("lhb200_state_device_bytes", C.c_int32, vp, C.POINTER(C.c_uint64))
 _sig("lhb200_debug_state_disjoint", C.c_int32, vp, vp, C.POINTER(C.c_int32))
 _sig("lhb200_debug_state_live_bytes", C.c_int32, vp, C.POINTER(C.c_uint64))
+_sig("lhb200_state_proofs", C.c_int32, vp, vp, C.c_uint32, vp, vp)
+_sig("lhb200_beacon_block_body_proofs", C.c_int32, vp, vp, C.c_uint32, C.c_int32, C.c_int32, vp, vp, C.c_uint32, vp, vp)
+_sig("lhb200_debug_proof_gather_ms", C.c_float)
 
 
 class ListEdit(C.Structure):

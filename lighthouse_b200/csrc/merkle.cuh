@@ -493,6 +493,64 @@ __global__ void __launch_bounds__(256) k_copy_ranges(const CopyRange* __restrict
     }
 }
 
+// Merkle branches by generalized index (lhb200_state_proofs, lhb200_beacon_block_body_proofs).  The host resolves each
+// proof down to the tree it enters (or to its end) and lists the siblings above that point once per distinct path
+// prefix, as ProofSrc entries.  One thread per output sibling: it finds its proof by binary search over the prefix
+// sums of the branch depths (first[k] = siblings of proofs [0, k)), reads the sibling and stores it with uint4 writes, so
+// consecutive threads write consecutive 32-byte entries of one branch.  A sibling that is a plain device address is
+// copied with uint4 loads: like every hash-program operand (load_operand) it must be 16-byte aligned, and so must a new
+// kind of operand source (level arrays, node pool, literals, leaf and item outputs all are).
+struct ProofTree {            // levels of one tree: lvl[l] holds ceil(n_leaves / 2^l) nodes, the rest are zero nodes
+    const uint8_t* lvl[41];
+    uint64_t n_leaves;
+};
+struct ProofSrc {             // operand `op` (a device address or OP_ZERO_FLAG | level), hashed with ZERO_HASHES[l] for
+    uint64_t op;              // l in [from, to): the left spine node of a list above its current top
+    uint32_t from, to;
+};
+struct ProofDesc {
+    uint64_t node;            // index of the proven node at level `level` of tree `tree`
+    uint32_t tree, level;
+    uint32_t n_tree;          // siblings 0 .. n_tree-1 (bottom-up) lie in the tree, the rest are srcs[src ..]
+    uint32_t src;
+};
+__global__ void __launch_bounds__(256) k_proof_branches(const ProofDesc* __restrict__ proofs,
+                                                        const uint64_t* __restrict__ first, uint32_t n,
+                                                        const ProofTree* __restrict__ trees,
+                                                        const ProofSrc* __restrict__ srcs, uint8_t* __restrict__ out) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= first[n]) return;
+    uint32_t lo = 0, hi = n;   // first[lo] <= t < first[hi]
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) / 2;
+        if (first[mid] <= t) lo = mid; else hi = mid;
+    }
+    const ProofDesc p = proofs[lo];
+    const uint32_t j = (uint32_t)(t - first[lo]);
+    uint64_t op;
+    uint32_t from = 0, to = 0;
+    if (j < p.n_tree) {
+        const ProofTree& tr = trees[p.tree];
+        const uint32_t l = p.level + j;
+        const uint64_t idx = (p.node >> j) ^ 1, cnt = (tr.n_leaves + ((1ull << l) - 1)) >> l;
+        op = idx < cnt ? reinterpret_cast<uint64_t>(tr.lvl[l] + 32 * idx) : (OP_ZERO_FLAG | l);
+    } else {
+        const ProofSrc s = srcs[p.src + (j - p.n_tree)];
+        op = s.op; from = s.from; to = s.to;
+    }
+    uint4* dst = reinterpret_cast<uint4*>(out + 32 * t);
+    if (!(op & OP_ZERO_FLAG) && from == to) {
+        const uint4* s = reinterpret_cast<const uint4*>(op);
+        dst[0] = s[0];
+        dst[1] = s[1];
+        return;
+    }
+    uint32_t w[8];
+    load_operand(op, w);
+    for (uint32_t l = from; l < to; l++) hash_pair(w, g_zero_words[l], w);
+    store_chunk(out + 32 * t, w);
+}
+
 // ---------------------------------------------------------------------------------------------
 // Byte items: hash_tree_root of packed byte strings that sit at ARBITRARY byte offsets inside an SSZ blob
 // (transactions, signatures, pubkeys, bitlists, index lists, proofs ... of a BeaconBlock):

@@ -8,6 +8,7 @@
 #include <array>
 #include <memory>
 #include <type_traits>
+#include <unordered_map>
 #include <vector>
 #include "ctx.h"
 #include "merkle.cuh"
@@ -94,6 +95,10 @@ struct Plan {
     struct TreeSpec { const uint8_t* chunks; uint64_t n_chunks; uint64_t top_addr; const uint8_t* src; LeafKind leaf;
                       size_t copy; uint32_t item_bytes; };
     std::vector<TreeSpec> trees;
+    // every merkle_list folded by reduce passes: its leaf chunks and the address of its data root at level
+    // ceil_log2(n), where a Merkle proof that enters the list rebuilds its levels (lhb200_state_proofs)
+    struct ListRec { const uint8_t* chunks; uint64_t n; uint64_t top_addr; };
+    std::vector<ListRec> merkle_lists;
     uint64_t hash_units = 0;
     // SSZ provenance of literal chunks (for lhb200_state_patch): chunk index <- n bytes at SSZ offset src_off
     struct LitSrc { uint32_t lit_index; uint32_t n; uint64_t src_off; };
@@ -221,6 +226,7 @@ struct Plan {
             in = out;
         }
         uint64_t r = reinterpret_cast<uint64_t>(in);
+        merkle_lists.push_back({d_in, hash_units_n0, r});
         if (warm) trees.push_back({d_in, hash_units_n0, r, warm->src, warm->leaf, warm->copy, warm->item_bytes});
         for (uint32_t l = level; l < depth; l++) r = op_hash(r, zero_op(l));
         return r;
@@ -573,7 +579,7 @@ struct StageCopy {
 // Sizes of a staged state's plan and copies when the describer starts a field: field k emitted everything from
 // marks[k] up to marks[k + 1], which is how a conversion to resizable lists drops the lists' share of the plan.
 struct PlanMark {
-    size_t ops, leaves, copies, trees;
+    size_t ops, leaves, copies, trees, merkle_lists;
     std::vector<size_t> passes;   // segments of each reduce pass
     size_t pass(size_t q) const { return q < passes.size() ? passes[q] : 0; }
 };
@@ -594,7 +600,8 @@ struct ShardedList {
 
 static uint8_t* g_spare_arena = nullptr;  // guarded by ctx().mu
 static size_t g_spare_bytes = 0;
-// lhb200_shutdown: the recycled arena belongs to the context that is going away
+static cudaEvent_t g_proof_ev[2] = {nullptr, nullptr};   // around the last k_proof_branches launch
+// lhb200_shutdown: the recycled arena and the events belong to the context that is going away
 namespace lhb200 {
 void merkle_shutdown();
 }
@@ -602,6 +609,10 @@ void lhb200::merkle_shutdown() {
     if (g_spare_arena) cudaFree(g_spare_arena);
     g_spare_arena = nullptr;
     g_spare_bytes = 0;
+    for (cudaEvent_t& e : g_proof_ev) {
+        if (e) cudaEventDestroy(e);
+        e = nullptr;
+    }
 }
 
 struct lhb200_state {
@@ -835,7 +846,7 @@ static int32_t describe_state(Plan& p, const uint8_t* s, uint64_t len, lhb200_st
         return p.merkle_list(src, nbytes / 32, depth, &warm);
     };
     auto mark = [&] {
-        PlanMark m{p.ops.size(), p.leaves.size(), st->copies.size(), p.trees.size(), {}};
+        PlanMark m{p.ops.size(), p.leaves.size(), st->copies.size(), p.trees.size(), p.merkle_lists.size(), {}};
         for (const auto& pass : p.passes) m.passes.push_back(pass.size());
         st->marks.push_back(std::move(m));
     };
@@ -967,6 +978,267 @@ static void index_resident(lhb200_state* st) {
     st->copy_tree.assign(st->copies.size(), -1);
     for (size_t t = 0; t < st->trees.size(); t++) st->copy_tree[st->trees[t].copy] = (int32_t)t;
 }
+
+// ---------------------------------------------------------------------------------------------------------
+// Merkle proofs by generalized index (consensus-specs ssz/merkle-proofs.md; BeaconState::compute_merkle_proof,
+// beacon_state.rs:2483-2557; BeaconBlockBody::kzg_commitment_merkle_proof, beacon_block_body.rs:178-227).  A gindex g
+// names the node at depth floor(log2 g) below a root; its branch lists the siblings along the path, bottom-up.  The
+// host walks g's bits from the root through what the describer emitted:
+//   - an op output: bit 0 goes to operand a, bit 1 to operand b, the other operand is the sibling;
+//   - a zero operand: the rest of the path lies in a zero subtree, whose siblings are zero hashes;
+//   - the top of a resident tree (an incremental handle's big lists) or of a merkle_list folded by reduce passes, whose
+//     levels are rebuilt into per-call scratch: the rest of the path is a leaf index into the tree's levels;
+//   - the field root of a converted resizable list, which k_list_finish writes with no op behind it: its length chunk
+//     and its ladder above the current top are synthesised, the left spine node a right turn above the top needs is
+//     hashed by k_proof_branches from the top node;
+//   - anything else is a leaf (a literal, a validator, record or byte-item root): a further bit is refused.
+// The siblings above the point where a path enters a tree are listed once per such entry node (of one root), and
+// later proofs that enter the same node below the same root (100 000 validator proofs) reuse them: per proof the host
+// then only computes a leaf index.
+constexpr uint64_t PROOF_IMM = 1ull << 62;   // ProofSrc::op until upload: index of an immediate chunk (a list length)
+
+struct ProofResolver {
+    const Plan& pl;
+    std::vector<std::pair<uint64_t, const TreeDev*>> resident;    // top node address -> tree with resident levels
+    std::vector<std::pair<uint64_t, const TreeDev*>> converted;   // field root address -> converted resizable list
+    // output: proofs, first[k] = siblings of proofs [0, k), sibling sources above the trees, immediate chunks, and the
+    // trees the proofs enter (resident levels, or a merkle_list whose levels this call rebuilds)
+    std::vector<ProofDesc> desc;
+    std::vector<uint64_t> first{0};
+    std::vector<ProofSrc> srcs;
+    std::vector<std::array<uint8_t, 32>> imm;
+    struct TreeUse { const TreeDev* dev; const Plan::ListRec* rec; };
+    std::vector<TreeUse> trees;
+
+    static constexpr uint32_t NONE = ~0u;
+    std::vector<uint32_t> pool_op, forced_op;   // node-pool slot / forced destination -> the op writing it
+    struct Entry { uint32_t tree, top, src; };  // a tree entry node: its tree and the siblings above it
+    // by (the root the walk started from, the entry node's gindex below it): the blocks of a batch share gindices but
+    // not trees or siblings
+    struct MemoKey {
+        uint64_t root, g;
+        bool operator==(const MemoKey& o) const { return root == o.root && g == o.g; }
+    };
+    struct MemoHash {
+        size_t operator()(const MemoKey& k) const { return std::hash<uint64_t>()(k.g ^ (k.root * 0x9e3779b97f4a7c15ull)); }
+    };
+    std::unordered_map<MemoKey, Entry, MemoHash> memo;
+    std::vector<uint32_t> memo_depths;
+
+    explicit ProofResolver(const Plan& p) : pl(p) {
+        pool_op.assign(p.node_used, NONE);
+        forced_op.assign(p.forced_wave.size(), NONE);
+        for (size_t i = 0; i < p.ops.size(); i++) {
+            const uint64_t dst = p.ops[i].dst, s = (dst - reinterpret_cast<uint64_t>(p.arena) - p.node_off) / 32;
+            if (s < pool_op.size()) pool_op[s] = (uint32_t)i;
+            else if ((dst - p.forced_base) / 32 < forced_op.size()) forced_op[(dst - p.forced_base) / 32] = (uint32_t)i;
+        }
+    }
+    // the resident trees and converted lists of a state handle
+    void add_state(const lhb200_state* st) {
+        for (const lhb200_state::Tree& t : st->trees) {
+            if (t.list >= 0) converted.push_back({reinterpret_cast<uint64_t>(t.dev.field_dst), &t.dev});
+            else resident.push_back({reinterpret_cast<uint64_t>(t.dev.top_dst), &t.dev});
+        }
+    }
+    uint32_t producer(uint64_t a) const {
+        const uint64_t off = a - reinterpret_cast<uint64_t>(pl.arena) - pl.node_off;   // outside the pool: huge
+        if (off % 32 == 0 && off / 32 < pool_op.size()) return pool_op[off / 32];
+        const uint64_t f = a - pl.forced_base;
+        if (f % 32 == 0 && f / 32 < forced_op.size()) return forced_op[f / 32];
+        return NONE;
+    }
+    static const TreeDev* find(const std::vector<std::pair<uint64_t, const TreeDev*>>& v, uint64_t a) {
+        for (const auto& e : v)
+            if (e.first == a) return e.second;
+        return nullptr;
+    }
+    uint32_t tree_id(const TreeDev* dev, const Plan::ListRec* rec) {
+        for (size_t k = 0; k < trees.size(); k++)
+            if (trees[k].dev == dev && trees[k].rec == rec) return (uint32_t)k;
+        trees.push_back({dev, rec});
+        return (uint32_t)trees.size() - 1;
+    }
+    static ProofSrc zero(uint32_t l) { return {OP_ZERO_FLAG | l, 0, 0}; }
+    // the left spine node of a non-empty converted list at level l >= top: its top node laddered with zero hashes
+    static ProofSrc spine(const TreeDev& t, uint32_t l) { return {reinterpret_cast<uint64_t>(t.lvl[t.top]), t.top, l}; }
+
+    void push(uint64_t node, uint32_t tree, uint32_t level, uint32_t n_tree, uint32_t src, uint32_t depth) {
+        desc.push_back({node, tree, level, n_tree, src});
+        first.push_back(first.back() + depth);
+    }
+    static int32_t refuse(uint64_t g, const char* why) {
+        set_error("merkle proof: gindex %llu: %s", (unsigned long long)g, why);
+        return LHB200_EINVAL;
+    }
+
+    // Resolve gindex g below the node `root` into one more proof.
+    int32_t resolve(uint64_t root, uint64_t g) {
+        if (g == 0) return refuse(g, "0 is not a generalized index");
+        const uint32_t D = 63 - (uint32_t)__builtin_clzll(g);
+        for (uint32_t d : memo_depths) {
+            if (d > D) continue;
+            const auto it = memo.find({root, g >> (D - d)});
+            if (it == memo.end()) continue;
+            const Entry& e = it->second;
+            if (D - d > e.top) return refuse(g, "below a leaf");
+            push(g & ((1ull << (D - d)) - 1), e.tree, e.top - (D - d), D - d, e.src, D);
+            return LHB200_OK;
+        }
+        std::vector<ProofSrc> up;   // siblings so far, top-down
+        uint64_t cur = root;
+        const TreeDev* list = nullptr;   // inside a converted list: at its field root (level limit_depth + 1) or on
+        uint32_t level = 0;              // its left spine at `level`
+        bool leaf = false;
+        auto enter = [&](uint32_t tree, uint32_t top, uint32_t r) {   // the remaining r bits index the tree's levels
+            if (r > top) return refuse(g, "below a leaf");
+            const uint32_t src = (uint32_t)srcs.size();
+            srcs.insert(srcs.end(), up.rbegin(), up.rend());
+            memo[{root, g >> r}] = {tree, top, src};
+            if (std::find(memo_depths.begin(), memo_depths.end(), D - r) == memo_depths.end()) memo_depths.push_back(D - r);
+            push(g & ((1ull << r) - 1), tree, top - r, r, src, D);
+            return LHB200_OK;
+        };
+        for (int k = (int)D - 1; k >= 0; k--) {
+            const uint32_t bit = (g >> k) & 1, r = (uint32_t)k + 1;   // r levels left below the current node
+            if (leaf) return refuse(g, "below a leaf");
+            if (!list && !(cur & OP_ZERO_FLAG)) {
+                const uint32_t i = producer(cur);
+                if (i != NONE) {
+                    const HashOp& op = pl.ops[i];
+                    up.push_back({bit ? op.a : op.b, 0, 0});
+                    cur = bit ? op.b : op.a;
+                    continue;
+                }
+                if (const TreeDev* t = find(resident, cur)) return enter(tree_id(t, nullptr), t->top, r);
+                if ((list = find(converted, cur))) {
+                    level = list->limit_depth + 1;
+                } else {
+                    for (const Plan::ListRec& lr : pl.merkle_lists)
+                        if (lr.top_addr == cur) return enter(tree_id(nullptr, &lr), ceil_log2(lr.n), r);
+                    return refuse(g, "below a leaf");
+                }
+            }
+            if (list) {
+                const TreeDev& t = *list;
+                if (level == t.top && t.n_leaves) return enter(tree_id(list, nullptr), t.top, r);
+                if (level > t.limit_depth) {   // field root = H(data root, length chunk)
+                    if (bit) {
+                        up.push_back(t.n_leaves ? spine(t, t.limit_depth) : zero(t.limit_depth));
+                        leaf = true;
+                        continue;
+                    }
+                    std::array<uint8_t, 32> len{};
+                    for (int b = 0; b < 8; b++) len[b] = (uint8_t)(t.length >> (8 * b));
+                    up.push_back({PROOF_IMM | imm.size(), 0, 0});
+                    imm.push_back(len);
+                    if (t.n_leaves) { level = t.limit_depth; } else { list = nullptr; cur = OP_ZERO_FLAG | t.limit_depth; }
+                    continue;
+                }
+                // on the left spine above the top: a left turn stays on it, a right turn enters a zero subtree
+                up.push_back(bit ? spine(t, level - 1) : zero(level - 1));
+                if (bit) { list = nullptr; cur = OP_ZERO_FLAG | (level - 1); }
+                level--;
+                continue;
+            }
+            const uint32_t z = (uint32_t)(cur & 0xff);   // a zero subtree of height z
+            if (r > z) return refuse(g, "below a leaf");
+            for (uint32_t l = z; l > z - r; l--) up.push_back(zero(l - 1));
+            break;
+        }
+        const uint32_t src = (uint32_t)srcs.size();
+        srcs.insert(srcs.end(), up.rbegin(), up.rend());
+        push(0, 0, 0, 0, src, D);
+        return LHB200_OK;
+    }
+
+    // Bytes of the tables (pinned staging and device alike), then of the rebuilt levels and of the branches.
+    size_t table_bytes() const {
+        return align_up(desc.size() * sizeof(ProofDesc), 256) + align_up(first.size() * 8, 256) +
+               align_up(srcs.size() * sizeof(ProofSrc), 256) + align_up(imm.size() * 32, 256) +
+               align_up(trees.size() * sizeof(ProofTree), 256);
+    }
+    size_t levels_bytes() const {
+        size_t b = 0;
+        for (const TreeUse& u : trees)
+            if (u.rec)
+                for (uint64_t n = u.rec->n, l = 1; l < ceil_log2(u.rec->n); l++) b += align_up((n = ceil_div(n, 2)) * 32, 256);
+        return b;
+    }
+    size_t device_bytes() const { return table_bytes() + levels_bytes() + align_up(first.back() * 32, 256) + 256; }
+
+    // Device state of one call: the tables at `d` (device_bytes()), staged through the pinned `h` (table_bytes()).
+    ProofDesc* d_desc = nullptr;
+    uint64_t* d_first = nullptr;
+    ProofSrc* d_srcs = nullptr;
+    ProofTree* d_trees = nullptr;
+    uint8_t* d_branches = nullptr;
+    std::vector<ProofTree> tabs;
+    int32_t upload(uint8_t* h, uint8_t* d, cudaStream_t s) {
+        size_t o = 0;
+        auto put = [&](const void* src, size_t bytes) {
+            uint8_t* p = d + o;
+            if (bytes) memcpy(h + o, src, bytes);
+            o += align_up(bytes, 256);
+            return p;
+        };
+        d_desc = reinterpret_cast<ProofDesc*>(put(desc.data(), desc.size() * sizeof(ProofDesc)));
+        d_first = reinterpret_cast<uint64_t*>(put(first.data(), first.size() * 8));
+        const size_t o_srcs = o;
+        d_srcs = reinterpret_cast<ProofSrc*>(put(srcs.data(), srcs.size() * sizeof(ProofSrc)));
+        uint8_t* d_imm = put(imm.data(), imm.size() * 32);
+        for (size_t i = 0; i < srcs.size(); i++) {   // immediates: now that they have an address
+            ProofSrc& x = reinterpret_cast<ProofSrc*>(h + o_srcs)[i];
+            if (!(x.op & OP_ZERO_FLAG) && (x.op & PROOF_IMM)) x.op = reinterpret_cast<uint64_t>(d_imm + 32 * (x.op & ~PROOF_IMM));
+        }
+        uint8_t* lv = d + table_bytes();   // rebuilt levels, laid out as levels_bytes() counts them
+        tabs.assign(trees.size(), ProofTree{});
+        for (size_t k = 0; k < trees.size(); k++) {
+            ProofTree& pt = tabs[k];
+            if (trees[k].dev) {
+                for (int l = 0; l < 41; l++) pt.lvl[l] = trees[k].dev->lvl[l];
+                pt.n_leaves = trees[k].dev->n_leaves;
+                continue;
+            }
+            const Plan::ListRec& lr = *trees[k].rec;
+            pt.lvl[0] = lr.chunks;
+            pt.n_leaves = lr.n;
+            uint64_t n = lr.n;
+            for (uint32_t l = 1; l < ceil_log2(lr.n); l++) {
+                pt.lvl[l] = lv;
+                lv += align_up((n = ceil_div(n, 2)) * 32, 256);
+            }
+        }
+        d_trees = reinterpret_cast<ProofTree*>(put(tabs.data(), tabs.size() * sizeof(ProofTree)));
+        d_branches = lv;
+        LHB_CUDA(cudaMemcpyAsync(d, h, o, cudaMemcpyHostToDevice, s));
+        return LHB200_OK;
+    }
+    // After the root: rebuild the levels of the merkle_lists the proofs enter (one k_tree_level launch per level), then
+    // gather every sibling (one k_proof_branches launch).  e0 / e1 (optional) are recorded around the gather.
+    int32_t enqueue(cudaStream_t s, cudaEvent_t e0 = nullptr, cudaEvent_t e1 = nullptr) const {
+        for (size_t k = 0; k < trees.size(); k++) {
+            if (!trees[k].rec) continue;
+            uint64_t n = trees[k].rec->n;
+            for (uint32_t l = 0; l + 2 <= ceil_log2(trees[k].rec->n); l++) {
+                k_tree_level<<<(unsigned)ceil_div(ceil_div(n, 2), 256), 256, 0, s>>>(tabs[k].lvl[l], n,
+                                                                                    const_cast<uint8_t*>(tabs[k].lvl[l + 1]), l);
+                count_launch();
+                n = ceil_div(n, 2);
+            }
+        }
+        const uint64_t total = first.back();
+        if (e0) cudaEventRecord(e0, s);
+        if (total) {
+            k_proof_branches<<<(unsigned)ceil_div(total, 256), 256, 0, s>>>(d_desc, d_first, (uint32_t)desc.size(), d_trees,
+                                                                           d_srcs, d_branches);
+            count_launch();
+        }
+        if (e1) cudaEventRecord(e1, s);
+        LHB_CUDA(cudaGetLastError());
+        return LHB200_OK;
+    }
+};
 
 }  // namespace lhb200
 
@@ -1645,6 +1917,7 @@ static int32_t state_convert(lhb200_state* st, cudaStream_t s) {
         cut(pl.ops, a.ops, b.ops);
         cut(pl.op_wave, a.ops, b.ops);
         cut(st->trees, a.trees, b.trees);
+        cut(pl.merkle_lists, a.merkle_lists, b.merkle_lists);
         stage_units += list_units(sp, st->var_len[sp.var] / sp.item_bytes);
     }
     pl.passes.erase(std::remove_if(pl.passes.begin(), pl.passes.end(), [](const std::vector<MerkleSeg>& p) { return p.empty(); }),
@@ -1879,6 +2152,50 @@ int32_t lhb200_state_root(lhb200_state* st, uint8_t out[32], uint8_t* field_root
     return LHB200_OK;
 }
 
+static int32_t proof_events() {
+    for (cudaEvent_t& e : g_proof_ev)
+        if (!e) LHB_CUDA(cudaEventCreate(&e));
+    return LHB200_OK;
+}
+float lhb200_debug_proof_gather_ms(void) {
+    std::lock_guard<std::recursive_mutex> g(ctx().mu);   // the events belong to the calls that record them
+    float ms = -1.f;
+    if (!g_proof_ev[0] || cudaEventElapsedTime(&ms, g_proof_ev[0], g_proof_ev[1]) != cudaSuccess) { cudaGetLastError(); return -1.f; }
+    return ms;
+}
+
+// Branches of generalized indices of a resident state.  Every gindex is resolved on the host before the handle is
+// touched, so a refused call leaves it as it was; then one root (warm or cold, as lhb200_state_root), the levels the
+// proofs rebuild, one gather and one synchronise.
+int32_t lhb200_state_proofs(lhb200_state* st, const uint64_t* gindices, uint32_t n, uint8_t* branches, uint8_t root[32]) {
+    LHB_REQUIRE_READY();
+    if (!st || !root || (n && !gindices)) { set_error("state_proofs: null argument"); return LHB200_EINVAL; }
+    if (st->shard.world != 1) { set_error("state_proofs: a sharded handle holds only its share of the lists"); return LHB200_EINVAL; }
+    Ctx& c = ctx();
+    std::lock_guard<std::recursive_mutex> g(c.mu);
+    ProofResolver pr(st->plan);
+    pr.add_state(st);
+    int32_t rc;
+    for (uint32_t i = 0; i < n; i++)
+        if ((rc = pr.resolve(st->root_op, gindices[i]))) return rc;
+    const uint64_t total = pr.first.back();
+    if (total && !branches) { set_error("state_proofs: null branches"); return LHB200_EINVAL; }
+    if ((rc = proof_events())) return rc;
+    // pinned: the front is what a root stages (its tree and dirty tables), then the proof tables and the root
+    const size_t front = align_up(st->trees_bytes() + st->dirty_bytes(), 256), tb = pr.table_bytes();
+    uint8_t* h = static_cast<uint8_t*>(pinned_scratch(front + tb + 256));
+    uint8_t* d = static_cast<uint8_t*>(dev_scratch(pr.device_bytes()));
+    if (!h || !d) return LHB200_ENOMEM;
+    if ((rc = pr.upload(h + front, d, c.stream))) return rc;
+    if ((rc = lhb200_state_root_enqueue(st, c.stream, nullptr))) return rc;
+    if ((rc = pr.enqueue(c.stream, g_proof_ev[0], g_proof_ev[1]))) return rc;
+    LHB_CUDA(cudaMemcpyAsync(h + front + tb, st->d_result, 32, cudaMemcpyDeviceToHost, c.stream));
+    if (total) LHB_CUDA(cudaMemcpyAsync(branches, pr.d_branches, total * 32, cudaMemcpyDefault, c.stream));
+    LHB_CUDA(cudaStreamSynchronize(c.stream));
+    memcpy(root, h + front + tb, 32);
+    return LHB200_OK;
+}
+
 int32_t lhb200_state_release(lhb200_state* st) {
     if (!st) return LHB200_OK;
     std::lock_guard<std::recursive_mutex> g(ctx().mu);
@@ -1934,6 +2251,7 @@ static void visit_device_addresses(lhb200_state* st, F&& f) {
     for (HashOp& op : pl.ops) { f(op.dst, 0); f(op.a, 0); f(op.b, 0); }
     for (ByteItem& it : pl.items) { at(it.src); at(it.out); }
     for (Plan::TreeSpec& ts : pl.trees) { at(ts.chunks); f(ts.top_addr, 0); at(ts.src); }
+    for (Plan::ListRec& lr : pl.merkle_lists) { at(lr.chunks); f(lr.top_addr, 0); }
     at(pl.d_ops); at(pl.d_waves); at(pl.d_items);
     for (StageCopy& cp : st->copies) at(cp.dst);
     for (uint64_t& op : st->field_ops) f(op, 0);
@@ -2419,9 +2737,19 @@ static uint64_t prescan_transactions(const uint8_t* blk, uint64_t len, const For
     return first <= tx.len ? first / 4 : 0;
 }
 
+// Proofs below the body roots of a block batch (lhb200_beacon_block_body_proofs), and the device and pinned bytes
+// their tables, rebuilt levels and branches can take.
+struct BodyProofs {
+    const uint32_t* block_of;
+    const uint64_t* gindices;
+    uint32_t n;
+    uint8_t* branches;
+    size_t dev_bytes, host_bytes;
+};
+
 static int32_t block_roots_attempt(Ctx& c, const uint8_t* ssz, const uint64_t* offsets, uint32_t n, uint8_t* roots,
                                    uint8_t* body_roots, bool blinded, const ForkLayout& fl, uint64_t base, uint64_t total, size_t in_pad,
-                                   size_t max_nodes, size_t lit_cap) {
+                                   size_t max_nodes, size_t lit_cap, const BodyProofs* pq) {
     uint8_t *d_in = nullptr, *d_roots = nullptr, *d_body = nullptr;
     bool bad = false;
     auto build = [&](Plan& p) {
@@ -2441,9 +2769,12 @@ static int32_t block_roots_attempt(Ctx& c, const uint8_t* ssz, const uint64_t* o
     const size_t prog_bytes = program_bytes(max_nodes, max_nodes);
     // literals | node pool (op outputs) | staged blob | roots | item outputs, leaf-kernel roots and reduce outputs
     // (one 32-byte root per 192-byte DepositRequest, well inside one node per 12 bytes) | program blobs
-    const size_t need = lit_cap + 32 * max_nodes + in_pad + 64ull * n + 32 * max_nodes + prog_bytes + 8192;
+    // | proof tables, rebuilt levels and branches (pq)
+    const size_t need = lit_cap + 32 * max_nodes + in_pad + 64ull * n + 32 * max_nodes + prog_bytes + 8192 +
+                        (pq ? pq->dev_bytes : 0);
     uint8_t* arena = static_cast<uint8_t*>(dev_scratch(need));
-    const size_t stage_bytes = align_up(total, 256) + lit_cap + prog_bytes + 64ull * n + 1024;
+    const size_t h_proofs = align_up(total, 256) + lit_cap + prog_bytes;   // after what plan_upload stages
+    const size_t stage_bytes = h_proofs + (pq ? pq->host_bytes : 0) + 64ull * n + 1024;
     uint8_t* hst = static_cast<uint8_t*>(pinned_scratch(stage_bytes));
     if (!arena || !hst) return LHB200_ENOMEM;
     Plan pl;
@@ -2454,13 +2785,32 @@ static int32_t block_roots_attempt(Ctx& c, const uint8_t* ssz, const uint64_t* o
                   "%zu of %zu arena bytes)", pl.ops.size(), pl.items.size(), max_nodes, pl.lit.size(), lit_cap, pl.bump, need);
         return LHB200_ERETRY;
     }
+    // the proofs are resolved over the finished plan; their tables and branches go after its program blobs
+    std::unique_ptr<ProofResolver> pr;
+    if (pq) {
+        pr.reset(new ProofResolver(pl));
+        for (uint32_t i = 0; i < pq->n; i++)
+            if ((rc = pr->resolve(reinterpret_cast<uint64_t>(d_body + 32ull * pq->block_of[i]), pq->gindices[i]))) return rc;
+        if (pr->table_bytes() > pq->host_bytes ||
+            pl.bump + program_bytes(pl.ops.size(), pl.items.size()) + pr->device_bytes() > need) {
+            set_error("internal: block proofs exceed their bound (%zu table bytes of %zu, %zu device bytes)",
+                      pr->table_bytes(), pq->host_bytes, pr->device_bytes());
+            return LHB200_EINVAL;
+        }
+    }
     memcpy(hst, ssz + base, total);
     memset(hst + total, 0, align_up(total, 256) - total);
     LHB_CUDA(cudaMemcpyAsync(d_in, hst, align_up(total, 256), cudaMemcpyHostToDevice, c.stream));
     rc = plan_upload(pl, c.stream, hst + align_up(total, 256));
     if (rc) return rc;
+    if (pr && (rc = pr->upload(hst + h_proofs, pl.alloc(pr->device_bytes()), c.stream))) return rc;
     rc = plan_enqueue(pl, c.stream);
     if (rc) return rc;
+    if (pr) {
+        if ((rc = proof_events()) || (rc = pr->enqueue(c.stream, g_proof_ev[0], g_proof_ev[1]))) return rc;
+        if (pr->first.back())
+            LHB_CUDA(cudaMemcpyAsync(pq->branches, pr->d_branches, pr->first.back() * 32, cudaMemcpyDefault, c.stream));
+    }
     uint8_t* h_out = hst + stage_bytes - 64ull * n - 64;
     LHB_CUDA(cudaMemcpyAsync(h_out, d_roots, 32ull * n, cudaMemcpyDeviceToHost, c.stream));
     if (body_roots) LHB_CUDA(cudaMemcpyAsync(h_out + 32ull * n, d_body, 32ull * n, cudaMemcpyDeviceToHost, c.stream));
@@ -2472,7 +2822,8 @@ static int32_t block_roots_attempt(Ctx& c, const uint8_t* ssz, const uint64_t* o
 
 // n BeaconBlock SSZ blobs of `fork`, concatenated; offsets[n+1]; roots n*32; body_roots n*32 or NULL.
 static int32_t block_roots(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, uint8_t* roots,
-                                 uint8_t* body_roots, bool blinded, int32_t fork = LHB200_FORK_DENEB) {
+                                 uint8_t* body_roots, bool blinded, int32_t fork = LHB200_FORK_DENEB,
+                                 BodyProofs* pq = nullptr) {
     LHB_REQUIRE_READY();
     const ForkLayout* fl = fork_layout(fork);
     if (!fl || (blinded && !fl->payload_fields)) {
@@ -2492,13 +2843,22 @@ static int32_t block_roots(const uint8_t* ssz, const uint64_t* offsets, uint32_t
     uint64_t n_tx = 0;
     if (!blinded)
         for (uint32_t i = 0; i < n; i++) n_tx += prescan_transactions(ssz + offsets[i], offsets[i + 1] - offsets[i], *fl);
+    if (pq) {   // bounds: one source per sibling, and one rebuilt tree per block (its DepositRequest list) of at most
+                // one chunk per 192 input bytes, over at most 13 levels
+        uint64_t siblings = 0;
+        for (uint32_t i = 0; i < pq->n; i++) siblings += pq->gindices[i] ? 63 - __builtin_clzll(pq->gindices[i]) : 0;
+        pq->host_bytes = align_up(pq->n * sizeof(ProofDesc), 256) + align_up((pq->n + 1) * 8ull, 256) +
+                         align_up(siblings * sizeof(ProofSrc), 256) + 256 + align_up(n * sizeof(ProofTree), 256);
+        pq->dev_bytes = pq->host_bytes + 32 * (total / 192) + n * 14 * 256ull + align_up(siblings * 32, 256) + 1024;
+    }
     int32_t rc = LHB200_OK;
     for (int attempt = 0; attempt < 2; attempt++) {
         // attempt 0: transactions counted, everything else <= one node per 12 bytes and one literal per 8 bytes;
         // attempt 1 (only if a plan ever exceeds that): the unconditional bound of one node and literal per 2 bytes.
         const size_t max_nodes = attempt == 0 ? 2 * n_tx + total / 12 + 512ull * n : total / 2 + 512ull * n;
         const size_t lit_cap = align_up(32 * (attempt == 0 ? n_tx + total / 8 + 128ull * n : total / 2 + 128ull * n), 256);
-        rc = block_roots_attempt(c, ssz, offsets, n, roots, body_roots, blinded, *fl, base, total, in_pad, max_nodes, lit_cap);
+        rc = block_roots_attempt(c, ssz, offsets, n, roots, body_roots, blinded, *fl, base, total, in_pad, max_nodes, lit_cap,
+                                 pq);
         if (rc != LHB200_ERETRY) break;
     }
     return rc == LHB200_ERETRY ? LHB200_EINVAL : rc;
@@ -2516,6 +2876,27 @@ int32_t lhb200_beacon_block_root_deneb(const uint8_t* ssz, uint64_t len, uint8_t
 int32_t lhb200_beacon_block_roots(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, int32_t fork, int32_t blinded,
                                   uint8_t* roots, uint8_t* body_roots) {
     return block_roots(ssz, offsets, n, roots, body_roots, blinded != 0, fork);
+}
+// Branches of generalized indices below the body roots of a block batch (BeaconBlockBody::kzg_commitment_merkle_proof,
+// beacon_block_body.rs:178-227, and the other body proofs): one plan for the batch as lhb200_beacon_block_roots builds
+// it, the proofs resolved over it before anything runs, and their branches gathered before the arena goes back.
+int32_t lhb200_beacon_block_body_proofs(const uint8_t* ssz, const uint64_t* offsets, uint32_t n_blocks, int32_t fork,
+                                        int32_t blinded, const uint32_t* block_of, const uint64_t* gindices, uint32_t n,
+                                        uint8_t* branches, uint8_t* body_roots) {
+    LHB_REQUIRE_READY();
+    if (!body_roots || (n && (!block_of || !gindices))) { set_error("beacon_block_body_proofs: null argument"); return LHB200_EINVAL; }
+    uint64_t siblings = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        if (block_of[i] >= n_blocks) {
+            set_error("beacon_block_body_proofs: proof %u is taken in block %u of %u", i, block_of[i], n_blocks);
+            return LHB200_EINVAL;
+        }
+        siblings += gindices[i] ? 63 - __builtin_clzll(gindices[i]) : 0;
+    }
+    if (siblings && !branches) { set_error("beacon_block_body_proofs: null branches"); return LHB200_EINVAL; }
+    std::vector<uint8_t> roots(32ull * std::max<uint32_t>(n_blocks, 1));
+    BodyProofs pq{block_of, gindices, n, branches, 0, 0};
+    return block_roots(ssz, offsets, n_blocks, roots.data(), body_roots, blinded != 0, fork, &pq);
 }
 // BlindedBeaconBlock (beacon_block.rs:80): the body carries the ExecutionPayloadHeader; the root equals the full block's.
 int32_t lhb200_blinded_beacon_block_roots_deneb(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, uint8_t* roots,

@@ -157,6 +157,67 @@ def beacon_block_roots(blocks, fork="deneb", want_body_roots=False, blinded=Fals
     return roots
 
 
+# Generalized indices the reference proves (light_client_update.rs, beacon_block_body.rs; consensus-specs
+# ssz/merkle-proofs.md).  The state ones are for the 32-leaf top tree of Altair to Deneb; Electra's 37 fields take a
+# 64-leaf top tree, one level deeper.
+FINALIZED_ROOT_INDEX = 105            # finalized_checkpoint.root: (32 + 20) * 2 + 1
+CURRENT_SYNC_COMMITTEE_INDEX = 54
+NEXT_SYNC_COMMITTEE_INDEX = 55
+FINALIZED_ROOT_INDEX_ELECTRA = 169    # (64 + 20) * 2 + 1
+CURRENT_SYNC_COMMITTEE_INDEX_ELECTRA = 86
+NEXT_SYNC_COMMITTEE_INDEX_ELECTRA = 87
+EXECUTION_PAYLOAD_INDEX = 25          # body field 9 of a 16-leaf body tree (Bellatrix to Electra)
+BLOB_KZG_COMMITMENTS_INDEX = 27       # body field 11
+KZG_COMMITMENT_INCLUSION_PROOF_DEPTH = 17
+
+
+def kzg_commitment_gindex(i):
+    """Body gindex of blob_kzg_commitments[i]: field 27, the list's data root (27 * 2), then depth 12 (4096 items)."""
+    return 54 * 4096 + i
+
+
+def _split_branches(g, call, where, raw):
+    """Run `call(out, root)` for the gindices g (uint64 array) and cut the flat output into per-proof branches."""
+    import numpy as np
+    depths = np.array([int(x).bit_length() - 1 if x else 0 for x in g.tolist()], dtype=np.int64)
+    total = int(depths.sum())
+    out = np.zeros(max(32 * total, 1), dtype=np.uint8)
+    root = C.create_string_buffer(32)
+    check(call(C.c_void_p(out.ctypes.data), root), where)
+    if raw:
+        return root.raw, out[:32 * total]
+    flat, at, branches = out.tobytes(), 0, []
+    for d in depths.tolist():
+        branches.append([flat[32 * (at + k): 32 * (at + k + 1)] for k in range(d)])
+        at += d
+    return root.raw, branches
+
+
+def beacon_block_body_proofs(blocks, proofs, fork="deneb", blinded=False, raw=False):
+    """Merkle branches below the BODY roots of a batch of BeaconBlock<fork> (or blinded) SSZ blobs, in one pass
+    (lhb200_beacon_block_body_proofs).  proofs: [(block index, body gindex), ...].  -> (body roots, branches), branches
+    as ResidentState.proofs gives them (kzg_commitment_gindex(i): the 17-sibling blob inclusion proof)."""
+    import numpy as np
+    blocks = [bytes(b) for b in blocks]
+    n = len(blocks)
+    offs = (C.c_uint64 * (n + 1))()
+    for i, b in enumerate(blocks):
+        offs[i + 1] = offs[i] + len(b)
+    p, keep = buf(b"".join(blocks))
+    block_of = np.ascontiguousarray([b for b, _ in proofs], dtype=np.uint32)
+    g = np.ascontiguousarray([x for _, x in proofs], dtype=np.uint64)
+    body = C.create_string_buffer(32 * max(n, 1))
+    root, branches = _split_branches(g, lambda out, _root: lib.lhb200_beacon_block_body_proofs(
+        p, C.cast(offs, C.c_void_p), n, FORKS[fork], 1 if blinded else 0, block_of.ctypes.data, g.ctypes.data, len(g),
+        out, body), "lhb200_beacon_block_body_proofs", raw)
+    return [body.raw[32 * i: 32 * i + 32] for i in range(n)], branches
+
+
+def debug_proof_gather_ms():
+    """Benchmark hook: device time of the last k_proof_branches launch (CUDA events), < 0 if unavailable."""
+    return float(lib.lhb200_debug_proof_gather_ms())
+
+
 def beacon_block_root_deneb(ssz, want_body_root=False, blinded=False):
     """canonical_root of one BeaconBlockDeneb; optionally also hash_tree_root(body) (BeaconBlockHeader.body_root)."""
     r = beacon_block_roots_deneb([ssz], want_body_root, blinded)
@@ -301,6 +362,19 @@ class ResidentState:
         new.fork = self.fork
         check(lib.lhb200_state_clone(self._h, C.byref(new._h)), "lhb200_state_clone")
         return new
+
+    def proofs(self, gindices, raw=False):
+        """Merkle branches of generalized indices of this state, in one call (lhb200_state_proofs): roots the handle
+        first, as root() does.  -> (state root, branches): branch i lists floor(log2(gindices[i])) 32-byte siblings,
+        bottom-up.  raw=True returns the branches as one flat uint8 array (proof i at 32 * the depths before it)."""
+        import numpy as np
+        g = np.ascontiguousarray(np.asarray(gindices, dtype=np.uint64).reshape(-1))
+        return _split_branches(g, lambda out, root: lib.lhb200_state_proofs(self._h, g.ctypes.data, len(g), out, root),
+                               "lhb200_state_proofs", raw)
+
+    def compute_merkle_proof(self, gindex):
+        """BeaconState::compute_merkle_proof (beacon_state.rs:2483) by the spec's generalized index: the branch."""
+        return self.proofs([gindex])[1][0]
 
     @property
     def device_bytes(self):
