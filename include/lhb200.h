@@ -460,6 +460,12 @@ LHB200_API int32_t lhb200_debug_group_messages(const uint8_t* msgs, uint32_t n, 
  * 5 fp2 op([opcode|a|b] -> 96), 6 pairing+final_exp(g1 96|g2 96 -> 576), 7 g1 sum([n|n*96] -> 96). */
 LHB200_API int32_t lhb200_debug_bls(int32_t op, const uint8_t* in, uint32_t in_len, uint8_t* out, uint32_t out_len,
                                     int32_t* rc);
+/* Test hook: n cases of one base-field operation on raw little-endian 32-bit limbs, one device thread per case, so
+ * `pytest -m gpu` can check the carry chains of the Fp arithmetic case by case (op codes, operand layouts and the
+ * 37-word result of a case in bls/fp_probe.cuh).  in: n x in_words words (the op's operand count, else EINVAL);
+ * out: n x out_words words (out_words = 37). */
+LHB200_API int32_t lhb200_debug_fp_batch(int32_t op, const uint32_t* in, uint32_t in_words, uint32_t n, uint32_t* out,
+                                         uint32_t out_words);
 
 #ifdef __cplusplus
 }

@@ -101,6 +101,7 @@ _sig("lhb200_sign", C.c_int32, vp, vp, C.c_uint32, vp)
 _sig("lhb200_g1_decompress_validate", C.c_int32, vp, C.c_uint32, vp, vp)
 _sig("lhb200_g2_decompress", C.c_int32, vp, C.c_uint32, vp, vp)
 _sig("lhb200_debug_bls", C.c_int32, C.c_int32, vp, C.c_uint32, vp, C.c_uint32, C.POINTER(C.c_int32))
+_sig("lhb200_debug_fp_batch", C.c_int32, C.c_int32, vp, C.c_uint32, C.c_uint32, vp, C.c_uint32)
 _sig("lhb200_bls_batch_dominant_kernel_ms", C.c_float, vp)
 _sig("lhb200_state_dominant_kernel_ms", C.c_float, vp)
 _sig("lhb200_pubkey_table_create", C.c_int32, C.c_uint64, C.POINTER(vp))

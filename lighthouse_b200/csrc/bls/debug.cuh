@@ -1,8 +1,10 @@
 // debug.cuh — single-thread stage probes used by the GPU parity tests (same stages as tests/hostsim):
 // lets `pytest -m gpu` compare every stage of the BLS pipeline with the oracle, not just the final boolean.
+// k_debug_fp_batch runs one base-field operation per thread over many cases (bls/fp_probe.cuh).
 #pragma once
 #include "kernels.cuh"
 #include "coop.cuh"
+#include "fp_probe.cuh"
 
 namespace lhb200 {
 namespace bls {
@@ -102,6 +104,19 @@ __global__ void k_debug_bls(int op, const uint8_t* __restrict__ in, uint8_t* __r
         } break;
         default: *rc = -100;
     }
+}
+
+// Batched field probe (lhb200_debug_fp_batch): one thread per case over as many blocks as the cases need.  The y
+// operands of the sum-of-products ops are streamed from this block's shared memory at a stride of FP_PROBE_BLOCK words,
+// the column layout the pipeline kernels use.
+constexpr int FP_PROBE_BLOCK = 32;
+__global__ void __launch_bounds__(FP_PROBE_BLOCK) k_debug_fp_batch(int op, const uint32_t* __restrict__ in, uint32_t n,
+                                                                   uint32_t* __restrict__ out) {
+    __shared__ uint32_t ycol[FP_PROBE_Y_WORDS * FP_PROBE_BLOCK];
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int w = fp_probe_in_words(op);
+    fp_probe(op, in + (size_t)w * i, ycol + threadIdx.x, FP_PROBE_BLOCK, out + (size_t)FP_PROBE_OUT_WORDS * i);
 }
 
 }  // namespace bls

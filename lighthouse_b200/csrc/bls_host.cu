@@ -1908,4 +1908,31 @@ int32_t lhb200_debug_bls(int32_t op, const uint8_t* in, uint32_t in_len, uint8_t
     return LHB200_OK;
 }
 
+// Test hook: n cases of one base-field operation, one device thread per case (op codes and layouts in bls/fp_probe.cuh).
+int32_t lhb200_debug_fp_batch(int32_t op, const uint32_t* in, uint32_t in_words, uint32_t n, uint32_t* out,
+                              uint32_t out_words) {
+    LHB_REQUIRE_READY();
+    const int w = fp_probe_in_words(op);
+    if (w == 0 || in_words != (uint32_t)w || out_words != (uint32_t)FP_PROBE_OUT_WORDS) {
+        set_error("debug_fp_batch: op %d takes %d words in and %d out", op, w, FP_PROBE_OUT_WORDS);
+        return LHB200_EINVAL;
+    }
+    if (n == 0) return LHB200_OK;
+    if (!in || !out) return LHB200_EINVAL;
+    Ctx& c = ctx();
+    std::lock_guard<std::recursive_mutex> g(c.mu);
+    const size_t b_in = ((size_t)n * w * 4 + 255) / 256 * 256, b_out = (size_t)n * FP_PROBE_OUT_WORDS * 4;
+    uint8_t* d = static_cast<uint8_t*>(dev_scratch(b_in + b_out + 256));
+    if (!d) return LHB200_ENOMEM;
+    uint32_t* d_in = reinterpret_cast<uint32_t*>(d);
+    uint32_t* d_out = reinterpret_cast<uint32_t*>(d + b_in);
+    LHB_CUDA(cudaMemcpyAsync(d_in, in, (size_t)n * w * 4, cudaMemcpyHostToDevice, c.stream));
+    k_debug_fp_batch<<<cdiv(n, FP_PROBE_BLOCK), FP_PROBE_BLOCK, 0, c.stream>>>(op, d_in, n, d_out);
+    count_launch();
+    LHB_CUDA(cudaGetLastError());
+    LHB_CUDA(cudaMemcpyAsync(out, d_out, b_out, cudaMemcpyDeviceToHost, c.stream));
+    LHB_CUDA(cudaStreamSynchronize(c.stream));
+    return LHB200_OK;
+}
+
 }  // extern "C"

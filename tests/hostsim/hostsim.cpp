@@ -12,6 +12,7 @@
 #include "../../lighthouse_b200/csrc/bls/miller_warp.cuh"
 #include "../../lighthouse_b200/csrc/bls/g2_warp.cuh"
 #include "../../lighthouse_b200/csrc/bls/fe_warp.cuh"
+#include "../../lighthouse_b200/csrc/bls/fp_probe.cuh"
 #include <vector>
 
 using namespace lhb200::bls;
@@ -112,6 +113,23 @@ EXPORT int hs_g1_sum(const uint8_t* keys, int n, uint8_t* out96) {
     G1Jac acc; jac_set_inf(acc);
     for (int i = 0; i < n; i++) { G1Affine a; if (g1_from_uncompressed(a, keys + 96 * i) == DEC_BAD) return -1; jac_add_affine(acc, acc, a); }
     G1Affine r; jac_to_affine(r, acc); g1_to_uncompressed(out96, r); return 0;
+}
+// the device's 96-byte key decoding as lhb200_g1_deserialize_uncompressed applies it: g1_from_uncompressed, then the
+// on-curve check for a finite point.  rc = DecodeStatus; out96 = the re-serialised point unless rc is DEC_BAD.
+EXPORT int hs_g1_from_uncompressed(const uint8_t* p96, uint8_t* out96) {
+    G1Affine a; int rc = g1_from_uncompressed(a, p96);
+    if (rc == DEC_OK && !g1_on_curve(a)) rc = DEC_BAD;
+    if (rc == DEC_BAD) return rc;
+    g1_to_uncompressed(out96, a); return rc;
+}
+// bls/fp_probe.cuh on n cases (the body of lhb200_debug_fp_batch): in n x fp_probe_in_words(op), out n x 37 words.
+// y operands are streamed at a stride of 3 words.  -1 for an unknown op.
+EXPORT int hs_fp_batch(int op, const uint32_t* in, uint32_t n, uint32_t* out) {
+    const int w = fp_probe_in_words(op);
+    if (w == 0) return -1;
+    std::vector<uint32_t> ycol(FP_PROBE_Y_WORDS * 3);
+    for (uint32_t i = 0; i < n; i++) fp_probe(op, in + (size_t)w * i, ycol.data(), 3, out + (size_t)FP_PROBE_OUT_WORDS * i);
+    return 0;
 }
 EXPORT int hs_g2_roundtrip(const uint8_t* p96, uint8_t* out96) {
     G2Affine a; int rc = g2_decompress(a, p96); if (rc == DEC_BAD) return rc;
