@@ -81,10 +81,13 @@ LHB200_API int32_t lhb200_validator_roots(const uint8_t* ssz, uint64_t n, uint8_
  * nodes) — consensus/types/src/beacon_state.rs:2031-2038, fields :343-484.  `ssz` is the SSZ encoding of
  * BeaconStateDeneb.  field_roots (28*32 bytes) is optional (NULL to skip). */
 LHB200_API int32_t lhb200_beacon_state_root_deneb(const uint8_t* ssz, uint64_t len, uint8_t out[32], uint8_t* field_roots);
-/* The other post-Altair variants of the BeaconState superstruct (consensus/types/src/beacon_state.rs:224-571) through
- * the same kernels; `fork` is one of LHB200_FORK_*.  Altair has 24 fields, Bellatrix 25 (+ a 14-field execution payload
- * header), Capella 28 (15-field header, withdrawal indices, historical_summaries), Deneb 28 (17-field header).
+/* The other variants of the BeaconState superstruct (consensus/types/src/beacon_state.rs:224-571) through the same
+ * kernels; `fork` is one of LHB200_FORK_*.  Base (phase0) has 21 fields, whose 15 and 16 are previous_ /
+ * current_epoch_attestations: List[PendingAttestation, 4096] (pending_attestation.rs:25-32), rooted by one
+ * k_pending_attestation_roots launch for both lists.  Altair has 24 fields, Bellatrix 25 (+ a 14-field execution
+ * payload header), Capella 28 (15-field header, withdrawal indices, historical_summaries), Deneb 28 (17-field header).
  * field_roots (optional, 28 x 32 B): entries beyond the fork's field count are zero chunks. */
+#define LHB200_FORK_BASE 0
 #define LHB200_FORK_ALTAIR 1
 #define LHB200_FORK_BELLATRIX 2
 #define LHB200_FORK_CAPELLA 3
@@ -101,7 +104,9 @@ LHB200_API int32_t lhb200_state_stage_deneb(const uint8_t* ssz, uint64_t len, lh
 LHB200_API int32_t lhb200_state_root(lhb200_state* st, uint8_t out[32], uint8_t* field_roots);
 /* Same-length in-place mutation of a staged state — the resident analogue of apply_pending_mutations
  * (beacon_state.rs:2459-2481): bytes [ssz_offset, ssz_offset+len) of the SSZ encoding are replaced; the next
- * lhb200_state_root re-hashes everything on the device (SURVEY.md §8f-3: warm path = patch + full re-hash). */
+ * lhb200_state_root re-hashes everything on the device (SURVEY.md §8f-3: warm path = patch + full re-hash).  On a Base
+ * handle a range inside previous_ / current_epoch_attestations gives LHB200_EINVAL (and the batch changes nothing):
+ * those lists change through lhb200_state_set_pending_attestations, which checks them. */
 LHB200_API int32_t lhb200_state_patch(lhb200_state* st, uint64_t ssz_offset, const uint8_t* data, uint64_t len);
 /* n non-overlapping same-length mutations in one call (offsets[i], lens[i], bytes concatenated in `data`): one H2D copy
  * and one scatter kernel instead of n round trips — what a slot's worth of milhouse pending updates looks like. */
@@ -126,7 +131,8 @@ LHB200_API uint64_t lhb200_state_last_root_hashes(const lhb200_state* st);
  * in [old_len, new_len) must be written.  Fields (container index, item bytes): 9 eth1_data_votes (72), 11 validators
  * (121), 12 balances (8), 15 / 16 previous_ / current_epoch_participation (1), 21 inactivity_scores (8),
  * 27 historical_summaries (64, Capella and later), 34 / 35 / 36 pending_balance_deposits / pending_partial_withdrawals /
- * pending_consolidations (16 / 24 / 16, Electra).  historical_roots is not resizable.  A field the fork does not have,
+ * pending_consolidations (16 / 24 / 16, Electra).  Base has 9, 11 and 12 only (see
+ * lhb200_state_set_pending_attestations for its fields 15 and 16).  historical_roots is not resizable.  A field the fork does not have,
  * a limit overrun, reserved != 0, or a non-incremental or sharded handle gives LHB200_EINVAL, and a refused call
  * changes nothing.  Afterwards roots, field roots, hash units and lhb200_state_patch offsets all refer to the current
  * encoding; bytes past a list's length are not resident.  Only the dirty paths, the changed lists' zero ladders and
@@ -146,6 +152,16 @@ LHB200_API int32_t lhb200_state_list_len(const lhb200_state* st, uint32_t field,
 /* Replace latest_execution_payload_header (Bellatrix and later) with `len` bytes of SSZ of the handle's fork; its
  * extra_data may change length.  Same handle requirements as lhb200_state_list_edit. */
 LHB200_API int32_t lhb200_state_set_payload_header(lhb200_state* st, const uint8_t* ssz, uint64_t len);
+/* Base: replace previous_epoch_attestations (field 15) or current_epoch_attestations (16) with `len` bytes of SSZ of a
+ * List[PendingAttestation, 4096] — per block the current list plus the block's attestations, at the epoch boundary
+ * two calls (current -> previous, then an empty current).  Same handle requirements as lhb200_state_list_edit, whose
+ * storage holds 4096 records of the largest size.  Another fork or field, malformed SSZ (offset table, record sizes,
+ * bitlist delimiter, more than 2048 bits or 4096 records) -> LHB200_EINVAL, and a refused call changes nothing.
+ * Afterwards lhb200_state_patch offsets and lhb200_state_list_len (which gives the record count of 15 / 16 on a Base
+ * handle) refer to the new encoding.  The next root re-roots every record of both lists (one launch,
+ * ~19 hashes a record) and re-hashes the replaced list's tree above the slots that changed. */
+LHB200_API int32_t lhb200_state_set_pending_attestations(lhb200_state* st, uint32_t field, const uint8_t* ssz,
+                                                         uint64_t len);
 /* Same as lhb200_state_root but only enqueues; the root lands in device memory (returned pointer valid until
  * the next call on this handle).  Used by bench.py to time kernels with CUDA events. */
 LHB200_API int32_t lhb200_state_root_enqueue(lhb200_state* st, void* stream, const void** d_root);
@@ -227,8 +243,9 @@ LHB200_API int32_t lhb200_beacon_block_roots_deneb(const uint8_t* ssz, const uin
  * the ExecutionPayloadHeaderDeneb, execution_payload_header.rs:46-87).  The root equals the full block's root. */
 LHB200_API int32_t lhb200_blinded_beacon_block_roots_deneb(const uint8_t* ssz, const uint64_t* offsets, uint32_t n,
                                                            uint8_t* roots, uint8_t* body_roots);
-/* The same for every variant of the BeaconBlock superstruct from Altair on (consensus/types/src/beacon_block.rs:41-90,
- * beacon_block_body.rs:43-121): fork = LHB200_FORK_ALTAIR (9 body fields, no execution payload), _BELLATRIX (14-field
+/* The same for every variant of the BeaconBlock superstruct from Base on (consensus/types/src/beacon_block.rs:19-90,
+ * beacon_block_body.rs:33-121): fork = LHB200_FORK_BASE (8 body fields: Altair's without sync_aggregate),
+ * _ALTAIR (9 body fields, no execution payload), _BELLATRIX (14-field
  * payload), _CAPELLA (+ withdrawals, bls_to_execution_changes), _DENEB (+ blob gas fields, blob_kzg_commitments),
  * _ELECTRA (+ consolidations; attestations with committee_bits and up to 131 072 aggregation bits, at most 8 of them
  * and 1 attester slashing; payload + deposit_requests (<= 8192) and withdrawal_requests (<= 16),

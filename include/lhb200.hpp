@@ -267,7 +267,7 @@ inline Hash256 beacon_state_root_deneb(const uint8_t* ssz, size_t len) {
     return out;
 }
 
-/// the same for any post-Altair fork id (LHB200_FORK_ALTAIR .. LHB200_FORK_ELECTRA; beacon_state.rs:224-571)
+/// the same for any fork id from Base (phase0) on (LHB200_FORK_BASE .. LHB200_FORK_ELECTRA; beacon_state.rs:224-571)
 inline Hash256 beacon_state_root(const uint8_t* ssz, size_t len, int32_t fork) {
     Hash256 out;
     check(lhb200_beacon_state_root(ssz, len, fork, out.data(), nullptr), "lhb200_beacon_state_root");
@@ -282,7 +282,8 @@ inline Hash256 beacon_block_root_deneb(const uint8_t* ssz, size_t len, Hash256* 
     return out;
 }
 
-/// canonical_root of one BeaconBlock / BlindedBeaconBlock of any fork from Altair to Electra (beacon_block.rs:41-90)
+/// canonical_root of one BeaconBlock / BlindedBeaconBlock of any fork from Base to Electra (beacon_block.rs:19-90;
+/// blinded blocks from Bellatrix on)
 inline Hash256 beacon_block_root(const uint8_t* ssz, size_t len, int32_t fork, bool blinded = false, Hash256* body_root = nullptr) {
     Hash256 out;
     const uint64_t offs[2] = {0, len};

@@ -144,6 +144,7 @@ _sig("lhb200_bls_batch_segment_gt", C.c_int32, vp, C.c_uint32, vp)
 _sig("lhb200_state_list_edit", C.c_int32, vp, vp, C.c_uint32, vp)
 _sig("lhb200_state_list_len", C.c_int32, vp, C.c_uint32, C.POINTER(C.c_uint64))
 _sig("lhb200_state_set_payload_header", C.c_int32, vp, vp, C.c_uint64)
+_sig("lhb200_state_set_pending_attestations", C.c_int32, vp, C.c_uint32, vp, C.c_uint64)
 _sig("lhb200_state_clone", C.c_int32, vp, C.POINTER(vp))
 _sig("lhb200_state_device_bytes", C.c_int32, vp, C.POINTER(C.c_uint64))
 _sig("lhb200_debug_state_disjoint", C.c_int32, vp, vp, C.POINTER(C.c_int32))

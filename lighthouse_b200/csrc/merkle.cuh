@@ -197,6 +197,109 @@ __global__ void __launch_bounds__(128) k_record_roots(const uint8_t* __restrict_
 }
 
 // ---------------------------------------------------------------------------------------------
+// Phase0 PendingAttestation (pending_attestation.rs:25-32): {aggregation_bits: Bitlist[2048] behind the offset at 0,
+// data: AttestationData (128 B at 4), inclusion_delay: u64 at 132, proposer_index: u64 at 140}, then the bitlist bytes.
+// A phase0 BeaconState holds two List[PendingAttestation, 4096] (fields 15 and 16).  k_pending_attestation_roots runs
+// one thread per slot of a 4096-slot root array per list, reading the records straight from the staged list bytes
+// through their offset table: slot i < n gets record i's root (19 hashes: 8 for the bitlist with its length, 8 for the
+// AttestationData, 3 for the record), slots n.. get zero chunks, so that the full 4096-leaf tree over the array is the
+// list's data root at every length.  The host has checked offsets, record sizes, delimiters and bit counts, and no patch
+// reaches a staged list; even so a record whose offsets do not frame 149 to 405 bytes inside the list gets a zero chunk,
+// so that no byte of a list can steer a read outside it.
+constexpr uint32_t PENDING_FIXED = 148, MAX_PENDING = 4096, PENDING_HASHES = 19;
+struct PendingSeg {
+    const uint8_t* in;   // the list's SSZ bytes: offset table, then the records
+    uint8_t* out;        // MAX_PENDING root chunks
+    uint64_t bytes;
+    uint32_t n;          // records
+};
+constexpr int MAX_PENDING_SEGS = 2;
+struct PendingTable {
+    int n;
+    PendingSeg s[MAX_PENDING_SEGS];
+};
+
+__device__ __forceinline__ uint32_t le_u32(const uint8_t* p) {
+    return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
+}
+// Chunk c of a bitlist's bits without its delimiter: the nb bytes at b, zero past them, the last byte's highest set
+// bit cleared.
+__device__ __forceinline__ void bitlist_chunk(const uint8_t* b, uint32_t nb, uint32_t c, uint32_t w[8]) {
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+        uint32_t x = 0;
+#pragma unroll
+        for (int q = 0; q < 4; q++) {
+            const uint32_t j = 32 * c + 4 * k + q;
+            uint32_t v = j < nb ? b[j] : 0;
+            if (j + 1 == nb && v) v &= ~(0x80000000u >> __clz(v));
+            x = (x << 8) | v;
+        }
+        w[k] = x;
+    }
+}
+// 8-byte little-endian field -> its chunk
+__device__ __forceinline__ void u64_chunk(const uint8_t* p, uint32_t w[8]) {
+#pragma unroll
+    for (int k = 0; k < 8; k++) w[k] = 0;
+    le64_words(p, w[0], w[1]);
+}
+__device__ __forceinline__ void h256_chunk(const uint8_t* p, uint32_t w[8]) {
+#pragma unroll
+    for (int k = 0; k < 8; k++) w[k] = be_word(p + 4 * k);
+}
+// hash_tree_root of the PendingAttestation of `len` bytes at r
+__device__ __forceinline__ void pending_attestation_root_words(const uint8_t* r, uint32_t len, uint32_t h[8]) {
+    uint32_t a[8], b[8], t[8];
+    // aggregation_bits: 8 chunks (2048 bits), then the bit count mixed in
+    const uint8_t* bits = r + PENDING_FIXED;
+    const uint32_t nb = len - PENDING_FIXED;
+    bitlist_chunk(bits, nb, 0, a); bitlist_chunk(bits, nb, 1, b); hash_pair(a, b, h);
+    bitlist_chunk(bits, nb, 2, a); bitlist_chunk(bits, nb, 3, b); hash_pair(a, b, a); hash_pair(h, a, h);
+    bitlist_chunk(bits, nb, 4, a); bitlist_chunk(bits, nb, 5, b); hash_pair(a, b, t);
+    bitlist_chunk(bits, nb, 6, a); bitlist_chunk(bits, nb, 7, b); hash_pair(a, b, a); hash_pair(t, a, t);
+    hash_pair(h, t, h);
+    const uint32_t last = bits[nb - 1];
+    const uint32_t n_bits = 8 * (nb - 1) + 31 - __clz(last);
+#pragma unroll
+    for (int k = 0; k < 8; k++) a[k] = 0;
+    a[0] = bswap32(n_bits);
+    hash_pair(h, a, h);
+    // AttestationData {slot, index, beacon_block_root, source, target}: 8 leaves
+    const uint8_t* d = r + 4;
+    u64_chunk(d, a); u64_chunk(d + 8, b); hash_pair(a, b, t);                        // H(slot, index)
+    u64_chunk(d + 48, a); h256_chunk(d + 56, b); hash_pair(a, b, b);                 // source
+    h256_chunk(d + 16, a); hash_pair(a, b, a);                                       // H(beacon_block_root, source)
+    hash_pair(t, a, t);
+    u64_chunk(d + 88, a); h256_chunk(d + 96, b); hash_pair(a, b, a);                 // target
+    hash_pair(a, g_zero_words[0], a);
+    hash_pair(a, g_zero_words[1], a);
+    hash_pair(t, a, t);
+    // the record: {aggregation_bits, data, inclusion_delay, proposer_index}
+    hash_pair(h, t, h);
+    u64_chunk(r + 132, a); u64_chunk(r + 140, b); hash_pair(a, b, a);
+    hash_pair(h, a, h);
+}
+
+__global__ void __launch_bounds__(128) k_pending_attestation_roots(const __grid_constant__ PendingTable tab) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t s = g / MAX_PENDING, i = g % MAX_PENDING;
+    if ((int)s >= tab.n) return;
+    const PendingSeg& seg = tab.s[s];
+    uint32_t h[8];
+    const uint64_t o0 = i < seg.n ? le_u32(seg.in + 4 * i) : 0;
+    const uint64_t o1 = i + 1 < seg.n ? le_u32(seg.in + 4 * i + 4) : seg.bytes;
+    if (i < seg.n && o0 >= 4ull * seg.n && o1 <= seg.bytes && o1 >= o0 + PENDING_FIXED + 1 &&
+        o1 - o0 <= PENDING_FIXED + 257) {
+        pending_attestation_root_words(seg.in + o0, (uint32_t)(o1 - o0), h);
+    } else {
+#pragma unroll
+        for (int k = 0; k < 8; k++) h[k] = 0;
+    }
+    store_chunk(seg.out + 32ull * i, h);
+}
+
+// ---------------------------------------------------------------------------------------------
 // Multi-segment tile reduce.
 struct MerkleSeg {
     const uint8_t* in;   // n_in chunks (32 B each, 16-B aligned); roots of height-`level_in` subtrees

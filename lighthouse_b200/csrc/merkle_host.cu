@@ -76,6 +76,7 @@ struct Plan {
     std::vector<uint8_t> lit;   // host literal block (32-byte chunks), copied to arena+lit_off
     size_t lit_off = 0, lit_cap = 0;
     std::vector<LeafLaunch> leaves;
+    std::vector<PendingSeg> pending;   // a phase0 state's two pending-attestation lists: one k_pending_attestation_roots
     std::vector<std::vector<MerkleSeg>> passes;
     std::vector<HashOp> ops;
     std::vector<int> op_wave;
@@ -231,6 +232,13 @@ struct Plan {
         for (uint32_t l = level; l < depth; l++) r = op_hash(r, zero_op(l));
         return r;
     }
+    // MAX_PENDING root chunks of the n PendingAttestations in `bytes` SSZ bytes at `in` (zero chunks past n)
+    uint8_t* pending_roots(const uint8_t* in, uint64_t bytes, uint32_t n) {
+        uint8_t* out = alloc(MAX_PENDING * 32);
+        pending.push_back({in, out, bytes, n});
+        hash_units += PENDING_HASHES * n;
+        return out;
+    }
     uint8_t* leaf_kernel(LeafKind kind, const uint8_t* in, uint64_t n) {
         uint8_t* out = alloc(std::max<uint64_t>(n, 1) * 32);
         if (n) leaves.push_back({kind, in, out, n});
@@ -254,6 +262,15 @@ static void enqueue_leaf_roots(uint32_t tree_kind, const uint8_t* in, uint64_t n
     count_launch();
 }
 // Leaf kernels, reduce passes and byte items of a plan: everything before its tail hash program.
+// Record roots of a phase0 state's pending-attestation lists: one launch for both.
+static void enqueue_pending_roots(const Plan& pl, cudaStream_t s) {
+    if (pl.pending.empty()) return;
+    PendingTable tab{};
+    tab.n = (int)pl.pending.size();
+    for (int k = 0; k < tab.n; k++) tab.s[k] = pl.pending[k];
+    k_pending_attestation_roots<<<(unsigned)(tab.n * MAX_PENDING / 128), 128, 0, s>>>(tab);
+    count_launch();
+}
 static void plan_enqueue_body(Plan& pl, cudaStream_t s, cudaEvent_t e0 = nullptr, cudaEvent_t e1 = nullptr) {
     for (const LeafLaunch& L : pl.leaves) {   // leaf_kernel is never called without a kernel
         if (L.kind.kernel == LeafKind::HASH_PAIRS) {
@@ -263,6 +280,7 @@ static void plan_enqueue_body(Plan& pl, cudaStream_t s, cudaEvent_t e0 = nullptr
             enqueue_leaf_roots(L.kind.tree, L.in, L.n, L.out, s, e0, e1);
         }
     }
+    enqueue_pending_roots(pl, s);
     for (auto& pass : pl.passes) {
         for (size_t i = 0; i < pass.size(); i += MAX_SEGS) {
             MerkleSegTable tab;
@@ -513,8 +531,10 @@ constexpr uint32_t PAYLOAD_PREFIX_FIELDS = 13;   // parent_hash .. block_hash: t
 constexpr uint32_t FIRST_VAR_POS[] = {0}, ATTESTER_SLASHING_VAR_POS[] = {0, 4};
 }  // namespace block_layout
 
-// One row per fork from Altair to Electra (beacon_state.rs:224-571, beacon_block_body.rs:43-121,
+// One row per fork from Base (phase0) to Electra (beacon_state.rs:224-571, beacon_block_body.rs:33-121,
 // execution_payload.rs:54-101, execution_payload_header.rs:46-93, attestation.rs:76-82; limits eth_spec.rs:389-440).
+// Base has Altair's fields 0-14 and 17-20 at the same offsets; its fields 15 and 16 are the pending-attestation lists
+// whose offsets sit where Altair's participation lists have theirs, and its body lacks sync_aggregate.
 struct ForkLayout {
     int state_fields, body_fields, payload_fields;   // payload_fields: also the header's; 0 before Bellatrix
     uint32_t state_fixed, header_fixed, body_fixed, payload_fixed, attestation_fixed;
@@ -523,6 +543,7 @@ struct ForkLayout {
 };
 constexpr ForkLayout FORK_LAYOUTS[] = {
     // fields: state, body, payload   fixed parts: state, header, body, payload, attestation   limits
+    {21,  8,  0, 2687377,   0, 220,   0, 228,   2048,   2048, 128, 2},   // Base
     {24,  9,  0, 2736629,   0, 380,   0, 228,   2048,   2048, 128, 2},   // Altair
     {25, 10, 14, 2736633, 536, 384, 508, 228,   2048,   2048, 128, 2},   // Bellatrix
     {28, 11, 15, 2736653, 568, 388, 512, 228,   2048,   2048, 128, 2},   // Capella
@@ -530,9 +551,9 @@ constexpr ForkLayout FORK_LAYOUTS[] = {
     {37, 13, 19, 2736713, 648, 396, 536, 236, 131072, 131072,   8, 1},   // Electra
 };
 static const ForkLayout* fork_layout(int32_t fork) {
-    return fork >= LHB200_FORK_ALTAIR && fork <= LHB200_FORK_ELECTRA ? &FORK_LAYOUTS[fork - LHB200_FORK_ALTAIR] : nullptr;
+    return fork >= LHB200_FORK_BASE && fork <= LHB200_FORK_ELECTRA ? &FORK_LAYOUTS[fork - LHB200_FORK_BASE] : nullptr;
 }
-constexpr int MAX_FIELDS = FORK_LAYOUTS[LHB200_FORK_ELECTRA - LHB200_FORK_ALTAIR].state_fields;   // the widest state
+constexpr int MAX_FIELDS = FORK_LAYOUTS[LHB200_FORK_ELECTRA - LHB200_FORK_BASE].state_fields;   // the widest state
 // chunk-tree depth of a packed list of at most `nbytes` bytes
 static inline uint32_t packed_depth(uint64_t nbytes) { return ceil_log2(ceil_div(nbytes, 32)); }
 
@@ -562,6 +583,29 @@ static bool read_offsets(const uint8_t* s, uint64_t len, uint32_t fixed, const u
     for (size_t k = 0; k < N; k++) span[k] = {at[k], at[k + 1] - at[k]};
     return true;
 }
+
+// A List[PendingAttestation, 4096] (pending_attestation.rs:25-32) of `len` bytes at s, as k_pending_attestation_roots
+// reads it: the first offset is 4 n with n <= 4096, offsets never decrease, each record is its 148-byte fixed part
+// (whose bitlist offset is 148) and a bitlist of at most 2048 bits with its delimiter.  Its record count goes to *n.
+static bool pending_list_ok(const uint8_t* s, uint64_t len, uint32_t* n) {
+    *n = 0;
+    if (len == 0) return true;
+    if (len < 4) return false;
+    const uint32_t first = rd32(s);
+    if (first % 4 || first == 0 || first > len || first / 4 > MAX_PENDING) return false;
+    const uint32_t cnt = first / 4;
+    for (uint32_t i = 0; i < cnt; i++) {
+        const uint64_t o0 = rd32(s + 4 * i), o1 = i + 1 < cnt ? rd32(s + 4 * i + 4) : len;
+        if (o1 > len || o1 < o0 + PENDING_FIXED + 1 || rd32(s + o0) != PENDING_FIXED) return false;
+        const uint64_t nb = o1 - o0 - PENDING_FIXED;
+        const uint8_t last = s[o1 - 1];
+        if (!last || 8 * (nb - 1) + (31 - __builtin_clz(last)) > 2048) return false;
+    }
+    *n = cnt;
+    return true;
+}
+// Bytes a pending-attestation list can take: 4096 offsets and 4096 records with full bitlists (2049 bits)
+constexpr uint64_t MAX_PENDING_BYTES = MAX_PENDING * (4ull + PENDING_FIXED + 257);
 
 }  // namespace lhb200
 
@@ -667,6 +711,12 @@ struct lhb200_state {
     std::vector<std::pair<uint32_t, uint32_t>> hdr_lits;   // payload header literals: (lit_src index, offset in header)
     int hdr_extra = -1;                  // lit_src index of extra_data
     uint32_t hdr_len_chunk = 0;          // literal chunk holding extra_data's length
+    // Base: the pending-attestation lists (fields 15, 16), each staged into MAX_PENDING_BYTES of arena and rooted over
+    // MAX_PENDING record-root chunks: their copies, the literal chunks holding their lengths, and whether
+    // lhb200_state_set_pending_attestations replaced one since the last root
+    int pending_copy[2] = {-1, -1};
+    uint32_t pending_len_chunk[2] = {0, 0};
+    bool pending_dirty = false;
 
     size_t trees_bytes() const { return trees.size() * sizeof(lhb200::TreeDev) + 256; }
     size_t dirty_bytes() const { return (size_t)DIRTY_CAP * 4 * trees.size(); }
@@ -764,6 +814,11 @@ static_assert(N_LIST_SPECS <= MAX_FINISH, "one finishing thread per list");
 static uint64_t list_leaves(const ListSpec& sp, uint64_t len) {
     return sp.leaf.tree == TREE_CHUNKS ? ceil_div(len * sp.item_bytes, 32) : len;
 }
+// Whether the state of `fork` has list `sp`: Base has fields 15 and 16, but they hold pending attestations
+static bool list_in_fork(const ListSpec& sp, int32_t fork) {
+    return (int)sp.field < fork_layout(fork)->state_fields &&
+           !(fork == LHB200_FORK_BASE && (sp.var == state_layout::V_PP || sp.var == state_layout::V_CP));
+}
 
 // Describe a whole BeaconState of any fork into `p` and the handle `st` (its copies, field and root operands, sharded
 // lists, marks and header literals).  `s` = host SSZ (read for offsets and small literal fields only).  Big fields
@@ -780,7 +835,10 @@ static int32_t describe_state(Plan& p, const uint8_t* s, uint64_t len, lhb200_st
         return LHB200_EINVAL;
     }
     bool fits = v[V_HIST].fits(32, 1u << 24);   // historical_roots: a list, but not a resizable one
-    for (const ListSpec& sp : LIST_SPECS) fits = fits && v[sp.var].fits(sp.item_bytes, sp.limit);
+    for (const ListSpec& sp : LIST_SPECS) fits = fits && (!list_in_fork(sp, sh.fork) || v[sp.var].fits(sp.item_bytes, sp.limit));
+    uint32_t n_pending[2] = {0, 0};
+    if (sh.fork == LHB200_FORK_BASE)
+        for (int q = 0; q < 2; q++) fits = fits && pending_list_ok(s + v[V_PP + q].off, v[V_PP + q].len, &n_pending[q]);
     if (!fits) {
         set_error("BeaconState SSZ: malformed variable part");
         return LHB200_EINVAL;
@@ -850,11 +908,23 @@ static int32_t describe_state(Plan& p, const uint8_t* s, uint64_t len, lhb200_st
         for (const auto& pass : p.passes) m.passes.push_back(pass.size());
         st->marks.push_back(std::move(m));
     };
+    // Base's pending-attestation lists: staged with room for the longest list, rooted over MAX_PENDING chunks (a tree
+    // the warm path keeps, addressed by no copy: a patch inside a list roots the state cold), length from a literal
+    auto pending_list = [&](int q) {
+        const Span x = v[V_PP + q];
+        uint8_t* d = p.alloc(align_up(MAX_PENDING_BYTES + 32, 256));
+        st->pending_copy[q] = (int)st->copies.size();
+        st->copies.push_back({x.off, x.len, d, align_up(MAX_PENDING_BYTES + 32, 256)});
+        const Plan::TreeSpec warm{nullptr, 0, 0, nullptr, LEAF_NONE, SIZE_MAX, 32};
+        const uint64_t r = p.merkle_list(p.pending_roots(d, x.len, n_pending[q]), MAX_PENDING, 12, &warm);
+        st->pending_len_chunk[q] = (uint32_t)(p.lit.size() / 32);   // the next literal: mix_in_length's length
+        return p.mix_in_length(r, n_pending[q]);
+    };
     const ListSpec* next_list = LIST_SPECS;   // in field order
     for (int k = 0; k < fl->state_fields; k++) {   // fields 24 on: appended by later forks (beacon_state.rs:339-525)
         mark();
-        if (next_list < LIST_SPECS + N_LIST_SPECS && (int)next_list->field == k) {
-            f[k] = list(*next_list++);
+        if (next_list < LIST_SPECS + N_LIST_SPECS && (int)next_list->field == k && list_in_fork(*next_list++, sh.fork)) {
+            f[k] = list(next_list[-1]);
             continue;
         }
         switch (k) {
@@ -872,6 +942,8 @@ static int32_t describe_state(Plan& p, const uint8_t* s, uint64_t len, lhb200_st
             case 10: f[k] = c.u64(O_DEPOSIT_INDEX); break;
             case 13: f[k] = big_list(13, O_RANDAO, 65536, 32, LEAF_NONE, 65536, 16, UINT64_MAX); break;
             case 14: f[k] = plain_vector(O_SLASHINGS, 8192 * 8, 11); break;
+            case 15:
+            case 16: f[k] = pending_list(k - 15); break;   // Base only: the other forks' fields 15, 16 are lists
             case 17: f[k] = p.literal_bytes(s + O_JUST, 1); break;
             case 18: f[k] = c.checkpoint(O_PJC); break;
             case 19: f[k] = c.checkpoint(O_CJC); break;
@@ -976,7 +1048,8 @@ static void index_resident(lhb200_state* st) {
         return ls[a].src_off != ls[b].src_off ? ls[a].src_off < ls[b].src_off : ls[a].n < ls[b].n;
     });
     st->copy_tree.assign(st->copies.size(), -1);
-    for (size_t t = 0; t < st->trees.size(); t++) st->copy_tree[st->trees[t].copy] = (int32_t)t;
+    for (size_t t = 0; t < st->trees.size(); t++)
+        if (st->trees[t].copy < st->copies.size()) st->copy_tree[st->trees[t].copy] = (int32_t)t;
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1436,7 +1509,7 @@ static int32_t stage_state(const uint8_t* ssz, uint64_t len, ShardCfg sh, lhb200
 int32_t lhb200_state_stage_deneb(const uint8_t* ssz, uint64_t len, lhb200_state** out) {
     return stage_state(ssz, len, ShardCfg(), out);
 }
-// Same for any post-Altair fork (LHB200_FORK_*): the describer is table-driven, the kernels are shared.
+// Same for any fork from Base on (LHB200_FORK_*): the describer is table-driven, the kernels are shared.
 int32_t lhb200_state_stage(const uint8_t* ssz, uint64_t len, int32_t fork, lhb200_state** out) {
     ShardCfg sh;
     sh.fork = fork;
@@ -1548,13 +1621,26 @@ int32_t lhb200_state_patch_batch(lhb200_state* st, const uint64_t* offsets, cons
     uint32_t lit_lo = ~0u, lit_hi = 0;
     // pass 1: every edit must hit resident bytes — validated BEFORE anything is modified, so a rejected batch leaves the
     // handle (host literals, dirty lists, device copy) exactly as it was
+    // A Base state's pending-attestation lists are refused: their offset tables and bitlists address the device reads
+    // of k_pending_attestation_roots, so they change only through lhb200_state_set_pending_attestations, which checks
+    // them first.
     auto stop = [](auto&&...) { return false; };
+    bool pending = false;
+    auto check_copy = [&](uint32_t ci, uint64_t, uint64_t) {
+        pending |= (int)ci == st->pending_copy[0] || (int)ci == st->pending_copy[1];
+        return !pending;
+    };
     size_t hint = ~(size_t)0;
     for (uint32_t i = 0; i < n; i++) {
         const uint64_t lo = offsets[i], hi = lo + lens[i];
-        if (lens[i] && !visit_resident(st, lo, hi, hint, stop, stop)) {
+        if (lens[i] && !visit_resident(st, lo, hi, hint, check_copy, stop)) {
             set_error("state_patch: range [%llu, %llu) is not resident on this handle (offset table or another rank's shard)",
                       (unsigned long long)lo, (unsigned long long)hi);
+            return LHB200_EINVAL;
+        }
+        if (pending) {
+            set_error("state_patch: range [%llu, %llu) lies in a pending-attestation list "
+                      "(lhb200_state_set_pending_attestations replaces those)", (unsigned long long)lo, (unsigned long long)hi);
             return LHB200_EINVAL;
         }
     }
@@ -1675,6 +1761,7 @@ static int32_t state_cold_enqueue(lhb200_state* st, cudaStream_t s) {
         if (rc) return rc;
     }
     st->last_root_hashes = st->plan.hash_units;
+    st->pending_dirty = false;   // the plan body has rooted every pending attestation
     return plan_enqueue_tail(st->plan, s);
 }
 
@@ -1703,6 +1790,11 @@ static int32_t state_incremental_enqueue(lhb200_state* st, cudaStream_t s) {
         total += (uint32_t)t.dirty.size();
     }
     uint64_t hashes = st->plan.ops.size();
+    if (st->pending_dirty) {   // a replaced pending-attestation list: every record root again, before the paths above
+        enqueue_pending_roots(st->plan, s);
+        for (const PendingSeg& sg : st->plan.pending) hashes += PENDING_HASHES * sg.n;
+        st->pending_dirty = false;
+    }
     FinishTable fin{};
     for (size_t k = 0; k < st->trees.size(); k++) {
         const lhb200_state::Tree& t = st->trees[k];
@@ -1812,9 +1904,8 @@ uint64_t lhb200_state_last_root_hashes(const lhb200_state* st) { return st ? st-
 
 // LIST_SPECS index of the resizable list `field` of the handle's fork, or -1
 static int list_spec_of(const lhb200_state* st, uint32_t field) {
-    const int n_fields = fork_layout(st->shard.fork)->state_fields;
     for (int k = 0; k < N_LIST_SPECS; k++)
-        if (LIST_SPECS[k].field == field && (int)field < n_fields) return k;
+        if (LIST_SPECS[k].field == field && list_in_fork(LIST_SPECS[k], st->shard.fork)) return k;
     return -1;
 }
 static lhb200_state::List& list_of(lhb200_state* st, int spec) {
@@ -1895,8 +1986,15 @@ static void state_relayout(lhb200_state* st) {
         st->copies[t.copy] = {off[sp.var], t.dev.length * sp.item_bytes, L.d_mem, 0};
         units += list_units(sp, t.dev.length);
     }
+    for (const PendingSeg& sg : st->plan.pending) units += PENDING_HASHES * sg.n;
     st->plan.hash_units = units;
     for (const auto& h : st->hdr_lits) st->plan.lit_src[h.first].src_off = off[V_LEPH] + h.second;
+    for (int q = 0; q < 2; q++)
+        if (st->pending_copy[q] >= 0) {
+            StageCopy& cp = st->copies[st->pending_copy[q]];
+            cp.src_off = off[V_PP + q];
+            cp.nbytes = st->var_len[V_PP + q];
+        }
     index_resident(st);
 }
 
@@ -1904,13 +2002,12 @@ static void state_relayout(lhb200_state* st) {
 // launches, reduce passes, tail ops and tree; st->marks) is dropped, and its staged copy moves to storage of its own,
 // where its tree is built on the device.
 static int32_t state_convert(lhb200_state* st, cudaStream_t s) {
-    const ForkLayout& fl = *fork_layout(st->shard.fork);
     Plan& pl = st->plan;
     auto cut = [](auto& v, size_t lo, size_t hi) { v.erase(v.begin() + lo, v.begin() + hi); };
     uint64_t stage_units = 0;
     for (int k = N_LIST_SPECS - 1; k >= 0; k--) {   // the last field first: earlier fields' marks stay valid
         const ListSpec& sp = LIST_SPECS[k];
-        if ((int)sp.field >= fl.state_fields) continue;
+        if (!list_in_fork(sp, st->shard.fork)) continue;
         const PlanMark &a = st->marks[sp.field], &b = st->marks[sp.field + 1];
         cut(pl.leaves, a.leaves, b.leaves);
         for (size_t q = 0; q < pl.passes.size(); q++) cut(pl.passes[q], a.pass(q), b.pass(q));
@@ -1931,11 +2028,12 @@ static int32_t state_convert(lhb200_state* st, cudaStream_t s) {
         LHB_CUDA(cudaMemcpyAsync(pl.d_ops, h, pl.ops.size() * sizeof(HashOp), cudaMemcpyHostToDevice, s));
         LHB_CUDA(cudaMemcpyAsync(pl.d_waves, h + nb, pl.h_waves.size() * 4, cudaMemcpyHostToDevice, s));
     }
+    for (const PendingSeg& sg : pl.pending) stage_units += PENDING_HASHES * sg.n;   // state_relayout counts the current records
     st->units_base = pl.hash_units - stage_units;
     // every list gets a resizable tree, seeded from the list's one staged copy, which then addresses its storage
     for (int k = 0; k < N_LIST_SPECS; k++) {
         const ListSpec& sp = LIST_SPECS[k];
-        if ((int)sp.field >= fl.state_fields) continue;
+        if (!list_in_fork(sp, st->shard.fork)) continue;
         const uint64_t len = st->var_len[sp.var] / sp.item_bytes;
         const bool packed = sp.leaf.tree == TREE_CHUNKS;
         lhb200_state::Tree t;
@@ -2072,6 +2170,10 @@ int32_t lhb200_state_list_edit(lhb200_state* st, const lhb200_list_edit* edits, 
 int32_t lhb200_state_list_len(const lhb200_state* st, uint32_t field, uint64_t* len) {
     LHB_REQUIRE_READY();
     if (!st || !len) return LHB200_EINVAL;
+    if (st->shard.fork == LHB200_FORK_BASE && (field == 15 || field == 16)) {   // pending attestations: records
+        *len = st->plan.pending[field - 15].n;
+        return LHB200_OK;
+    }
     const int k = list_spec_of(st, field);
     if (k < 0) { set_error("state_list_len: field %u is not a resizable list of this fork", field); return LHB200_EINVAL; }
     *len = st->var_len[LIST_SPECS[k].var] / LIST_SPECS[k].item_bytes;
@@ -2117,6 +2219,65 @@ int32_t lhb200_state_set_payload_header(lhb200_state* st, const uint8_t* ssz, ui
     st->var_len[state_layout::V_LEPH] = len;
     state_relayout(st);
     LHB_CUDA(cudaStreamSynchronize(c.stream));
+    return LHB200_OK;
+}
+
+// Base: the tree a pending-attestation list's record roots are the leaves of (incremental handles), or null
+static lhb200_state::Tree* pending_tree(lhb200_state* st, int q) {
+    for (lhb200_state::Tree& t : st->trees)
+        if (t.dev.lvl[0] == st->plan.pending[q].out) return &t;
+    return nullptr;
+}
+
+// A replacement writes the list's storage, its length literal and its length; the next root recomputes every record
+// root of both lists (one launch) and, on the warm path, re-hashes the list's tree above the slots that held or now
+// hold a record.
+int32_t lhb200_state_set_pending_attestations(lhb200_state* st, uint32_t field, const uint8_t* ssz, uint64_t len) {
+    LHB_REQUIRE_READY();
+    if (!st || (len && !ssz)) return LHB200_EINVAL;
+    Ctx& c = ctx();
+    std::lock_guard<std::recursive_mutex> g(c.mu);
+    int32_t rc = check_resizable(st, "state_set_pending_attestations");
+    if (rc) return rc;
+    if (st->shard.fork != LHB200_FORK_BASE || (field != 15 && field != 16)) {
+        set_error("state_set_pending_attestations: fields 15 and 16 of a Base state only (fork %d, field %u)", st->shard.fork,
+                  field);
+        return LHB200_EINVAL;
+    }
+    uint32_t n = 0;
+    if (len > MAX_PENDING_BYTES || !pending_list_ok(ssz, len, &n)) {
+        set_error("state_set_pending_attestations: malformed List[PendingAttestation, 4096] SSZ (%llu bytes)",
+                  (unsigned long long)len);
+        return LHB200_EINVAL;
+    }
+    if (!st->converted && (rc = state_convert(st, c.stream))) return rc;
+    const int q = (int)field - 15;
+    Plan& pl = st->plan;
+    PendingSeg& seg = pl.pending[q];
+    const uint32_t old = seg.n;
+    const size_t lb = align_up(len, 256);
+    uint8_t* h = static_cast<uint8_t*>(pinned_scratch(lb + 32));
+    if (!h) return LHB200_ENOMEM;
+    if (len) {
+        memcpy(h, ssz, len);
+        LHB_CUDA(cudaMemcpyAsync(st->copies[st->pending_copy[q]].dst, h, len, cudaMemcpyHostToDevice, c.stream));
+    }
+    uint8_t* lc = &pl.lit[(size_t)st->pending_len_chunk[q] * 32];
+    memset(lc, 0, 32);
+    for (int k = 0; k < 4; k++) lc[k] = (uint8_t)(n >> (8 * k));
+    memcpy(h + lb, lc, 32);
+    LHB_CUDA(cudaMemcpyAsync(pl.arena + pl.lit_off + (size_t)st->pending_len_chunk[q] * 32, h + lb, 32,
+                             cudaMemcpyHostToDevice, c.stream));
+    seg.bytes = len;
+    seg.n = n;
+    st->var_len[state_layout::V_PP + q] = len;
+    st->pending_dirty = true;
+    const uint32_t hi = std::max(old, n);
+    lhb200_state::Tree* t = pending_tree(st, q);
+    if (!t || t->n_marks + hi > 4ull * lhb200_state::DIRTY_CAP) st->need_full = true;
+    else if (!st->need_full) for (uint32_t i = 0; i < hi; i++) t->mark(i);
+    state_relayout(st);
+    LHB_CUDA(cudaStreamSynchronize(c.stream));   // the staging slab is reused by the next call
     return LHB200_OK;
 }
 
@@ -2246,6 +2407,7 @@ static void visit_device_addresses(lhb200_state* st, F&& f) {
     Plan& pl = st->plan;
     at(pl.arena);
     for (LeafLaunch& L : pl.leaves) { at(L.in); at(L.out); }
+    for (PendingSeg& sg : pl.pending) { at(sg.in); at(sg.out); }
     for (auto& pass : pl.passes)
         for (MerkleSeg& sg : pass) { at(sg.in); at(sg.out); }
     for (HashOp& op : pl.ops) { f(op.dst, 0); f(op.a, 0); f(op.b, 0); }
@@ -2431,7 +2593,7 @@ float lhb200_state_dominant_kernel_ms(const lhb200_state* st) {
 int32_t lhb200_beacon_state_root_deneb(const uint8_t* ssz, uint64_t len, uint8_t out[32], uint8_t* field_roots) {
     return lhb200_beacon_state_root(ssz, len, LHB200_FORK_DENEB, out, field_roots);
 }
-// BeaconState::update_tree_hash_cache for any post-Altair variant of the superstruct (beacon_state.rs:224-571).
+// BeaconState::update_tree_hash_cache for any variant of the superstruct from Base on (beacon_state.rs:224-571).
 // field_roots (optional): 28 x 32 bytes (entries beyond the fork's field count are the zero chunk); 37 x 32 for Electra.
 int32_t lhb200_beacon_state_root(const uint8_t* ssz, uint64_t len, int32_t fork, uint8_t out[32], uint8_t* field_roots) {
     LHB_REQUIRE_READY();
@@ -2536,7 +2698,7 @@ int32_t lhb200_verify_merkle_proofs(const uint8_t* leaves, const uint8_t* branch
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// BeaconBlock (mainnet preset) of any fork from Altair to Electra: BeaconBlock::canonical_root
+// BeaconBlock (mainnet preset) of any fork from Base to Electra: BeaconBlock::canonical_root
 // (consensus/types/src/beacon_block.rs:158-160).  Layouts: beacon_block.rs:41-90, beacon_block_body.rs:43-121,
 // execution_payload.rs:54-101, sizes and limits per fork in FORK_LAYOUTS; operation containers as cited in
 // include/lhb200.h.  The host only walks SSZ offsets: every packed byte string (transactions, signatures, pubkeys,
@@ -2671,7 +2833,7 @@ struct BlockDescriber : SszDescriber {
         using namespace block_layout;
         Span v[N_BODY_VAR];
         if (!read_offsets(s + off, len, fl.body_fixed, BODY_VAR_POS, v)) return fail();
-        std::vector<uint64_t> f(9), b, roots;
+        std::vector<uint64_t> f(8), b, roots;
         f[0] = sig(off);
         f[1] = eth1_data(off + 96);
         f[2] = h256(off + 168);
@@ -2696,7 +2858,7 @@ struct BlockDescriber : SszDescriber {
         f[5] = list_of(roots, ceil_log2(fl.max_attestations));
         f[6] = fixed_list(off, v[B_DEPOSITS], 1240, 4, [&](uint64_t o) { return deposit(o); });
         f[7] = fixed_list(off, v[B_EXITS], 112, 4, [&](uint64_t o) { return voluntary_exit(o); });
-        f[8] = p.op_hash(blob(off + 220, 64, 1), sig(off + 284));  // sync_aggregate.rs:38
+        if (fl.body_fields > 8) f.push_back(p.op_hash(blob(off + 220, 64, 1), sig(off + 284)));  // sync_aggregate.rs:38
         for (int k = 9; k < fl.body_fields && !bad; k++) {   // appended by later forks
             const Span x = v[B_PAYLOAD + (k - 9)];
             switch (k) {
@@ -2827,7 +2989,7 @@ static int32_t block_roots(const uint8_t* ssz, const uint64_t* offsets, uint32_t
     LHB_REQUIRE_READY();
     const ForkLayout* fl = fork_layout(fork);
     if (!fl || (blinded && !fl->payload_fields)) {
-        set_error("beacon_block_roots: fork id %d not supported (Altair .. Electra; blinded blocks from Bellatrix)", fork);
+        set_error("beacon_block_roots: fork id %d not supported (Base .. Electra; blinded blocks from Bellatrix)", fork);
         return LHB200_EINVAL;
     }
     if (!ssz || !offsets || !roots || n == 0) { set_error("beacon_block_roots: null argument or zero blocks"); return LHB200_EINVAL; }
@@ -2871,8 +3033,8 @@ int32_t lhb200_beacon_block_root_deneb(const uint8_t* ssz, uint64_t len, uint8_t
     const uint64_t offs[2] = {0, len};
     return block_roots(ssz, offs, 1, out, body_root, false);
 }
-// The variants of the BeaconBlock superstruct from Altair on (beacon_block.rs:41-90, beacon_block_body.rs:43-121): fork is
-// LHB200_FORK_ALTAIR .. LHB200_FORK_ELECTRA; blinded != 0 selects the BlindedBeaconBlock form (Bellatrix and later).
+// The variants of the BeaconBlock superstruct from Base on (beacon_block.rs:19-90, beacon_block_body.rs:33-121): fork is
+// LHB200_FORK_BASE .. LHB200_FORK_ELECTRA; blinded != 0 selects the BlindedBeaconBlock form (Bellatrix and later).
 int32_t lhb200_beacon_block_roots(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, int32_t fork, int32_t blinded,
                                   uint8_t* roots, uint8_t* body_roots) {
     return block_roots(ssz, offsets, n, roots, body_roots, blinded != 0, fork);

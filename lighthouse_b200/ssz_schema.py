@@ -177,7 +177,13 @@ BeaconStateElectra = C(*(_f[:24] + [("latest_execution_payload_header", Executio
     ("pending_balance_deposits", ("list", PendingBalanceDeposit, 1 << 27)),
     ("pending_partial_withdrawals", ("list", PendingPartialWithdrawal, 1 << 27)),
     ("pending_consolidations", ("list", PendingConsolidation, 1 << 18))]))
-BEACON_STATE_BY_FORK = {"altair": BeaconStateAltair, "bellatrix": BeaconStateBellatrix, "capella": BeaconStateCapella,
+# ---- Base (phase0: beacon_state.rs:225-406 Base fields, pending_attestation.rs:25-32; limits eth_spec.rs:389-430):
+# Altair's first 21 fields with the participation lists replaced by pending-attestation lists
+PendingAttestation = C(("aggregation_bits", ("bitlist", 2048)), ("data", AttestationData), ("inclusion_delay", U64),
+                       ("proposer_index", U64))
+BeaconStateBase = C(*(_f[:15] + [("previous_epoch_attestations", ("list", PendingAttestation, 4096)),
+                                 ("current_epoch_attestations", ("list", PendingAttestation, 4096))] + _f[17:21]))
+BEACON_STATE_BY_FORK = {"base": BeaconStateBase, "altair": BeaconStateAltair, "bellatrix": BeaconStateBellatrix, "capella": BeaconStateCapella,
                         "deneb": BeaconStateDeneb, "electra": BeaconStateElectra}
 
 
@@ -189,6 +195,7 @@ def _block_of(body):
 _pf, _bf = ExecutionPayloadDeneb[1], BeaconBlockBodyDeneb[1]
 ExecutionPayloadBellatrix = C(*_pf[:14])
 ExecutionPayloadCapella = C(*_pf[:15])
+BeaconBlockBodyBase = C(*_bf[:8])   # beacon_block_body.rs:33-119: no sync_aggregate
 BeaconBlockBodyAltair = C(*_bf[:9])
 BeaconBlockBodyBellatrix = C(*(_bf[:9] + [("execution_payload", ExecutionPayloadBellatrix)]))
 BeaconBlockBodyCapella = C(*(_bf[:9] + [("execution_payload", ExecutionPayloadCapella)] + _bf[10:11]))
@@ -210,17 +217,18 @@ _electra_body = {"attester_slashings": ("list", AttesterSlashingElectra, 1), "at
                  "execution_payload": ExecutionPayloadElectra}
 BeaconBlockBodyElectra = C(*([(n, _electra_body.get(n, t)) for n, t in _bf] +
                              [("consolidations", ("list", SignedConsolidation, 1))]))
-BEACON_BLOCK_BODY_BY_FORK = {"altair": BeaconBlockBodyAltair, "bellatrix": BeaconBlockBodyBellatrix,
+BEACON_BLOCK_BODY_BY_FORK = {"base": BeaconBlockBodyBase, "altair": BeaconBlockBodyAltair, "bellatrix": BeaconBlockBodyBellatrix,
                              "capella": BeaconBlockBodyCapella, "deneb": BeaconBlockBodyDeneb,
                              "electra": BeaconBlockBodyElectra}
 BEACON_BLOCK_BY_FORK = {k: _block_of(v) for k, v in BEACON_BLOCK_BODY_BY_FORK.items()}
+BeaconBlockBase = BEACON_BLOCK_BY_FORK["base"]
 EXECUTION_PAYLOAD_BY_FORK = {"bellatrix": ExecutionPayloadBellatrix, "capella": ExecutionPayloadCapella,
                              "deneb": ExecutionPayloadDeneb, "electra": ExecutionPayloadElectra}
 EXECUTION_PAYLOAD_HEADER_BY_FORK = {"bellatrix": ExecutionPayloadHeaderBellatrix, "capella": ExecutionPayloadHeaderCapella,
                                     "deneb": ExecutionPayloadHeaderDeneb, "electra": ExecutionPayloadHeaderElectra}
 BLINDED_BEACON_BLOCK_BODY_BY_FORK = {
     f: C(*[(n, EXECUTION_PAYLOAD_HEADER_BY_FORK[f]) if n == "execution_payload" else (n, t) for n, t in b[1]])
-    for f, b in BEACON_BLOCK_BODY_BY_FORK.items() if f != "altair"}
+    for f, b in BEACON_BLOCK_BODY_BY_FORK.items() if f not in ("base", "altair")}
 BLINDED_BEACON_BLOCK_BY_FORK = {k: _block_of(v) for k, v in BLINDED_BEACON_BLOCK_BODY_BY_FORK.items()}
 
 # BlindedBeaconBlock (beacon_block.rs:80; payload.rs BlindedPayload): the body carries the payload HEADER

@@ -5,7 +5,9 @@ import struct
 import numpy as np
 
 DENEB_FIXED = 2736653
+BASE_FIXED = 2687377
 U64_MAX = (1 << 64) - 1
+PENDING_BIT_LENGTHS = (0, 1, 255, 256, 257, 2048)
 
 
 def validators_ssz(n, rng, pubkeys=None):
@@ -24,13 +26,43 @@ def validators_ssz(n, rng, pubkeys=None):
     return v.tobytes()
 
 
+def pending_attestation_ssz(rng, n_bits, slot=0):
+    """One phase0 PendingAttestation (pending_attestation.rs:25-32) with n_bits seeded aggregation bits: its 148-byte
+    fixed part (bitlist offset, AttestationData, inclusion_delay, proposer_index), then the bitlist with its delimiter."""
+    bits = np.append(rng.integers(0, 2, size=n_bits).astype(np.uint8), np.uint8(1))
+    data = (struct.pack("<QQ", slot, int(rng.integers(0, 64))) + rng.integers(0, 256, size=32, dtype=np.uint8).tobytes()
+            + struct.pack("<Q", int(rng.integers(0, 1 << 40))) + rng.integers(0, 256, size=32, dtype=np.uint8).tobytes()
+            + struct.pack("<Q", int(rng.integers(0, 1 << 40))) + rng.integers(0, 256, size=32, dtype=np.uint8).tobytes())
+    tail = struct.pack("<QQ", int(rng.integers(1, 33)), int(rng.integers(0, 1 << 20)))
+    return struct.pack("<I", 148) + data + tail + np.packbits(bits, bitorder="little").tobytes()
+
+
+def pending_attestations_list_ssz(records):
+    """SSZ of a List[PendingAttestation, 4096] from its records' SSZ: the offset table, then the records."""
+    out, at = [], 4 * len(records)
+    for r in records:
+        out.append(struct.pack("<I", at))
+        at += len(r)
+    return b"".join(out + list(records))
+
+
+def pending_attestations_ssz(n, rng, bit_lengths=PENDING_BIT_LENGTHS, slot=0):
+    """n seeded PendingAttestations, record i with bit_lengths[i % len(bit_lengths)] aggregation bits, as a list."""
+    return pending_attestations_list_ssz([pending_attestation_ssz(rng, bit_lengths[i % len(bit_lengths)], slot)
+                                          for i in range(n)])
+
+
 def beacon_state_deneb_ssz(n_validators, seed=1, all_default=False, n_hist_roots=758, n_votes=1024,
-                           n_summaries=600, extra_data_len=14, fork="deneb", n_pending=(700, 333, 45)):
-    """SSZ(BeaconState<fork>), mainnet preset; fork in altair / bellatrix / capella / deneb / electra
+                           n_summaries=600, extra_data_len=14, fork="deneb", n_pending=(700, 333, 45),
+                           n_pending_attestations=(128, 64), pending_bit_lengths=PENDING_BIT_LENGTHS):
+    """SSZ(BeaconState<fork>), mainnet preset; fork in base / altair / bellatrix / capella / deneb / electra
     (beacon_state.rs:224-571: later forks append fields and widen the execution payload header; n_pending = lengths of
-    Electra's pending_balance_deposits / pending_partial_withdrawals / pending_consolidations).  all_default=True leaves
-    every non-validator field zero so the ZERO_HASHES ladder paths are exercised."""
-    hdr_fixed = {"altair": 0, "bellatrix": 536, "capella": 568, "deneb": 584, "electra": 648}[fork]
+    Electra's pending_balance_deposits / pending_partial_withdrawals / pending_consolidations).  Base (phase0) has
+    Altair's first 21 fields with previous_ / current_epoch_attestations (n_pending_attestations records, with
+    pending_bit_lengths aggregation bits in turn) in place of the participation lists.  all_default=True leaves every
+    non-validator field zero so the ZERO_HASHES ladder paths are exercised."""
+    base = fork == "base"
+    hdr_fixed = {"base": 0, "altair": 0, "bellatrix": 536, "capella": 568, "deneb": 584, "electra": 648}[fork]
     has_tail = fork in ("capella", "deneb", "electra")
     electra = fork == "electra"
     rng = np.random.default_rng(seed)
@@ -44,6 +76,7 @@ def beacon_state_deneb_ssz(n_validators, seed=1, all_default=False, n_hist_roots
     if all_default:
         n_hist_roots = n_votes = n_summaries = extra_data_len = 0
         n_pending = (0, 0, 0)
+        n_pending_attestations = (0, 0)
     hist = rnd(32 * n_hist_roots)
     votes = rnd(72 * n_votes)
     vals = validators_ssz(V, rng)
@@ -65,6 +98,10 @@ def beacon_state_deneb_ssz(n_validators, seed=1, all_default=False, n_hist_roots
     summ = rnd(64 * n_summaries) if has_tail else b""
     pend = [rnd(sz * n) if electra else b"" for sz, n in zip((16, 24, 16), n_pending)]
     fixed_len = DENEB_FIXED - (0 if has_tail else 20) - (0 if hdr_fixed else 4) + (60 if electra else 0)
+    if base:   # the pending-attestation lists take the participation lists' places; nothing after the checkpoints
+        pp, cp = (pending_attestations_ssz(n, rng, pending_bit_lengths) for n in n_pending_attestations)
+        inact = b""
+        fixed_len = BASE_FIXED
 
     o_hist = fixed_len
     o_votes = o_hist + len(hist)
@@ -90,12 +127,15 @@ def beacon_state_deneb_ssz(n_validators, seed=1, all_default=False, n_hist_roots
         u32(o_pp), u32(o_cp),
         bytes([0 if all_default else 0x0B]),           # justification_bits
         rnd(40), rnd(40), rnd(40),                     # checkpoints
-        u32(o_inact),
-        (vals[:48] * 1 if False else rnd(513 * 48)),   # current_sync_committee (512 pubkeys + aggregate)
-        rnd(513 * 48),                                 # next_sync_committee
-        (u32(o_leph) if hdr_fixed else b""), ((rnd(8) + rnd(8) + u32(o_hs)) if has_tail else b""),
-        ((rnd(48) + u32(o_pbd) + u32(o_ppw) + u32(o_pc)) if electra else b""),   # six u64s, three list offsets
     ])
+    if not base:   # Altair on: inactivity scores, sync committees, then what later forks append
+        fixed += b"".join([
+            u32(o_inact),
+            (vals[:48] * 1 if False else rnd(513 * 48)),   # current_sync_committee (512 pubkeys + aggregate)
+            rnd(513 * 48),                                 # next_sync_committee
+            (u32(o_leph) if hdr_fixed else b""), ((rnd(8) + rnd(8) + u32(o_hs)) if has_tail else b""),
+            ((rnd(48) + u32(o_pbd) + u32(o_ppw) + u32(o_pc)) if electra else b""),   # six u64s, three list offsets
+        ])
     assert len(fixed) == fixed_len, len(fixed)
     return b"".join([fixed, hist, votes, vals, bal, pp, cp, inact, leph, summ] + pend)
 
@@ -252,8 +292,9 @@ def block_signature_key_counts(n_blocks=32, n_validators=524288):
 def beacon_block_deneb(seed=1, n_attestations=128, n_transactions=150, n_proposer_slashings=1,
                        n_attester_slashings=1, n_deposits=2, n_exits=3, n_bls_changes=4, n_withdrawals=16,
                        n_blobs=6, tx_sizes=None, committee=244, extra_data_len=13, fork="deneb"):
-    """-> (value, ssz_bytes) of a BeaconBlock<fork> (altair / bellatrix / capella / deneb: the later forks' fields are
-    dropped, beacon_block_body.rs:43-110) filled with seeded pseudo-random content of mainnet shape."""
+    """-> (value, ssz_bytes) of a BeaconBlock<fork> (base / altair / bellatrix / capella / deneb: the later forks' fields
+    are dropped, beacon_block_body.rs:33-110; Base has no sync_aggregate) filled with seeded pseudo-random content of
+    mainnet shape."""
     from . import ssz_schema as S
     rng = np.random.default_rng(seed)
 
@@ -317,7 +358,7 @@ def beacon_block_deneb(seed=1, n_attestations=128, n_transactions=150, n_propose
              "body": body}
     if fork != "deneb":
         body_t = S.BEACON_BLOCK_BODY_BY_FORK[fork]
-        if fork != "altair":
+        if fork not in ("base", "altair"):
             pt = S.EXECUTION_PAYLOAD_BY_FORK[fork]
             body["execution_payload"] = {n: payload[n] for n, _ in pt[1]}
         block["body"] = {n: body[n] for n, _ in body_t[1]}

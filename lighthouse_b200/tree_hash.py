@@ -104,7 +104,7 @@ def validator_roots(ssz: bytes) -> bytes:
     return out.raw[: 32 * n]
 
 
-FORKS = {"altair": 1, "bellatrix": 2, "capella": 3, "deneb": 4, "electra": 5}   # LHB200_FORK_*
+FORKS = {"base": 0, "altair": 1, "bellatrix": 2, "capella": 3, "deneb": 4, "electra": 5}   # LHB200_FORK_*
 
 
 def _n_field_roots(fork):
@@ -119,7 +119,7 @@ def beacon_state_root_deneb(ssz, want_field_roots=False):
 
 
 def beacon_state_root(ssz, fork="deneb", want_field_roots=False):
-    """BeaconState::update_tree_hash_cache (cold) for any post-Altair variant of the superstruct
+    """BeaconState::update_tree_hash_cache (cold) for any variant of the superstruct from Base (phase0) on
     (consensus/types/src/beacon_state.rs:224-571): lhb200_beacon_state_root."""
     out = C.create_string_buffer(32)
     n_fr = _n_field_roots(fork)
@@ -139,8 +139,8 @@ def beacon_block_roots_deneb(blocks, want_body_roots=False, blinded=False):
 
 
 def beacon_block_roots(blocks, fork="deneb", want_body_roots=False, blinded=False):
-    """canonical_root of a batch of BeaconBlock<fork> (or BlindedBeaconBlock<fork>) SSZ blobs, fork in altair / bellatrix /
-    capella / deneb / electra (beacon_block.rs:41-90): lhb200_beacon_block_roots."""
+    """canonical_root of a batch of BeaconBlock<fork> (or BlindedBeaconBlock<fork>) SSZ blobs, fork in base / altair /
+    bellatrix / capella / deneb / electra (beacon_block.rs:19-90; no blinded Base form): lhb200_beacon_block_roots."""
     blocks = [bytes(b) for b in blocks]
     n = len(blocks)
     offs = (C.c_uint64 * (n + 1))()
@@ -265,8 +265,8 @@ class ShardedState:
 
 
 class ResidentState:
-    """A BeaconState staged once into HBM (DESIGN.md §3) and hashed from there.  `fork` in altair / bellatrix / capella /
-    deneb / electra; Deneb stages through lhb200_state_stage_deneb, the others through lhb200_state_stage."""
+    """A BeaconState staged once into HBM (DESIGN.md §3) and hashed from there.  `fork` in base / altair / bellatrix /
+    capella / deneb / electra; Deneb stages through lhb200_state_stage_deneb, the others through lhb200_state_stage."""
 
     def __init__(self, ssz, fork="deneb"):
         self._h = C.c_void_p()
@@ -353,6 +353,14 @@ class ResidentState:
         """Replace latest_execution_payload_header with SSZ of this fork's header (extra_data may change length)."""
         p, keep = buf(ssz)
         check(lib.lhb200_state_set_payload_header(self._h, p, len(ssz)), "lhb200_state_set_payload_header")
+
+    def set_pending_attestations(self, name, ssz):
+        """Base: replace previous_epoch_attestations or current_epoch_attestations (by name or field index 15 / 16)
+        with the SSZ of a List[PendingAttestation, 4096] (lhb200_state_set_pending_attestations).  A block appends to
+        the current list; the epoch rotation is two calls.  Needs enable_incremental()."""
+        idx = name if isinstance(name, int) else {"previous_epoch_attestations": 15, "current_epoch_attestations": 16}[name]
+        p, keep = buf(ssz)
+        check(lib.lhb200_state_set_pending_attestations(self._h, idx, p, len(ssz)), "lhb200_state_set_pending_attestations")
 
     def clone(self):
         """BeaconState::clone on the device (lhb200_state_clone): a new handle of the same fork whose device memory is
