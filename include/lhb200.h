@@ -260,6 +260,29 @@ LHB200_API int32_t lhb200_beacon_block_roots(const uint8_t* ssz, const uint64_t*
 LHB200_API int32_t lhb200_shuffle_list(const uint64_t* input, uint64_t n, uint8_t rounds, const uint8_t seed[32],
                                        int32_t forwards, uint64_t* out);
 
+/* Committees, proposers and the next sync committee of a resident, unsharded BeaconState of any fork (mainnet preset,
+ * reference semantics for every fork from Base to Electra).  They read the handle's validator records, randao_mixes
+ * and slot on the device, as patches, list edits and clones left them, and change nothing a later root, clone or
+ * proof sees.  Refusals -> LHB200_EINVAL with lhb200_last_error set: a sharded handle, a cap below the validator
+ * count, an epoch out of bounds (checked before anything is launched); no validator active at the epoch, or more
+ * than 2^24 active (found by the counting pass, which writes only library scratch).  Each call makes a fixed number
+ * of launches and one synchronise before its final copy. */
+typedef struct {
+    uint64_t epoch, n_validators, n_active, committees_per_slot;
+    uint8_t seed[32];                       /* get_seed(epoch, DOMAIN_BEACON_ATTESTER) */
+} lhb200_committee_info;
+/* CommitteeCache::initialized(state, epoch) (committee_cache.rs:64-125): shuffling[0..n_active) = shuffle_list(active
+ * indices, 90, seed, forwards = false); positions[0..n_validators) (0 = None, else position + 1; may be NULL).  cap =
+ * entries each buffer holds, at least the handle's validator count.  The epoch is out of bounds when epoch - 2 (saturating)
+ * is below min_randao_epoch = current_epoch + 1 - 65536 (saturating), or when it is above current_epoch + 1. */
+LHB200_API int32_t lhb200_state_committee_cache(lhb200_state* st, uint64_t epoch, uint64_t* shuffling,
+                                               uint32_t* positions, uint64_t cap, lhb200_committee_info* info);
+/* get_beacon_proposer_indices (beacon_state.rs:1025-1037): the proposer of each slot of the current epoch. */
+LHB200_API int32_t lhb200_state_beacon_proposer_indices(lhb200_state* st, uint64_t out[32]);
+/* get_next_sync_committee_indices (beacon_state.rs:1091-1125): 512 indices drawn at current_epoch + 1, duplicates
+ * kept. */
+LHB200_API int32_t lhb200_state_next_sync_committee_indices(lhb200_state* st, uint64_t out[512]);
+
 /* ---- BLS batch verification path ---------------------------------------------------------------- */
 
 /* bls::verify_signature_sets (crypto/bls/src/impls/blst.rs:37-119) over SoA-flattened SignatureSets

@@ -152,9 +152,18 @@ _sig("lhb200_debug_state_live_bytes", C.c_int32, vp, C.POINTER(C.c_uint64))
 _sig("lhb200_state_proofs", C.c_int32, vp, vp, C.c_uint32, vp, vp)
 _sig("lhb200_beacon_block_body_proofs", C.c_int32, vp, vp, C.c_uint32, C.c_int32, C.c_int32, vp, vp, C.c_uint32, vp, vp)
 _sig("lhb200_debug_proof_gather_ms", C.c_float)
+_sig("lhb200_state_committee_cache", C.c_int32, vp, C.c_uint64, vp, vp, C.c_uint64, vp)
+_sig("lhb200_state_beacon_proposer_indices", C.c_int32, vp, vp)
+_sig("lhb200_state_next_sync_committee_indices", C.c_int32, vp, vp)
 
 
 class ListEdit(C.Structure):
     """struct lhb200_list_edit"""
     _fields_ = [("field", C.c_uint32), ("reserved", C.c_uint32), ("new_len", C.c_uint64), ("first", C.c_uint64),
                 ("n", C.c_uint64)]
+
+
+class CommitteeInfo(C.Structure):
+    """lhb200_committee_info"""
+    _fields_ = [("epoch", C.c_uint64), ("n_validators", C.c_uint64), ("n_active", C.c_uint64),
+                ("committees_per_slot", C.c_uint64), ("seed", C.c_uint8 * 32)]

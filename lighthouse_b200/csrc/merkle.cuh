@@ -868,4 +868,227 @@ __global__ void __launch_bounds__(256) k_shuffle_permute(const uint64_t* __restr
     else out[i] = in[index];
 }
 
+// ---------------------------------------------------------------------------------------------
+// Committees, proposers and the next sync committee from a resident BeaconState (lhb200_state_committee_cache,
+// lhb200_state_beacon_proposer_indices, lhb200_state_next_sync_committee_indices): CommitteeCache::initialized
+// (committee_cache.rs:64-125), compute_proposer_index (beacon_state.rs:890-936) and get_next_sync_committee_indices
+// (:1091-1125).  The inputs are the handle's own device bytes: its 121-byte validator records and randao_mixes.
+constexpr uint32_t SHUFFLE_ROUND_COUNT = 90;
+constexpr uint64_t MAX_EFFECTIVE_BALANCE = 32000000000ull, MAX_RANDOM_BYTE = 255;
+constexpr uint32_t VAL_EFFECTIVE_BALANCE = 80, VAL_ACTIVATION_EPOCH = 97, VAL_EXIT_EPOCH = 105;
+
+// SHA-256 of a message of at most 55 bytes, given as its one padded block of big-endian words (w is clobbered)
+__device__ __forceinline__ void sha256_one_block(uint32_t w[16], uint32_t st[8]) {
+    sha256_init(st);
+    sha256_compress(st, w);
+}
+// byte k (0..31) of a digest in word form: a tree of selects on the bits of k >> 2, so that no register array is
+// indexed at run time (which would put the digest in local memory)
+__device__ __forceinline__ uint32_t digest_byte(const uint32_t st[8], uint32_t k) {
+    const bool b0 = k & 4, b1 = k & 8, b2 = k & 16;
+    const uint32_t a0 = b0 ? st[1] : st[0], a1 = b0 ? st[3] : st[2], a2 = b0 ? st[5] : st[4], a3 = b0 ? st[7] : st[6];
+    const uint32_t w = b2 ? (b1 ? a3 : a2) : (b1 ? a1 : a0);
+    return (w >> (24 - 8 * (k & 3))) & 0xff;
+}
+// little-endian u64 at any byte address: funnel shifts over the three aligned words that cover it (the record fields
+// read here end at least 3 bytes before their record does, so no read leaves the record)
+__device__ __forceinline__ uint64_t le64_at(const uint8_t* p) {
+    const uintptr_t a = reinterpret_cast<uintptr_t>(p);
+    const uint32_t* q = reinterpret_cast<const uint32_t*>(a & ~uintptr_t(3));
+    const uint32_t sh = 8 * (uint32_t)(a & 3), w0 = q[0], w1 = q[1], w2 = q[2];
+    return (uint64_t)__funnelshift_r(w0, w1, sh) | ((uint64_t)__funnelshift_r(w1, w2, sh) << 32);
+}
+// Validator::is_active_at (validator.rs:39-41)
+__device__ __forceinline__ bool validator_active_at(const uint8_t* v, uint64_t epoch) {
+    return le64_at(v + VAL_ACTIVATION_EPOCH) <= epoch && epoch < le64_at(v + VAL_EXIT_EPOCH);
+}
+
+// Ordered active-index compaction (get_active_validator_indices, committee_cache.rs:356-373) in two passes over tiles
+// of ACTIVE_TILE records: k_active_count counts each tile's active validators, k_active_write adds up the counts of the
+// tiles before its own and writes its tile's indices in ascending order, one 256-record step at a time (a warp ballot
+// and the warp counts give each active record its slot).  Both read records at one thread per record, so a warp's
+// loads cover 32 consecutive records.
+constexpr int ACTIVE_THREADS = 256, ACTIVE_STEPS = 16, ACTIVE_TILE = ACTIVE_THREADS * ACTIVE_STEPS;
+
+__global__ void __launch_bounds__(ACTIVE_THREADS) k_active_count(const uint8_t* __restrict__ vals, uint64_t n,
+                                                                 uint64_t epoch, uint32_t* __restrict__ tile_counts) {
+    const uint64_t first = (uint64_t)blockIdx.x * ACTIVE_TILE;
+    uint32_t cnt = 0;
+    for (int k = 0; k < ACTIVE_STEPS; k++) {
+        const uint64_t i = first + k * ACTIVE_THREADS + threadIdx.x;
+        cnt += i < n && validator_active_at(vals + VAL_SSZ * i, epoch);
+    }
+    __shared__ uint32_t warp_sum[ACTIVE_THREADS / 32];
+    cnt = __reduce_add_sync(0xffffffffu, cnt);
+    if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = cnt;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t t = 0;
+        for (int w = 0; w < ACTIVE_THREADS / 32; w++) t += warp_sum[w];
+        tile_counts[blockIdx.x] = t;
+    }
+}
+
+__global__ void __launch_bounds__(ACTIVE_THREADS) k_active_write(const uint8_t* __restrict__ vals, uint64_t n,
+                                                                 uint64_t epoch, const uint32_t* __restrict__ tile_counts,
+                                                                 uint64_t* __restrict__ active,
+                                                                 uint64_t* __restrict__ n_active) {
+    __shared__ uint64_t warp_sum64[ACTIVE_THREADS / 32];
+    __shared__ uint32_t warp_cnt[ACTIVE_THREADS / 32];
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    // this tile's first slot: the active validators of the tiles before it
+    uint64_t before = 0;
+    for (uint32_t t = threadIdx.x; t < blockIdx.x; t += ACTIVE_THREADS) before += tile_counts[t];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) before += __shfl_xor_sync(0xffffffffu, before, o);
+    if (lane == 0) warp_sum64[warp] = before;
+    __syncthreads();
+    uint64_t slot = 0;
+#pragma unroll
+    for (int w = 0; w < ACTIVE_THREADS / 32; w++) slot += warp_sum64[w];
+    if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) *n_active = slot + tile_counts[blockIdx.x];
+    const uint64_t first = (uint64_t)blockIdx.x * ACTIVE_TILE;
+    for (int k = 0; k < ACTIVE_STEPS; k++) {
+        const uint64_t i = first + k * ACTIVE_THREADS + threadIdx.x;
+        const bool a = i < n && validator_active_at(vals + VAL_SSZ * i, epoch);
+        const uint32_t ballot = __ballot_sync(0xffffffffu, a);
+        if (lane == 0) warp_cnt[warp] = __popc(ballot);
+        __syncthreads();
+        uint64_t at = slot + __popc(ballot & ((1u << lane) - 1));
+        uint32_t step = 0;
+#pragma unroll
+        for (int w = 0; w < ACTIVE_THREADS / 32; w++) {
+            at += (uint32_t)w < warp ? warp_cnt[w] : 0;
+            step += warp_cnt[w];
+        }
+        if (a) active[at] = i;
+        slot += step;
+        __syncthreads();   // warp_cnt is rewritten by the next step
+    }
+}
+
+// get_seed (beacon_state.rs:1507-1536): H(le32(domain) || le64(epoch) || randao_mixes[(epoch + 65536 - 2) mod 65536]);
+// with_slot: the proposer seed of `slot`, H(get_seed(epoch, DOMAIN_BEACON_PROPOSER) || le64(slot)) (:1040-1050).  One
+// thread per requested seed.
+struct SeedReq {
+    uint64_t epoch, slot;
+    uint32_t domain, with_slot;
+};
+constexpr int MAX_SEED_REQS = 32;
+struct SeedTable {
+    uint32_t n;
+    SeedReq r[MAX_SEED_REQS];
+};
+__global__ void __launch_bounds__(MAX_SEED_REQS) k_committee_seeds(const uint8_t* __restrict__ mixes,
+                                                                   const __grid_constant__ SeedTable tab,
+                                                                   uint8_t* __restrict__ seeds) {
+    if (threadIdx.x >= tab.n) return;
+    const SeedReq q = tab.r[threadIdx.x];
+    uint32_t w[16], st[8], mix[8];
+    load_chunk(mixes + 32 * ((q.epoch % 65536 + 65534) % 65536), mix);
+    w[0] = bswap32(q.domain);
+    w[1] = bswap32((uint32_t)q.epoch);
+    w[2] = bswap32((uint32_t)(q.epoch >> 32));
+#pragma unroll
+    for (int k = 0; k < 8; k++) w[3 + k] = mix[k];
+    w[11] = 0x80000000u;
+    w[12] = w[13] = w[14] = 0;
+    w[15] = 44 * 8;
+    sha256_one_block(w, st);
+    if (q.with_slot) {
+#pragma unroll
+        for (int k = 0; k < 8; k++) w[k] = st[k];
+        w[8] = bswap32((uint32_t)q.slot);
+        w[9] = bswap32((uint32_t)(q.slot >> 32));
+        w[10] = 0x80000000u;
+        w[11] = w[12] = w[13] = w[14] = 0;
+        w[15] = 40 * 8;
+        sha256_one_block(w, st);
+    }
+    store_chunk(seeds + 32 * threadIdx.x, st);
+}
+
+// shuffling_positions (committee_cache.rs:110-114): positions[shuffling[i]] = i + 1 over a zero-filled array
+__global__ void __launch_bounds__(256) k_shuffling_positions(const uint64_t* __restrict__ shuffling, uint64_t n,
+                                                             uint32_t* __restrict__ positions) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) positions[shuffling[i]] = (uint32_t)(i + 1);
+}
+
+// Balance-weighted sampling over the active set: candidate i is active[compute_shuffled_index(i mod n, n, seed, 90)],
+// accepted when effective_balance * 255 >= MAX_EFFECTIVE_BALANCE * H(seed || le64(i / 32))[i mod 32]; the first `want`
+// accepted candidates in order are the seed's winners.  One CTA per seed (the proposer draw: 32 seeds, 1 winner each;
+// the sync draw: 1 seed, 512 winners).  The seed's 90 pivots are hashed once into shared memory; then each thread
+// takes one speculative candidate of a batch of SAMPLE_THREADS (its 90 source hashes, its record's effective balance,
+// its random byte), a ballot and the warp counts order the accepted ones, and batches repeat until the seed has its
+// winners.  n <= 2^24 (the host refuses more), so positions and pivots fit 32 bits.
+constexpr int SAMPLE_THREADS = 256;
+__global__ void __launch_bounds__(SAMPLE_THREADS) k_sample_validators(const uint8_t* __restrict__ seeds,
+                                                                      const uint64_t* __restrict__ active, uint32_t n,
+                                                                      const uint8_t* __restrict__ vals, uint32_t want,
+                                                                      uint64_t* __restrict__ out) {
+    __shared__ uint32_t s_seed[8];
+    __shared__ uint32_t s_pivot[SHUFFLE_ROUND_COUNT];
+    __shared__ uint32_t warp_cnt[SAMPLE_THREADS / 32];
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid < 8) s_seed[tid] = be_word(seeds + 32 * blockIdx.x + 4 * tid);
+    __syncthreads();
+    uint32_t w[16], st[8];
+    if (tid < SHUFFLE_ROUND_COUNT) {   // pivot = le64(H(seed || round)[0:8]) mod n
+#pragma unroll
+        for (int k = 0; k < 8; k++) w[k] = s_seed[k];
+        w[8] = (tid << 24) | 0x800000u;
+#pragma unroll
+        for (int k = 9; k < 15; k++) w[k] = 0;
+        w[15] = 33 * 8;
+        sha256_one_block(w, st);
+        s_pivot[tid] = (uint32_t)((((uint64_t)bswap32(st[1]) << 32) | bswap32(st[0])) % n);
+    }
+    __syncthreads();
+    uint64_t* dst = out + (uint64_t)blockIdx.x * want;
+    uint32_t have = 0;
+    for (uint64_t base = 0; have < want; base += SAMPLE_THREADS) {
+        const uint64_t i = base + tid;
+        uint32_t index = (uint32_t)(i % n);
+        for (uint32_t r = 0; r < SHUFFLE_ROUND_COUNT; r++) {   // compute_shuffled_index (shuffle_list.rs:18-44)
+            uint32_t flip = s_pivot[r] + n - index;
+            if (flip >= n) flip -= n;
+            const uint32_t pos = index > flip ? index : flip, blk = pos >> 8;
+#pragma unroll
+            for (int k = 0; k < 8; k++) w[k] = s_seed[k];
+            w[8] = (r << 24) | ((blk & 0xff) << 16) | (((blk >> 8) & 0xff) << 8) | ((blk >> 16) & 0xff);
+            w[9] = ((blk >> 24) << 24) | 0x800000u;
+#pragma unroll
+            for (int k = 10; k < 15; k++) w[k] = 0;
+            w[15] = 37 * 8;
+            sha256_one_block(w, st);
+            if ((digest_byte(st, (pos & 0xff) >> 3) >> (pos & 7)) & 1) index = flip;
+        }
+        const uint64_t cand = active[index];
+        const uint64_t eb = le64_at(vals + VAL_SSZ * cand + VAL_EFFECTIVE_BALANCE);
+#pragma unroll
+        for (int k = 0; k < 8; k++) w[k] = s_seed[k];
+        w[8] = bswap32((uint32_t)(i >> 5));
+        w[9] = bswap32((uint32_t)(i >> 37));
+        w[10] = 0x80000000u;
+#pragma unroll
+        for (int k = 11; k < 15; k++) w[k] = 0;
+        w[15] = 40 * 8;
+        sha256_one_block(w, st);
+        const bool ok = eb * MAX_RANDOM_BYTE >= MAX_EFFECTIVE_BALANCE * digest_byte(st, (uint32_t)(i & 31));
+        const uint32_t ballot = __ballot_sync(0xffffffffu, ok);
+        if (lane == 0) warp_cnt[warp] = __popc(ballot);
+        __syncthreads();
+        uint32_t at = have + __popc(ballot & ((1u << lane) - 1)), step = 0;
+#pragma unroll
+        for (int k = 0; k < SAMPLE_THREADS / 32; k++) {
+            at += (uint32_t)k < warp ? warp_cnt[k] : 0;
+            step += warp_cnt[k];
+        }
+        if (ok && at < want) dst[at] = cand;
+        have += step;
+        __syncthreads();   // warp_cnt is rewritten by the next batch
+    }
+}
+
 }  // namespace lhb200

@@ -3104,4 +3104,201 @@ int32_t lhb200_shuffle_list(const uint64_t* input, uint64_t n, uint8_t rounds, c
     return LHB200_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// Committees, proposers and the next sync committee of a resident BeaconState (mainnet preset, chain_spec.rs:627-734).
+// The calls only read the handle: the validator records are the staged copy of field 11 (after a conversion, the
+// list's own storage, which state_relayout keeps that copy pointing at), randao_mixes the staged copy of field 13, and
+// the slot the host literal of field 2, which lhb200_state_patch(_batch) rewrites.  Each call counts the active set,
+// reads its size back (one synchronise: it sizes the shuffle's grids and decides the refusals the reference makes on
+// the active set), then runs the rest and copies the results out.
+constexpr uint64_t SLOTS_PER_EPOCH = 32, EPOCHS_PER_HISTORICAL_VECTOR = 65536, MAX_COMMITTEES_PER_SLOT = 64,
+                   TARGET_COMMITTEE_SIZE = 128, SYNC_COMMITTEE_SIZE = 512, MAX_SHUFFLE_LIST = 1ull << 24;
+constexpr uint32_t DOMAIN_BEACON_PROPOSER = 0, DOMAIN_BEACON_ATTESTER = 1, DOMAIN_SYNC_COMMITTEE = 7;
+
+struct CommitteeInputs {
+    const uint8_t* vals;     // n 121-byte records
+    uint64_t n;
+    const uint8_t* mixes;    // 65536 x 32 bytes
+    uint64_t slot;
+};
+static int32_t committee_inputs(const lhb200_state* st, const char* what, CommitteeInputs& in) {
+    using namespace state_layout;
+    if (st->shard.world != 1) { set_error("%s: a sharded handle holds only its share of the validators", what); return LHB200_EINVAL; }
+    in.vals = st->copies[st->marks[11].copies].dst;
+    in.n = st->var_len[V_VAL] / VAL_SSZ;
+    in.mixes = st->copies[st->marks[13].copies].dst;
+    for (const Plan::LitSrc& ls : st->plan.lit_src)
+        if (ls.src_off == O_SLOT && ls.n == 8) {
+            memcpy(&in.slot, &st->plan.lit[(size_t)ls.lit_index * 32], 8);
+            return LHB200_OK;
+        }
+    set_error("%s: the handle has no slot literal", what);   // not reached: every describer emits field 2
+    return LHB200_EINVAL;
+}
+
+// Device scratch of one committee call over n validators, all carved from one dev_scratch block sized by n up front
+struct CommitteeScratch {
+    uint64_t* n_active;      // then the seeds, contiguous with it: one read-back
+    uint8_t* seeds;
+    uint32_t* tiles;
+    uint64_t* active;
+    uint64_t* shuffled;      // the shuffle's output, or the sampler's winners
+    uint64_t* pivots;
+    uint8_t* sources;
+    uint32_t* positions;
+    uint32_t n_tiles;
+};
+static int32_t committee_scratch(uint64_t n, CommitteeScratch& s) {
+    const uint64_t n_tiles = std::max<uint64_t>(1, ceil_div(n, ACTIVE_TILE)), n_blocks = ceil_div(std::max<uint64_t>(n, 1), 256);
+    const size_t b_head = 256 + MAX_SEED_REQS * 32, b_tiles = align_up(n_tiles * 4, 256), b_list = align_up(n * 8 + 8, 256),
+                 b_out = align_up(std::max<uint64_t>(n * 8, SYNC_COMMITTEE_SIZE * 8), 256), b_piv = 2048,
+                 b_src = align_up(SHUFFLE_ROUND_COUNT * n_blocks * 32, 256), b_pos = align_up(n * 4 + 4, 256);
+    uint8_t* d = static_cast<uint8_t*>(dev_scratch(b_head + b_tiles + b_list + b_out + b_piv + b_src + b_pos));
+    if (!d) return LHB200_ENOMEM;
+    s.n_active = reinterpret_cast<uint64_t*>(d);
+    s.seeds = d + 256;
+    s.tiles = reinterpret_cast<uint32_t*>(d += b_head);
+    s.active = reinterpret_cast<uint64_t*>(d += b_tiles);
+    s.shuffled = reinterpret_cast<uint64_t*>(d += b_list);
+    s.pivots = reinterpret_cast<uint64_t*>(d += b_out);
+    s.sources = (d += b_piv);
+    s.positions = reinterpret_cast<uint32_t*>(d + b_src);
+    s.n_tiles = (uint32_t)n_tiles;
+    return LHB200_OK;
+}
+
+// Seeds for `tab`, then the ascending indices of the validators active at `epoch` and their count, read back with the
+// seeds (h: pinned, 256 + 32 * tab.n bytes).  Three launches and the one synchronise of a committee call.
+static int32_t committee_front(const CommitteeInputs& in, const CommitteeScratch& s, uint64_t epoch, const SeedTable& tab,
+                               uint8_t* h, uint64_t* n_active, cudaStream_t stream) {
+    k_committee_seeds<<<1, MAX_SEED_REQS, 0, stream>>>(in.mixes, tab, s.seeds);
+    k_active_count<<<s.n_tiles, ACTIVE_THREADS, 0, stream>>>(in.vals, in.n, epoch, s.tiles);
+    k_active_write<<<s.n_tiles, ACTIVE_THREADS, 0, stream>>>(in.vals, in.n, epoch, s.tiles, s.active, s.n_active);
+    count_launch(3);
+    LHB_CUDA(cudaGetLastError());
+    LHB_CUDA(cudaMemcpyAsync(h, s.n_active, 256 + 32 * tab.n, cudaMemcpyDeviceToHost, stream));
+    LHB_CUDA(cudaStreamSynchronize(stream));
+    memcpy(n_active, h, 8);
+    return LHB200_OK;
+}
+// The reference's refusals on the active set: none active (InsufficientValidators), or more than the shuffle takes
+// (compute_shuffled_index / shuffle_list return None: UnableToShuffle)
+static int32_t check_active(uint64_t n_active, uint64_t epoch, const char* what) {
+    if (n_active == 0) { set_error("%s: no validator is active at epoch %llu", what, (unsigned long long)epoch); return LHB200_EINVAL; }
+    if (n_active > MAX_SHUFFLE_LIST) {
+        set_error("%s: %llu active validators, more than the shuffle takes (2^24)", what, (unsigned long long)n_active);
+        return LHB200_EINVAL;
+    }
+    return LHB200_OK;
+}
+
+int32_t lhb200_state_committee_cache(lhb200_state* st, uint64_t epoch, uint64_t* shuffling, uint32_t* positions,
+                                     uint64_t cap, lhb200_committee_info* info) {
+    LHB_REQUIRE_READY();
+    if (!st || !shuffling || !info) { set_error("state_committee_cache: null argument"); return LHB200_EINVAL; }
+    Ctx& c = ctx();
+    std::lock_guard<std::recursive_mutex> g(c.mu);
+    CommitteeInputs in;
+    int32_t rc = committee_inputs(st, "state_committee_cache", in);
+    if (rc) return rc;
+    if (cap < in.n) {
+        set_error("state_committee_cache: cap %llu is below the validator count %llu", (unsigned long long)cap,
+                  (unsigned long long)in.n);
+        return LHB200_EINVAL;
+    }
+    // EpochOutOfBounds: the seed's mix must still be in randao_mixes, and at most one epoch ahead
+    const uint64_t current = in.slot / SLOTS_PER_EPOCH;
+    const uint64_t min_randao = current + 1 > EPOCHS_PER_HISTORICAL_VECTOR ? current + 1 - EPOCHS_PER_HISTORICAL_VECTOR : 0;
+    if ((epoch > 2 ? epoch - 2 : 0) < min_randao || epoch > current + 1) {
+        set_error("state_committee_cache: epoch %llu is out of bounds at current epoch %llu (min randao epoch %llu)",
+                  (unsigned long long)epoch, (unsigned long long)current, (unsigned long long)min_randao);
+        return LHB200_EINVAL;
+    }
+    CommitteeScratch s;
+    uint8_t* h = static_cast<uint8_t*>(pinned_scratch(256 + 32 * MAX_SEED_REQS));
+    if (!h) return LHB200_ENOMEM;
+    if ((rc = committee_scratch(in.n, s))) return rc;
+    SeedTable tab{};
+    tab.n = 1;
+    tab.r[0] = {epoch, 0, DOMAIN_BEACON_ATTESTER, 0};
+    uint64_t n_active = 0;
+    if ((rc = committee_front(in, s, epoch, tab, h, &n_active, c.stream))) return rc;
+    if ((rc = check_active(n_active, epoch, "state_committee_cache"))) return rc;
+    info->epoch = epoch;
+    info->n_validators = in.n;
+    info->n_active = n_active;
+    info->committees_per_slot = std::max<uint64_t>(1, std::min(MAX_COMMITTEES_PER_SLOT, n_active / SLOTS_PER_EPOCH / TARGET_COMMITTEE_SIZE));
+    memcpy(info->seed, h + 256, 32);
+    // shuffle_list(active, 90, seed, forwards = false) on the device-resident active list
+    const uint32_t n_blocks = (uint32_t)ceil_div(n_active, 256);
+    const uint64_t total = (uint64_t)SHUFFLE_ROUND_COUNT * n_blocks;
+    k_shuffle_hashes<<<(unsigned)ceil_div(total, 128), 128, 0, c.stream>>>(s.seeds, SHUFFLE_ROUND_COUNT, n_active, n_blocks,
+                                                                           s.pivots, s.sources);
+    k_shuffle_permute<<<(unsigned)ceil_div(n_active, 256), 256, 0, c.stream>>>(s.active, s.shuffled, n_active,
+                                                                               SHUFFLE_ROUND_COUNT, n_blocks, s.pivots,
+                                                                               s.sources, 0);
+    count_launch(2);
+    if (positions) {
+        LHB_CUDA(cudaMemsetAsync(s.positions, 0, in.n * 4, c.stream));
+        k_shuffling_positions<<<(unsigned)ceil_div(n_active, 256), 256, 0, c.stream>>>(s.shuffled, n_active, s.positions);
+        count_launch();
+    }
+    LHB_CUDA(cudaGetLastError());
+    LHB_CUDA(cudaMemcpyAsync(shuffling, s.shuffled, n_active * 8, cudaMemcpyDefault, c.stream));
+    if (positions && in.n) LHB_CUDA(cudaMemcpyAsync(positions, s.positions, in.n * 4, cudaMemcpyDefault, c.stream));
+    LHB_CUDA(cudaStreamSynchronize(c.stream));
+    return LHB200_OK;
+}
+
+// The first `want` accepted candidates of each seed of `tab` over the validators active at `epoch` -> out
+static int32_t sample_validators(const CommitteeInputs& in, const char* what, uint64_t epoch, const SeedTable& tab,
+                                 uint32_t want, uint64_t* out) {
+    Ctx& c = ctx();
+    CommitteeScratch s;
+    uint8_t* h = static_cast<uint8_t*>(pinned_scratch(256 + 32 * MAX_SEED_REQS));
+    if (!h) return LHB200_ENOMEM;
+    int32_t rc = committee_scratch(in.n, s);
+    if (rc) return rc;
+    uint64_t n_active = 0;
+    if ((rc = committee_front(in, s, epoch, tab, h, &n_active, c.stream))) return rc;
+    if ((rc = check_active(n_active, epoch, what))) return rc;
+    k_sample_validators<<<tab.n, SAMPLE_THREADS, 0, c.stream>>>(s.seeds, s.active, (uint32_t)n_active, in.vals, want,
+                                                               s.shuffled);
+    count_launch();
+    LHB_CUDA(cudaGetLastError());
+    LHB_CUDA(cudaMemcpyAsync(out, s.shuffled, (size_t)tab.n * want * 8, cudaMemcpyDefault, c.stream));
+    LHB_CUDA(cudaStreamSynchronize(c.stream));
+    return LHB200_OK;
+}
+
+// get_beacon_proposer_indices (beacon_state.rs:1025-1037): one proposer per slot of the current epoch
+int32_t lhb200_state_beacon_proposer_indices(lhb200_state* st, uint64_t out[32]) {
+    LHB_REQUIRE_READY();
+    if (!st || !out) { set_error("state_beacon_proposer_indices: null argument"); return LHB200_EINVAL; }
+    std::lock_guard<std::recursive_mutex> g(ctx().mu);
+    CommitteeInputs in;
+    int32_t rc = committee_inputs(st, "state_beacon_proposer_indices", in);
+    if (rc) return rc;
+    const uint64_t epoch = in.slot / SLOTS_PER_EPOCH;
+    SeedTable tab{};
+    tab.n = SLOTS_PER_EPOCH;
+    for (uint32_t k = 0; k < SLOTS_PER_EPOCH; k++) tab.r[k] = {epoch, epoch * SLOTS_PER_EPOCH + k, DOMAIN_BEACON_PROPOSER, 1};
+    return sample_validators(in, "state_beacon_proposer_indices", epoch, tab, 1, out);
+}
+
+// get_next_sync_committee_indices (beacon_state.rs:1091-1125): 512 draws at the next epoch, duplicates kept
+int32_t lhb200_state_next_sync_committee_indices(lhb200_state* st, uint64_t out[512]) {
+    LHB_REQUIRE_READY();
+    if (!st || !out) { set_error("state_next_sync_committee_indices: null argument"); return LHB200_EINVAL; }
+    std::lock_guard<std::recursive_mutex> g(ctx().mu);
+    CommitteeInputs in;
+    int32_t rc = committee_inputs(st, "state_next_sync_committee_indices", in);
+    if (rc) return rc;
+    const uint64_t epoch = in.slot / SLOTS_PER_EPOCH + 1;
+    SeedTable tab{};
+    tab.n = 1;
+    tab.r[0] = {epoch, 0, DOMAIN_SYNC_COMMITTEE, 0};
+    return sample_validators(in, "state_next_sync_committee_indices", epoch, tab, SYNC_COMMITTEE_SIZE, out);
+}
+
 }  // extern "C"

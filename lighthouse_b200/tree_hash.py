@@ -384,6 +384,33 @@ class ResidentState:
         """BeaconState::compute_merkle_proof (beacon_state.rs:2483) by the spec's generalized index: the branch."""
         return self.proofs([gindex])[1][0]
 
+    def committee_cache(self, epoch):
+        """CommitteeCache::initialized(state, epoch) on the device (lhb200_state_committee_cache) -> a
+        committees.CommitteeCache.  Refused (Lhb200Error, EINVAL): an epoch out of bounds, no active validator, a
+        sharded handle.  The handle is only read."""
+        import numpy as np
+        from .committees import CommitteeCache
+        n = self.list_len("validators")
+        shuffling = np.zeros(max(n, 1), dtype=np.uint64)
+        positions = np.zeros(max(n, 1), dtype=np.uint32)
+        info = _ffi.CommitteeInfo()
+        check(lib.lhb200_state_committee_cache(self._h, epoch, shuffling.ctypes.data, positions.ctypes.data, n,
+                                               C.byref(info)), "lhb200_state_committee_cache")
+        return CommitteeCache(info.epoch, shuffling[:info.n_active], positions[:n], info.committees_per_slot,
+                              bytes(info.seed))
+
+    def beacon_proposer_indices(self):
+        """BeaconState::get_beacon_proposer_indices: the proposer of each of the current epoch's 32 slots."""
+        out = (C.c_uint64 * 32)()
+        check(lib.lhb200_state_beacon_proposer_indices(self._h, out), "lhb200_state_beacon_proposer_indices")
+        return list(out)
+
+    def next_sync_committee_indices(self):
+        """BeaconState::get_next_sync_committee_indices: 512 validator indices, duplicates kept."""
+        out = (C.c_uint64 * 512)()
+        check(lib.lhb200_state_next_sync_committee_indices(self._h, out), "lhb200_state_next_sync_committee_indices")
+        return list(out)
+
     @property
     def device_bytes(self):
         """HBM the handle holds (lhb200_state_device_bytes)."""
