@@ -282,6 +282,16 @@ LHB200_API int32_t lhb200_state_beacon_proposer_indices(lhb200_state* st, uint64
 /* get_next_sync_committee_indices (beacon_state.rs:1091-1125): 512 indices drawn at current_epoch + 1, duplicates
  * kept. */
 LHB200_API int32_t lhb200_state_next_sync_committee_indices(lhb200_state* st, uint64_t out[512]);
+/* A committee cache that stays on the device: the same steps, refusals and messages as lhb200_state_committee_cache
+ * (5 launches, the one read-back of the active count), with the shuffling left in device memory the handle owns.  The handle does not depend
+ * on the state once created: releasing, patching or cloning the state leaves it as it is (Lighthouse keeps committee
+ * caches across states).  lhb200_committee_cache_shuffling copies the n_active shuffled indices out (one copy; cap =
+ * entries `out` holds, at least info.n_active).  Release frees the handle (NULL is a no-op). */
+typedef struct lhb200_committee_cache lhb200_committee_cache;
+LHB200_API int32_t lhb200_state_committee_cache_create(lhb200_state* st, uint64_t epoch, lhb200_committee_cache** out);
+LHB200_API int32_t lhb200_committee_cache_info(const lhb200_committee_cache* cc, lhb200_committee_info* info);
+LHB200_API int32_t lhb200_committee_cache_shuffling(const lhb200_committee_cache* cc, uint64_t* out, uint64_t cap);
+LHB200_API int32_t lhb200_committee_cache_release(lhb200_committee_cache* cc);
 
 /* ---- BLS batch verification path ---------------------------------------------------------------- */
 
@@ -381,6 +391,48 @@ LHB200_API uint64_t lhb200_pubkey_table_len(const lhb200_pubkey_table* t);
 LHB200_API int32_t lhb200_bls_batch_upload_indexed(lhb200_bls_batch* b, const lhb200_pubkey_table* table,
                                                    const uint8_t* sigs, const uint8_t* msgs, const uint32_t* key_indices,
                                                    const uint32_t* pk_offsets, const uint64_t* rands, uint32_t n_sets);
+/* Attestations verified against resident committee caches and the pubkey table: get_attesting_indices
+ * (get_attesting_indices.rs), indexed_attestation_signature_set (signature_sets.rs:271-332) and verify_signature_sets,
+ * with the committee lookup, attesting indices, AttestationData and signing roots and the key gather on the device.
+ *   ssz, offsets  n Attestation encodings, record i = ssz[offsets[i] .. offsets[i + 1]).  fork = LHB200_FORK_*: Base
+ *                 to Deneb share one shape (228-byte fixed part, Bitlist[2048]); Electra adds committee_bits
+ *                 (236 bytes, Bitlist[131072]).
+ *   caches        1 to 3 committee caches of distinct epochs; an attestation uses the one of data.slot / 32.
+ *   fork_info     domain = compute_domain(DOMAIN_BEACON_ATTESTER, previous_version if target.epoch < epoch else
+ *                 current_version, genesis_validators_root) (ChainSpec::get_domain).
+ *   rands         n nonzero scalars (attestation i's), or NULL to draw them like lhb200_verify_signature_sets.
+ *   *ok           verify_signature_sets over the attestations whose status is 0 (0 when there is none).
+ *   status        n bytes: 0 fine; LHB200_ATT_* (10-14) an indexing error, in that precedence, and the attestation is
+ *                 left out of the batch; else the set's verify status (1-6, see lhb200_verify_signature_sets; an
+ *                 empty index set reaches the batch and reports 4).
+ *   signing_roots optional, n x 32 B (zeros for a MALFORMED record).
+ *   indices_offsets, indices  optional together: the IndexedAttestation indices, sorted ascending, as a CSR
+ *                 (indices_offsets: n + 1 entries) for every attestation of status 0, 1-6 or UNKNOWN_VALIDATOR (empty
+ *                 for the others).  indices_cap below the total -> LHB200_EINVAL before any output is written.
+ * One read-back (status, key count and signing root per attestation) lets the host group the messages and size the
+ * key-index buffer; the indices then go from the committee caches straight into the batch on the device.  The launch
+ * count does not depend on n or on committee sizes.  Refusals -> LHB200_EINVAL: null pointers, n == 0, non-monotone
+ * offsets, a zero scalar, n_caches outside 1..3 or two caches of one epoch, an unknown fork.  Concurrent calls each
+ * borrow a pooled batch handle and hold no library-wide lock. */
+#define LHB200_ATT_MALFORMED 10          /* bad offset, missing delimiter, over-long bitlist, short record */
+#define LHB200_ATT_NO_CACHE 11           /* no cache at data.slot's epoch (CommitteeCacheUninitialized) */
+#define LHB200_ATT_NO_COMMITTEE 12       /* a committee index >= committees_per_slot (NoCommittee) */
+#define LHB200_ATT_BITFIELD_LENGTH 13    /* bitlist length != committee length(s) (InvalidBitfield) */
+#define LHB200_ATT_UNKNOWN_VALIDATOR 14  /* an index >= lhb200_pubkey_table_len (ValidatorUnknown) */
+typedef struct {
+    uint8_t previous_version[4], current_version[4];
+    uint64_t epoch;
+} lhb200_fork;
+LHB200_API int32_t lhb200_attestations_verify(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, int32_t fork,
+                                              const lhb200_committee_cache* const* caches, uint32_t n_caches,
+                                              const lhb200_pubkey_table* table, const lhb200_fork* fork_info,
+                                              const uint8_t genesis_validators_root[32], const uint64_t* rands,
+                                              uint8_t* ok, uint8_t* status, uint8_t* signing_roots,
+                                              uint64_t* indices_offsets, uint64_t* indices, uint64_t indices_cap);
+/* Test hook: the final-exponentiated product (format of lhb200_bls_batch_gt) and the kernel plan (format of
+ * lhb200_bls_batch_plan; gt576 or plan may be NULL) of the batch check the calling thread's last
+ * lhb200_attestations_verify ran.  LHB200_EINVAL when that call verified no set. */
+LHB200_API int32_t lhb200_debug_attestations_last(uint8_t gt576[576], uint32_t* plan, uint32_t n_words);
 /* Test hook: final-exponentiated product of the last verify as 12 x 48-byte big-endian Fp (tower order
  * c0.c0.c0 .. c1.c2.c1).  NOTE: this is the cube of the canonical GT element (3 is coprime to r). */
 LHB200_API int32_t lhb200_bls_batch_gt(lhb200_bls_batch* b, uint8_t out576[576]);

@@ -155,6 +155,13 @@ _sig("lhb200_debug_proof_gather_ms", C.c_float)
 _sig("lhb200_state_committee_cache", C.c_int32, vp, C.c_uint64, vp, vp, C.c_uint64, vp)
 _sig("lhb200_state_beacon_proposer_indices", C.c_int32, vp, vp)
 _sig("lhb200_state_next_sync_committee_indices", C.c_int32, vp, vp)
+_sig("lhb200_state_committee_cache_create", C.c_int32, vp, C.c_uint64, C.POINTER(vp))
+_sig("lhb200_committee_cache_info", C.c_int32, vp, vp)
+_sig("lhb200_committee_cache_shuffling", C.c_int32, vp, vp, C.c_uint64)
+_sig("lhb200_committee_cache_release", C.c_int32, vp)
+_sig("lhb200_attestations_verify", C.c_int32, vp, vp, C.c_uint32, C.c_int32, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp,
+     vp, vp, C.c_uint64)
+_sig("lhb200_debug_attestations_last", C.c_int32, vp, vp, C.c_uint32)
 
 
 class ListEdit(C.Structure):
@@ -167,3 +174,8 @@ class CommitteeInfo(C.Structure):
     """lhb200_committee_info"""
     _fields_ = [("epoch", C.c_uint64), ("n_validators", C.c_uint64), ("n_active", C.c_uint64),
                 ("committees_per_slot", C.c_uint64), ("seed", C.c_uint8 * 32)]
+
+
+class Fork(C.Structure):
+    """lhb200_fork"""
+    _fields_ = [("previous_version", C.c_uint8 * 4), ("current_version", C.c_uint8 * 4), ("epoch", C.c_uint64)]

@@ -107,3 +107,49 @@ class CommitteeCache:
         start, end = self._committee_range(nth)
         slot = self.initialized_epoch * self.slots_per_epoch + nth // self._committees_per_slot
         return AttestationDuty(slot, nth % self._committees_per_slot, i - start, end - start, self._committees_per_slot)
+
+
+class DeviceCommitteeCache:
+    """A committee cache that stays on the device (lhb200_state_committee_cache_create), what
+    lighthouse_b200.attestations.verify_attestations reads.  It owns its shuffling and does not depend on the state it
+    came from: releasing, patching or cloning that state leaves it as it is."""
+
+    def __init__(self, handle):
+        self._h = handle
+
+    @property
+    def info(self):
+        """lhb200_committee_info: epoch, n_validators, n_active, committees_per_slot, seed."""
+        from . import _ffi
+        info = _ffi.CommitteeInfo()
+        _ffi.check(_ffi.lib.lhb200_committee_cache_info(self._h, _ffi.C.byref(info)), "lhb200_committee_cache_info")
+        return info
+
+    @property
+    def epoch(self):
+        return self.info.epoch
+
+    def to_host(self):
+        """The same cache as a CommitteeCache, from one device-to-host copy of the shuffling (the positions are its
+        inverse, scattered here)."""
+        from . import _ffi
+        info = self.info
+        shuffling = np.zeros(max(info.n_active, 1), dtype=np.uint64)
+        _ffi.check(_ffi.lib.lhb200_committee_cache_shuffling(self._h, shuffling.ctypes.data, len(shuffling)),
+                   "lhb200_committee_cache_shuffling")
+        shuffling = shuffling[:info.n_active]
+        positions = np.zeros(info.n_validators, dtype=np.uint32)
+        positions[shuffling.astype(np.int64)] = np.arange(1, info.n_active + 1, dtype=np.uint32)
+        return CommitteeCache(info.epoch, shuffling, positions, info.committees_per_slot, bytes(info.seed))
+
+    def release(self):
+        if self._h:
+            from . import _ffi
+            _ffi.lib.lhb200_committee_cache_release(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass

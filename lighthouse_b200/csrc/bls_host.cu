@@ -269,6 +269,11 @@ struct lhb200_bls_batch {
     Fp12* d_seg_gt = nullptr;
     uint8_t* d_seg_ok = nullptr;
     uint8_t* h_seg_ok = nullptr;             // pinned
+    // grow-only scratch of a caller that drives this handle from another file (bls_batch_aux)
+    void* d_aux = nullptr;
+    size_t d_aux_bytes = 0;
+    uint8_t* h_aux = nullptr;                // pinned
+    size_t h_aux_bytes = 0;
 };
 
 static void batch_free(lhb200_bls_batch* b) {
@@ -283,6 +288,8 @@ static void batch_free(lhb200_bls_batch* b) {
         if (p) cudaFree(p);
     if (b->h_res) cudaFreeHost(b->h_res);
     if (b->h_seg_ok) cudaFreeHost(b->h_seg_ok);
+    if (b->d_aux) cudaFree(b->d_aux);
+    if (b->h_aux) cudaFreeHost(b->h_aux);
     if (b->s_main) cudaStreamDestroy(b->s_main);
     if (b->s2) cudaStreamDestroy(b->s2);
     if (b->s3) cudaStreamDestroy(b->s3);
@@ -1936,3 +1943,99 @@ int32_t lhb200_debug_fp_batch(int32_t op, const uint32_t* in, uint32_t in_words,
 }
 
 }  // extern "C"
+
+// ---- a pooled handle driven from another file (lhb200_attestations_verify in merkle_host.cu) ---------------------
+// The caller borrows a handle, keeps its own scratch on it, stages sets whose key indices it writes on the device, then
+// verifies.  Nothing here takes the library mutex: the handle is the caller's alone until it is returned.
+namespace {
+thread_local Fp12 t_last_gt;                          // the calling thread's last bls_batch_finish (test hook)
+thread_local uint32_t t_last_plan[LHB200_PLAN_WORDS];
+thread_local bool t_last_valid = false;
+}  // namespace
+
+namespace lhb200 {
+lhb200_bls_batch* bls_pool_borrow(uint32_t n_sets) {
+    t_last_valid = false;
+    lhb200_bls_batch* b = pool_acquire(n_sets, 0);
+    if (!b) set_error("bls_pool_borrow: no batch handle for %u sets", n_sets);
+    return b;
+}
+
+void bls_pool_return(lhb200_bls_batch* b) {
+    cudaStreamSynchronize(b->s_main);
+    cudaStreamSynchronize(b->s2);
+    cudaStreamSynchronize(b->s3);
+    pool_release(b);
+}
+
+cudaStream_t bls_batch_stream(const lhb200_bls_batch* b) { return b->s_main; }
+
+// Grow-only device and pinned scratch owned by the handle; nullptr (error set) when an allocation fails
+void* bls_batch_aux(lhb200_bls_batch* b, size_t dev_bytes, uint8_t** pinned, size_t pinned_bytes) {
+    if (dev_bytes > b->d_aux_bytes || pinned_bytes > b->h_aux_bytes) {
+        cudaStreamSynchronize(b->s_main);
+        if (dev_bytes > b->d_aux_bytes) {
+            if (b->d_aux) cudaFree(b->d_aux);
+            b->d_aux = nullptr;
+            b->d_aux_bytes = 0;
+            const size_t sz = std::max<size_t>(dev_bytes + dev_bytes / 4, 1 << 20);
+            const cudaError_t e = cudaMalloc(&b->d_aux, sz);
+            if (e != cudaSuccess) { b->d_aux = nullptr; cuda_fail(e, "cudaMalloc(batch scratch)"); return nullptr; }
+            b->d_aux_bytes = sz;
+        }
+        if (pinned_bytes > b->h_aux_bytes) {
+            if (b->h_aux) cudaFreeHost(b->h_aux);
+            b->h_aux = nullptr;
+            b->h_aux_bytes = 0;
+            const size_t sz = std::max<size_t>(pinned_bytes + pinned_bytes / 4, 64 << 10);
+            const cudaError_t e = cudaHostAlloc(reinterpret_cast<void**>(&b->h_aux), sz, cudaHostAllocDefault);
+            if (e != cudaSuccess) { b->h_aux = nullptr; cuda_fail(e, "cudaHostAlloc(batch scratch)"); return nullptr; }
+            b->h_aux_bytes = sz;
+        }
+    }
+    *pinned = b->h_aux;
+    return b->d_aux;
+}
+
+// What lhb200_bls_batch_upload_indexed stages (signatures, messages with their grouping, offsets, scalars), queued on
+// the handle's stream, with the key indices left to the caller: *d_key_indices holds pk_offsets[n_sets] of them.
+int32_t bls_batch_stage_table(lhb200_bls_batch* b, const lhb200_pubkey_table* table, const uint8_t* sigs,
+                              const uint8_t* msgs, const uint32_t* pk_offsets, const uint64_t* rands, uint32_t n_sets,
+                              uint32_t** d_key_indices) {
+    const uint64_t n_keys = pk_offsets[n_sets];
+    if (n_keys > b->cap_indices) {
+        LHB_CUDA(cudaStreamSynchronize(b->s_main));
+        if (b->d_indices) cudaFree(b->d_indices);
+        b->d_indices = nullptr;
+        b->cap_indices = 0;
+        LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&b->d_indices), std::max<uint64_t>(n_keys + n_keys / 4, 1) * 4));
+        b->cap_indices = n_keys + n_keys / 4;
+    }
+    if (int32_t rc = stage_inputs("attestations_verify", b, table, sigs, msgs, b->d_indices, pk_offsets, rands, n_sets,
+                                  b->s_main))
+        return rc;
+    *d_key_indices = b->d_indices;
+    return LHB200_OK;
+}
+
+// verify_enqueue and result on the handle's stream: *ok, and the n statuses of the staged sets
+int32_t bls_batch_finish(lhb200_bls_batch* b, uint8_t* ok, uint8_t* set_status) {
+    if (int32_t rc = lhb200_bls_batch_verify_enqueue(b, b->s_main)) return rc;
+    uint8_t* h_gt = b->h_res + 64 + 2 * (size_t)b->cap_sets;   // the Fp12 slot behind the status bytes
+    LHB_CUDA(cudaMemcpyAsync(h_gt, b->d_gt, sizeof(Fp12), cudaMemcpyDeviceToHost, b->s_main));
+    if (int32_t rc = lhb200_bls_batch_result(b, b->s_main, ok, set_status)) return rc;
+    memcpy(&t_last_gt, h_gt, sizeof(Fp12));
+    memcpy(t_last_plan, b->plan, sizeof t_last_plan);
+    t_last_valid = true;
+    return LHB200_OK;
+}
+}  // namespace lhb200
+
+// Test hook: the final-exponentiated product (format of lhb200_bls_batch_gt) and the kernel plan (lhb200_bls_batch_plan)
+// of the batch check the calling thread's last lhb200_attestations_verify ran; LHB200_EINVAL when it ran none.
+extern "C" LHB200_API int32_t lhb200_debug_attestations_last(uint8_t gt576[576], uint32_t* plan, uint32_t n_words) {
+    if (!t_last_valid) { set_error("debug_attestations_last: the last call on this thread verified no set"); return LHB200_EINVAL; }
+    if (gt576) gt_to_bytes(t_last_gt, gt576);
+    if (plan) memcpy(plan, t_last_plan, sizeof(uint32_t) * std::min<uint32_t>(n_words, LHB200_PLAN_WORDS));
+    return LHB200_OK;
+}

@@ -55,4 +55,15 @@ int32_t comm_allgather_bytes(const void* d_send, void* d_recv, size_t bytes_per_
 
 inline void count_launch(uint64_t n = 1) { ctx().launches.fetch_add(n, std::memory_order_relaxed); }
 
+// A pooled BLS batch handle driven from outside bls_host.cu (lhb200_attestations_verify): borrow, keep scratch on it,
+// stage sets whose key indices the caller writes on the device, verify, return.  No library mutex is held.
+lhb200_bls_batch* bls_pool_borrow(uint32_t n_sets);
+void bls_pool_return(lhb200_bls_batch* b);
+cudaStream_t bls_batch_stream(const lhb200_bls_batch* b);
+void* bls_batch_aux(lhb200_bls_batch* b, size_t dev_bytes, uint8_t** pinned, size_t pinned_bytes);
+int32_t bls_batch_stage_table(lhb200_bls_batch* b, const lhb200_pubkey_table* table, const uint8_t* sigs,
+                              const uint8_t* msgs, const uint32_t* pk_offsets, const uint64_t* rands, uint32_t n_sets,
+                              uint32_t** d_key_indices);
+int32_t bls_batch_finish(lhb200_bls_batch* b, uint8_t* ok, uint8_t* set_status);
+
 }  // namespace lhb200

@@ -10,8 +10,10 @@
 #include <type_traits>
 #include <unordered_map>
 #include <vector>
+#include <cub/device/device_segmented_sort.cuh>
 #include "ctx.h"
 #include "merkle.cuh"
+#include "attest.cuh"
 
 namespace lhb200 {
 
@@ -3192,17 +3194,19 @@ static int32_t check_active(uint64_t n_active, uint64_t epoch, const char* what)
     return LHB200_OK;
 }
 
-int32_t lhb200_state_committee_cache(lhb200_state* st, uint64_t epoch, uint64_t* shuffling, uint32_t* positions,
-                                     uint64_t cap, lhb200_committee_info* info) {
-    LHB_REQUIRE_READY();
-    if (!st || !shuffling || !info) { set_error("state_committee_cache: null argument"); return LHB200_EINVAL; }
+// CommitteeCache::initialized up to the shuffle, the body lhb200_state_committee_cache and
+// lhb200_state_committee_cache_create share: the refusals (cap: the caller's buffer size, checked against the validator
+// count when given), the seeds and the active set with the one read-back, then shuffle_list(active, 90, seed,
+// forwards = false) on c.stream into s.shuffled or, with `owned`, into device memory allocated for the caller (5
+// launches).  Called with the library mutex held.
+static int32_t committee_shuffle(lhb200_state* st, uint64_t epoch, const char* what, const uint64_t* cap,
+                                 CommitteeInputs& in, CommitteeScratch& s, lhb200_committee_info* info,
+                                 uint64_t** owned) {
     Ctx& c = ctx();
-    std::lock_guard<std::recursive_mutex> g(c.mu);
-    CommitteeInputs in;
-    int32_t rc = committee_inputs(st, "state_committee_cache", in);
+    int32_t rc = committee_inputs(st, what, in);
     if (rc) return rc;
-    if (cap < in.n) {
-        set_error("state_committee_cache: cap %llu is below the validator count %llu", (unsigned long long)cap,
+    if (cap && *cap < in.n) {
+        set_error("%s: cap %llu is below the validator count %llu", what, (unsigned long long)*cap,
                   (unsigned long long)in.n);
         return LHB200_EINVAL;
     }
@@ -3210,11 +3214,10 @@ int32_t lhb200_state_committee_cache(lhb200_state* st, uint64_t epoch, uint64_t*
     const uint64_t current = in.slot / SLOTS_PER_EPOCH;
     const uint64_t min_randao = current + 1 > EPOCHS_PER_HISTORICAL_VECTOR ? current + 1 - EPOCHS_PER_HISTORICAL_VECTOR : 0;
     if ((epoch > 2 ? epoch - 2 : 0) < min_randao || epoch > current + 1) {
-        set_error("state_committee_cache: epoch %llu is out of bounds at current epoch %llu (min randao epoch %llu)",
+        set_error("%s: epoch %llu is out of bounds at current epoch %llu (min randao epoch %llu)", what,
                   (unsigned long long)epoch, (unsigned long long)current, (unsigned long long)min_randao);
         return LHB200_EINVAL;
     }
-    CommitteeScratch s;
     uint8_t* h = static_cast<uint8_t*>(pinned_scratch(256 + 32 * MAX_SEED_REQS));
     if (!h) return LHB200_ENOMEM;
     if ((rc = committee_scratch(in.n, s))) return rc;
@@ -3223,21 +3226,39 @@ int32_t lhb200_state_committee_cache(lhb200_state* st, uint64_t epoch, uint64_t*
     tab.r[0] = {epoch, 0, DOMAIN_BEACON_ATTESTER, 0};
     uint64_t n_active = 0;
     if ((rc = committee_front(in, s, epoch, tab, h, &n_active, c.stream))) return rc;
-    if ((rc = check_active(n_active, epoch, "state_committee_cache"))) return rc;
+    if ((rc = check_active(n_active, epoch, what))) return rc;
     info->epoch = epoch;
     info->n_validators = in.n;
     info->n_active = n_active;
     info->committees_per_slot = std::max<uint64_t>(1, std::min(MAX_COMMITTEES_PER_SLOT, n_active / SLOTS_PER_EPOCH / TARGET_COMMITTEE_SIZE));
     memcpy(info->seed, h + 256, 32);
+    uint64_t* out = s.shuffled;
+    if (owned) {
+        LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(owned), n_active * 8));
+        out = *owned;
+    }
     // shuffle_list(active, 90, seed, forwards = false) on the device-resident active list
     const uint32_t n_blocks = (uint32_t)ceil_div(n_active, 256);
     const uint64_t total = (uint64_t)SHUFFLE_ROUND_COUNT * n_blocks;
     k_shuffle_hashes<<<(unsigned)ceil_div(total, 128), 128, 0, c.stream>>>(s.seeds, SHUFFLE_ROUND_COUNT, n_active, n_blocks,
                                                                            s.pivots, s.sources);
-    k_shuffle_permute<<<(unsigned)ceil_div(n_active, 256), 256, 0, c.stream>>>(s.active, s.shuffled, n_active,
+    k_shuffle_permute<<<(unsigned)ceil_div(n_active, 256), 256, 0, c.stream>>>(s.active, out, n_active,
                                                                                SHUFFLE_ROUND_COUNT, n_blocks, s.pivots,
                                                                                s.sources, 0);
     count_launch(2);
+    return LHB200_OK;
+}
+
+int32_t lhb200_state_committee_cache(lhb200_state* st, uint64_t epoch, uint64_t* shuffling, uint32_t* positions,
+                                     uint64_t cap, lhb200_committee_info* info) {
+    LHB_REQUIRE_READY();
+    if (!st || !shuffling || !info) { set_error("state_committee_cache: null argument"); return LHB200_EINVAL; }
+    Ctx& c = ctx();
+    std::lock_guard<std::recursive_mutex> g(c.mu);
+    CommitteeInputs in;
+    CommitteeScratch s;
+    if (int32_t rc = committee_shuffle(st, epoch, "state_committee_cache", &cap, in, s, info, nullptr)) return rc;
+    const uint64_t n_active = info->n_active;
     if (positions) {
         LHB_CUDA(cudaMemsetAsync(s.positions, 0, in.n * 4, c.stream));
         k_shuffling_positions<<<(unsigned)ceil_div(n_active, 256), 256, 0, c.stream>>>(s.shuffled, n_active, s.positions);
@@ -3299,6 +3320,243 @@ int32_t lhb200_state_next_sync_committee_indices(lhb200_state* st, uint64_t out[
     tab.n = 1;
     tab.r[0] = {epoch, 0, DOMAIN_SYNC_COMMITTEE, 0};
     return sample_validators(in, "state_next_sync_committee_indices", epoch, tab, SYNC_COMMITTEE_SIZE, out);
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Committee caches that stay on the device, and attestations verified against them (attest.cuh).
+struct lhb200_committee_cache {
+    lhb200_committee_info info;
+    uint64_t* d_shuffling;   // info.n_active entries, owned
+};
+
+int32_t lhb200_state_committee_cache_create(lhb200_state* st, uint64_t epoch, lhb200_committee_cache** out) {
+    LHB_REQUIRE_READY();
+    if (!st || !out) { set_error("state_committee_cache_create: null argument"); return LHB200_EINVAL; }
+    Ctx& c = ctx();
+    std::lock_guard<std::recursive_mutex> g(c.mu);
+    CommitteeInputs in;
+    CommitteeScratch s;
+    lhb200_committee_info info{};
+    uint64_t* d = nullptr;
+    int32_t rc = committee_shuffle(st, epoch, "state_committee_cache_create", nullptr, in, s, &info, &d);
+    if (!rc) {
+        cudaError_t e = cudaGetLastError();
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
+        if (e != cudaSuccess) rc = cuda_fail(e, "state_committee_cache_create");
+    }
+    if (rc) {
+        if (d) cudaFree(d);
+        return rc;
+    }
+    *out = new lhb200_committee_cache{info, d};
+    return LHB200_OK;
+}
+
+int32_t lhb200_committee_cache_info(const lhb200_committee_cache* cc, lhb200_committee_info* info) {
+    if (!cc || !info) { set_error("committee_cache_info: null argument"); return LHB200_EINVAL; }
+    *info = cc->info;
+    return LHB200_OK;
+}
+
+int32_t lhb200_committee_cache_shuffling(const lhb200_committee_cache* cc, uint64_t* out, uint64_t cap) {
+    LHB_REQUIRE_READY();
+    if (!cc || !out) { set_error("committee_cache_shuffling: null argument"); return LHB200_EINVAL; }
+    if (cap < cc->info.n_active) {
+        set_error("committee_cache_shuffling: cap %llu is below the active count %llu", (unsigned long long)cap,
+                  (unsigned long long)cc->info.n_active);
+        return LHB200_EINVAL;
+    }
+    LHB_CUDA(cudaMemcpy(out, cc->d_shuffling, cc->info.n_active * 8, cudaMemcpyDeviceToHost));
+    return LHB200_OK;
+}
+
+int32_t lhb200_committee_cache_release(lhb200_committee_cache* cc) {
+    if (!cc) return LHB200_OK;
+    if (ctx().ready) cudaFree(cc->d_shuffling);
+    delete cc;
+    return LHB200_OK;
+}
+
+// The argument checks of lhb200_attestations_verify, made before anything is queued
+static int32_t attestation_args(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, int32_t fork,
+                                const lhb200_committee_cache* const* caches, uint32_t n_caches,
+                                const lhb200_pubkey_table* table, const lhb200_fork* fork_info, const uint8_t* gvr,
+                                const uint64_t* rands, const uint8_t* ok, const uint8_t* status,
+                                const uint64_t* indices_offsets, const uint64_t* indices) {
+    const char* fn = "attestations_verify";
+    if (!ssz || !offsets || !caches || !table || !fork_info || !gvr || !ok || !status || !indices != !indices_offsets) {
+        set_error("%s: null argument", fn);
+        return LHB200_EINVAL;
+    }
+    if (n == 0) { set_error("%s: no attestations", fn); return LHB200_EINVAL; }
+    if (fork < LHB200_FORK_BASE || fork > LHB200_FORK_ELECTRA) { set_error("%s: unknown fork %d", fn, fork); return LHB200_EINVAL; }
+    if (n_caches == 0 || n_caches > ATT_MAX_CACHES) {
+        set_error("%s: %u committee caches (1 to %u)", fn, n_caches, ATT_MAX_CACHES);
+        return LHB200_EINVAL;
+    }
+    for (uint32_t k = 0; k < n_caches; k++) {
+        if (!caches[k]) { set_error("%s: null committee cache", fn); return LHB200_EINVAL; }
+        for (uint32_t j = 0; j < k; j++)
+            if (caches[j]->info.epoch == caches[k]->info.epoch) {
+                set_error("%s: two committee caches of epoch %llu", fn, (unsigned long long)caches[k]->info.epoch);
+                return LHB200_EINVAL;
+            }
+    }
+    for (uint32_t i = 0; i < n; i++)
+        if (offsets[i] > offsets[i + 1]) { set_error("%s: offsets not monotone", fn); return LHB200_EINVAL; }
+    if (rands)
+        for (uint32_t i = 0; i < n; i++)
+            if (rands[i] == 0) { set_error("%s: zero random scalar", fn); return LHB200_EINVAL; }
+    return LHB200_OK;
+}
+
+// The call on a borrowed batch handle b: count (one read-back), stage the sets, write the indices, verify.
+static int32_t attestations_on(lhb200_bls_batch* b, AttParams& p, const uint8_t* ssz, const uint64_t* offsets,
+                               const lhb200_pubkey_table* table, const uint64_t* rands, uint8_t* ok, uint8_t* status,
+                               uint8_t* signing_roots, uint64_t* indices_offsets, uint64_t* indices,
+                               uint64_t indices_cap) {
+    const char* fn = "attestations_verify";
+    const uint32_t n = p.n;
+    const bool electra = p.electra, want = indices != nullptr;
+    const uint64_t bytes = offsets[n] - offsets[0];
+    // every set bit is a bit of the records' bytes, so 8 x bytes bounds the indices: the output buffers are sized
+    // before the first launch and the scratch never moves under a queued kernel
+    const uint64_t max_idx = want ? std::min<uint64_t>(indices_cap, 8 * bytes) : 0;
+    cudaStream_t s = bls_batch_stream(b);
+    size_t cub_bytes = 0;
+    if (want && electra)
+        LHB_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, cub_bytes, (const uint64_t*)nullptr, (uint64_t*)nullptr,
+                                                    (int64_t)max_idx, (int64_t)n, (const uint64_t*)nullptr,
+                                                    (const uint64_t*)nullptr, s));
+    const size_t b_ssz = align_up(bytes + 16, 256), b_offs = align_up((n + 1) * 8ull, 256), b_rec = align_up(37ull * n, 256),
+                 b_koff = align_up(4ull * n, 256), b_ooff = align_up(8ull * (n + 1), 256), b_out = align_up(8 * max_idx, 256),
+                 b_out2 = electra ? b_out : 0, b_cub = align_up(cub_bytes, 256);
+    const size_t h_rec = align_up(37ull * n, 64), h_koff = align_up(4ull * n, 64);
+    uint8_t* h = nullptr;
+    uint8_t* d = static_cast<uint8_t*>(bls_batch_aux(b, b_ssz + b_offs + b_rec + b_koff + b_ooff + b_out + b_out2 + b_cub,
+                                                     &h, h_rec + h_koff + 8ull * (n + 1)));
+    if (!d) return LHB200_ENOMEM;
+    uint8_t* d_ssz = d;
+    uint64_t* d_offs = reinterpret_cast<uint64_t*>(d += b_ssz);
+    uint8_t* d_rec = (d += b_offs);
+    uint32_t* d_koff = reinterpret_cast<uint32_t*>(d += b_rec);
+    uint64_t* d_ooff = reinterpret_cast<uint64_t*>(d += b_koff);
+    uint64_t* d_out = reinterpret_cast<uint64_t*>(d += b_ooff);
+    uint64_t* d_out2 = reinterpret_cast<uint64_t*>(d += b_out);
+    void* d_cub = (d += b_out2);
+    uint32_t* hk = reinterpret_cast<uint32_t*>(h + h_rec);
+    uint64_t* ho = reinterpret_cast<uint64_t*>(h + h_rec + h_koff);
+
+    // 1. frame, resolve, count and root every record; read status, count and signing root back (one synchronise)
+    if (bytes) LHB_CUDA(cudaMemcpyAsync(d_ssz, ssz + offsets[0], bytes, cudaMemcpyHostToDevice, s));
+    LHB_CUDA(cudaMemcpyAsync(d_offs, offsets, (n + 1) * 8ull, cudaMemcpyHostToDevice, s));
+    p.ssz = d_ssz;
+    p.offs = d_offs;
+    p.roots = d_rec;
+    p.counts = reinterpret_cast<uint32_t*>(d_rec + 32ull * n);
+    p.status = d_rec + 36ull * n;
+    k_attestation_index_count<<<(unsigned)ceil_div(n, ATT_COUNT_WARPS), 32 * ATT_COUNT_WARPS, 0, s>>>(p);
+    count_launch();
+    LHB_CUDA(cudaGetLastError());
+    LHB_CUDA(cudaMemcpyAsync(h, d_rec, 37ull * n, cudaMemcpyDeviceToHost, s));
+    LHB_CUDA(cudaStreamSynchronize(s));
+    const uint8_t* h_roots = h;
+    const uint32_t* h_counts = reinterpret_cast<const uint32_t*>(h + 32ull * n);
+    const uint8_t* h_st = h + 36ull * n;
+
+    // 2. the sets: the attestations of status 0, in order, with their key-count CSR; the indexed output's CSR
+    std::vector<uint32_t> pk_off(1, 0), set_of;
+    std::vector<uint8_t> sigs, msgs;
+    std::vector<uint64_t> r_sets;
+    uint64_t total = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const uint8_t st = h_st[i];
+        ho[i] = total;
+        if (want && (st == ATT_OK || st == ATT_UNKNOWN_VALIDATOR)) total += h_counts[i];
+        hk[i] = UINT32_MAX;
+        if (st != ATT_OK) continue;
+        if ((uint64_t)pk_off.back() + h_counts[i] >= UINT32_MAX) { set_error("%s: more than 2^32 keys", fn); return LHB200_EINVAL; }
+        hk[i] = pk_off.back();
+        pk_off.push_back(pk_off.back() + h_counts[i]);
+        set_of.push_back(i);
+        sigs.insert(sigs.end(), ssz + offsets[i] + ATT_SIG, ssz + offsets[i] + ATT_SIG + 96);
+        msgs.insert(msgs.end(), h_roots + 32ull * i, h_roots + 32ull * i + 32);
+        if (rands) r_sets.push_back(rands[i]);
+    }
+    ho[n] = total;
+    if (want && total > indices_cap) {
+        set_error("%s: indices_cap %llu is below the %llu attesting indices", fn, (unsigned long long)indices_cap,
+                  (unsigned long long)total);
+        return LHB200_EINVAL;
+    }
+    const uint32_t n_sets = (uint32_t)set_of.size();
+
+    // 3. stage the sets (grouped by signing root), then write their key indices on the device
+    uint32_t* d_keys = nullptr;
+    if (n_sets)
+        if (int32_t rc = bls_batch_stage_table(b, table, sigs.data(), msgs.data(), pk_off.data(),
+                                               rands ? r_sets.data() : nullptr, n_sets, &d_keys))
+            return rc;
+    LHB_CUDA(cudaMemcpyAsync(d_koff, hk, 4ull * n, cudaMemcpyHostToDevice, s));
+    if (want) LHB_CUDA(cudaMemcpyAsync(d_ooff, ho, 8ull * (n + 1), cudaMemcpyHostToDevice, s));
+    const AttWrite wr{d_koff, d_keys, want ? d_ooff : nullptr, want ? (electra ? d_out2 : d_out) : nullptr};
+    k_attestation_index_write<<<n, ATT_WRITE_THREADS, 0, s>>>(p, wr);
+    count_launch();
+    if (want && electra) {   // sort_unstable per attestation: one segmented sort over the output CSR
+        LHB_CUDA(cub::DeviceSegmentedSort::SortKeys(d_cub, cub_bytes, d_out2, d_out, (int64_t)total, (int64_t)n,
+                                                    d_ooff, d_ooff + 1, s));
+        count_launch();
+    }
+    LHB_CUDA(cudaGetLastError());
+
+    // 4. the batch check, then the outputs
+    std::vector<uint8_t> set_st(n_sets);
+    uint8_t verdict = 0;
+    if (n_sets) {
+        if (int32_t rc = bls_batch_finish(b, &verdict, set_st.data())) return rc;
+    } else {
+        LHB_CUDA(cudaStreamSynchronize(s));
+    }
+    if (want && total) LHB_CUDA(cudaMemcpy(indices, d_out, total * 8, cudaMemcpyDeviceToHost));
+    if (want) memcpy(indices_offsets, ho, 8ull * (n + 1));
+    for (uint32_t i = 0; i < n; i++) status[i] = h_st[i];
+    for (uint32_t j = 0; j < n_sets; j++) status[set_of[j]] = set_st[j];
+    if (signing_roots) memcpy(signing_roots, h_roots, 32ull * n);
+    *ok = verdict;
+    return LHB200_OK;
+}
+
+int32_t lhb200_attestations_verify(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, int32_t fork,
+                                   const lhb200_committee_cache* const* caches, uint32_t n_caches,
+                                   const lhb200_pubkey_table* table, const lhb200_fork* fork_info,
+                                   const uint8_t genesis_validators_root[32], const uint64_t* rands, uint8_t* ok,
+                                   uint8_t* status, uint8_t* signing_roots, uint64_t* indices_offsets,
+                                   uint64_t* indices, uint64_t indices_cap) {
+    LHB_REQUIRE_READY();
+    if (int32_t rc = attestation_args(ssz, offsets, n, fork, caches, n_caches, table, fork_info,
+                                      genesis_validators_root, rands, ok, status, indices_offsets, indices))
+        return rc;
+    AttParams p{};
+    p.n = n;
+    p.electra = fork == LHB200_FORK_ELECTRA;
+    p.n_caches = n_caches;
+    for (uint32_t k = 0; k < n_caches; k++)
+        p.cache[k] = {caches[k]->d_shuffling, caches[k]->info.epoch, (uint32_t)caches[k]->info.n_active,
+                      (uint32_t)caches[k]->info.committees_per_slot};
+    p.table_len = lhb200_pubkey_table_len(table);
+    p.fork_epoch = fork_info->epoch;
+    auto be32 = [](const uint8_t* q) {
+        return ((uint32_t)q[0] << 24) | ((uint32_t)q[1] << 16) | ((uint32_t)q[2] << 8) | (uint32_t)q[3];
+    };
+    p.version[0] = be32(fork_info->previous_version);
+    p.version[1] = be32(fork_info->current_version);
+    for (int k = 0; k < 8; k++) p.gvr[k] = be32(genesis_validators_root + 4 * k);
+    lhb200_bls_batch* b = bls_pool_borrow(n);
+    if (!b) return LHB200_ENOMEM;
+    const int32_t rc = attestations_on(b, p, ssz, offsets, table, rands, ok, status, signing_roots, indices_offsets,
+                                       indices, indices_cap);
+    bls_pool_return(b);
+    return rc;
 }
 
 }  // extern "C"

@@ -444,3 +444,90 @@ def blind_block_electra(block, transactions_root: bytes, withdrawals_root: bytes
                deposit_requests_root=deposit_requests_root, withdrawal_requests_root=withdrawal_requests_root)
     v["body"]["execution_payload"] = {n: hdr[n] for n, _ in S.ExecutionPayloadHeaderElectra[1]}
     return v, S.serialize(S.BLINDED_BEACON_BLOCK_BY_FORK["electra"], v)
+
+
+# ---------------------------------------------------------------------------------------------------------
+# Signed Attestations over a committee cache (lhb200_attestations_verify, lighthouse_b200.attestations).  Validator i
+# holds interop key i (interop_pubkey_table); an attestation is signed by (sum of its attesters' secret keys mod r) .
+# H(signing root) through the CUDA library's lhb200_sign, which is the aggregate of the attesters' own signatures.
+def attestation_data_ssz(slot, index, beacon_block_root, source, target):
+    """AttestationData {slot, index, beacon_block_root, source: (epoch, root), target: (epoch, root)}: 128 bytes."""
+    return (struct.pack("<QQ", slot, index) + beacon_block_root + struct.pack("<Q", source[0]) + source[1]
+            + struct.pack("<Q", target[0]) + target[1])
+
+
+def attestation_data_root(data):
+    """hash_tree_root(AttestationData): 8 leaves, the checkpoints as 2-leaf containers."""
+    def leaf(b):
+        return b + bytes(32 - len(b))
+    z = bytes(32)
+    l0 = _sha(_sha(leaf(data[0:8]) + leaf(data[8:16])) + _sha(data[16:48] + _sha(leaf(data[48:56]) + data[56:88])))
+    l1 = _sha(_sha(_sha(leaf(data[88:96]) + data[96:128]) + z) + _sha(z + z))
+    return _sha(l0 + l1)
+
+
+def attestation_ssz(bits, data, signature, committee_bits=None):
+    """SSZ of an Attestation: Base to Deneb {aggregation_bits: Bitlist[2048], data, signature}, or with committee_bits
+    (an int, Bitvector[64]) Electra's {aggregation_bits: Bitlist[131072], data, signature, committee_bits}."""
+    bits = np.append(np.asarray(bits, dtype=np.uint8), np.uint8(1))
+    tail = b"" if committee_bits is None else struct.pack("<Q", committee_bits)
+    fixed = 228 + len(tail)
+    return struct.pack("<I", fixed) + data + signature + tail + np.packbits(bits, bitorder="little").tobytes()
+
+
+ATTESTATION_KINDS = ("unaggregated", "aggregate", "electra")
+
+
+def signed_attestations(cache, kind, n, sks, fork_info, gvr=MAINNET_GVR, seed=0, slot=None, n_committees=2,
+                        committees_per_attestation=4, fill=1.0):
+    """n signed Attestations over a committees.CommitteeCache whose validators hold the interop keys `sks`
+    (interop_secret_keys), signed for fork_info = (previous_version, current_version, fork epoch) and gvr.
+      unaggregated  one bit each, at `slot` (default the epoch's first), over n_committees committees of that slot:
+                    attestation j is committee j % n_committees, member j // n_committees; the attestations of one
+                    committee share their AttestationData, as gossip does.
+      aggregate     attestation j is committee j % committees_per_slot of slot epoch_start + (j // committees_per_slot)
+                    % 32, with `fill` of its bits set (1.0: all).
+      electra       Electra: attestation j covers committees_per_attestation consecutive committees (mod
+                    committees_per_slot) of slot epoch_start + j % 32 in committee_bits, with `fill` of the bits set.
+    The target epoch is the cache's, so fork_info's epoch picks the version.  Needs lighthouse_b200.init()."""
+    from . import bls
+    assert kind in ATTESTATION_KINDS
+    rng = np.random.default_rng(seed)
+    epoch = cache.initialized_epoch
+    start = epoch * 32
+    cps = cache.committees_per_slot()
+    prev, cur, fork_epoch = fork_info
+    domain = attester_domain(bytes(prev) if epoch < fork_epoch else bytes(cur), gvr)
+    source = (max(epoch - 1, 0), _sha(b"source" + struct.pack("<QQ", seed, epoch)))
+    target = (epoch, _sha(b"target" + struct.pack("<QQ", seed, epoch)))
+    records = []   # (bits, data, committee_bits or None, attesters)
+    for j in range(n):
+        if kind == "unaggregated":
+            s = start if slot is None else slot
+            index = (j % n_committees) % cps
+            members = cache.get_beacon_committee(s, index).committee
+            bits = np.zeros(len(members), dtype=np.uint8)
+            if len(members):
+                bits[(j // n_committees) % len(members)] = 1
+            bbr = _sha(b"head" + struct.pack("<QQQ", seed, s, index))
+            records.append((bits, attestation_data_ssz(s, index, bbr, source, target), None, members[bits == 1]))
+            continue
+        if kind == "aggregate":
+            s, indices = start + (j // cps) % 32, [j % cps]
+        else:
+            k = min(committees_per_attestation, cps)
+            s, indices = start + j % 32, sorted({(j * k + t) % cps for t in range(k)})
+        members = np.concatenate([cache.get_beacon_committee(s, c).committee for c in indices])
+        bits = (rng.random(len(members)) < fill).astype(np.uint8)
+        if len(members) and not bits.any():
+            bits[int(rng.integers(0, len(members)))] = 1
+        bbr = _sha(b"head" + struct.pack("<QQ", seed, j))
+        data = attestation_data_ssz(s, 0 if kind == "electra" else indices[0], bbr, source, target)
+        cbits = sum(1 << c for c in indices) if kind == "electra" else None
+        records.append((bits, data, cbits, members[bits == 1]))
+    # (an attestation without attesters is signed with key 1: its set has no keys and fails with status 4 anyway)
+    agg = [sum(sks[int(v)] for v in attesters) % CURVE_ORDER or 1 for _, _, _, attesters in records]
+    msgs = b"".join(_sha(attestation_data_root(data) + domain) for _, data, _, _ in records)
+    sigs = bls.sign(b"".join(a.to_bytes(32, "big") for a in agg), msgs)
+    return [attestation_ssz(bits, data, sigs[96 * j:96 * j + 96], cbits)
+            for j, (bits, data, cbits, _) in enumerate(records)]

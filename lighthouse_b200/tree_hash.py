@@ -399,6 +399,14 @@ class ResidentState:
         return CommitteeCache(info.epoch, shuffling[:info.n_active], positions[:n], info.committees_per_slot,
                               bytes(info.seed))
 
+    def device_committee_cache(self, epoch):
+        """The same cache left on the device (lhb200_state_committee_cache_create) -> a
+        committees.DeviceCommitteeCache, independent of this handle once made.  Refused as committee_cache is."""
+        from .committees import DeviceCommitteeCache
+        h = C.c_void_p()
+        check(lib.lhb200_state_committee_cache_create(self._h, epoch, C.byref(h)), "lhb200_state_committee_cache_create")
+        return DeviceCommitteeCache(h)
+
     def beacon_proposer_indices(self):
         """BeaconState::get_beacon_proposer_indices: the proposer of each of the current epoch's 32 slots."""
         out = (C.c_uint64 * 32)()
