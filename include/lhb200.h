@@ -433,6 +433,79 @@ LHB200_API int32_t lhb200_attestations_verify(const uint8_t* ssz, const uint64_t
  * lhb200_bls_batch_plan; gt576 or plan may be NULL) of the batch check the calling thread's last
  * lhb200_attestations_verify ran.  LHB200_EINVAL when that call verified no set. */
 LHB200_API int32_t lhb200_debug_attestations_last(uint8_t gt576[576], uint32_t* plan, uint32_t n_words);
+/* Every signature set of n SignedBeaconBlocks of one fork, built against a resident BeaconState and verified in one
+ * batch: BlockSignatureVerifier::include_all_signatures (block_signature_verifier.rs:150-173, signature_sets.rs), the
+ * call signature_verify_chain_segment, SignatureVerifiedBlock::new (n = 1) and the gossip path (n = 1,
+ * LHB200_BLOCK_SKIP_PROPOSAL) make.
+ *   ssz, offsets  n SignedBeaconBlock encodings of `fork`, which must be the state's fork.
+ *   block_roots   n x 32: each block's root (ConsensusContext::set_current_block_root), signed by the proposal.
+ *   st            an unsharded resident state advanced to the blocks' epoch.  Its fork, genesis_validators_root, slot,
+ *                 validator records and current_sync_committee are read from the handle, not from the caller.
+ *   caches        the committee caches of the attestations' epochs (as for lhb200_attestations_verify).
+ *   table         the pubkey table; a validator index at or above min(table length, the state's validator count) is
+ *                 UNKNOWN_VALIDATOR.
+ *   versions      genesis_fork_version (BLS-to-execution changes, consolidations) and capella_fork_version (exits
+ *                 from Deneb on, EIP-7044).
+ *   rands         optional: rands[j] (nonzero) scales set j of `sets`; n_rands at least the sets the blocks contribute.
+ *   *ok           1 only when every set was constructed and the batch check passed.
+ *   block_status  n bytes: the code of the block's first failing set in push order, or 0.
+ *   sets, *n_sets every set in push order (proposal, randao, proposer slashings, attester slashings, attestations,
+ *                 exits, sync aggregate, BLS-to-execution changes, consolidations), with its status: 0, the set's
+ *                 verify status 1-6, or a construction code 10-17.  A set that fails construction stays out of the
+ *                 batch.
+ * Domains: get_domain(epoch, type, state.fork, gvr), except exits from Deneb on (capella_fork_version), and
+ * BLS-to-execution changes and consolidations (genesis_fork_version).  The proposer of a block is get_beacon_proposer_index(block.slot); a block
+ * outside the state's current epoch gets SLOT_OUT_OF_BOUNDS on its proposal and RANDAO sets.  The sync aggregate's
+ * keys are the current_sync_committee members' validator indices, found by matching the resident records' pubkeys
+ * (the smallest index wins); an unmatched participant gives PUBKEY_DECOMPRESSION.  A BLS-to-execution change's key is
+ * its from_bls_pubkey, decompressed and key-validated on the device (PublicKey::deserialize): an infinity, off-curve or
+ * non-subgroup key gives PUBKEY_DECOMPRESSION.  All-zero bits with the infinity
+ * signature give no set.  Deposits carry no set (block_signature_verifier.rs:169).  The caller keeps the fork-schedule
+ * check (InconsistentBlockFork), which needs the ChainSpec.
+ * Refusals -> LHB200_EINVAL, nothing launched: null arguments, n == 0, a fork other than the state's, a sharded state,
+ * a SignedBeaconBlock whose 100-byte fixed part does not frame its message, malformed offsets or lengths in the block,
+ * its body or any list a set is read from, sets_cap or n_rands below the sets the blocks contribute, a zero scalar, and
+ * the committee-cache errors of lhb200_attestations_verify.  The fields no set reads (deposits, the execution payload,
+ * blob commitments) are not framed here: the blocks' roots, which the caller already has, are where they are checked.
+ * The launch count and the number of host synchronises depend on neither n, the number of sets nor the validator
+ * count. */
+#define LHB200_BSET_PROPOSAL 0
+#define LHB200_BSET_RANDAO 1
+#define LHB200_BSET_PROPOSER_SLASHING 2
+#define LHB200_BSET_ATTESTER_SLASHING 3
+#define LHB200_BSET_ATTESTATION 4
+#define LHB200_BSET_EXIT 5
+#define LHB200_BSET_SYNC_AGGREGATE 6
+#define LHB200_BSET_BLS_CHANGE 7
+#define LHB200_BSET_CONSOLIDATION 8
+#define LHB200_BLOCK_INCORRECT_PROPOSER 15   /* block.proposer_index != the state's proposer (IncorrectBlockProposer) */
+#define LHB200_BLOCK_SLOT_OUT_OF_BOUNDS 16   /* the block's epoch is not the state's current epoch (SlotOutOfBounds) */
+#define LHB200_BLOCK_PUBKEY_DECOMPRESSION 17 /* a sync participant's key matches no validator record, or a
+                                                BLS-to-execution change's key does not decode and validate */
+#define LHB200_BLOCK_SKIP_PROPOSAL 1         /* include_all_signatures_except_proposal (the gossip path) */
+#define LHB200_BLOCK_MAX_SETS 199            /* sets one block can contribute (mainnet preset, pre-Electra) */
+typedef struct { uint8_t genesis_fork_version[4], capella_fork_version[4]; } lhb200_chain_versions;
+typedef struct {
+    uint32_t block;          /* index of the block in the call */
+    uint16_t item;           /* index in its body list; proposer / attester slashings: 2 i + (0 | 1); else 0 */
+    uint8_t kind;            /* LHB200_BSET_* */
+    uint8_t status;          /* 0, the set's verify status 1-6, or a construction code 10-17 */
+    uint8_t signing_root[32];
+} lhb200_block_set;
+LHB200_API int32_t lhb200_block_signatures_verify(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, int32_t fork,
+                                                  uint32_t flags, const uint8_t* block_roots, lhb200_state* st,
+                                                  const lhb200_committee_cache* const* caches, uint32_t n_caches,
+                                                  const lhb200_pubkey_table* table,
+                                                  const lhb200_chain_versions* versions, const uint64_t* rands,
+                                                  uint64_t n_rands, uint8_t* ok, uint8_t* block_status,
+                                                  lhb200_block_set* sets, uint64_t sets_cap, uint64_t* n_sets);
+/* Test hook: lhb200_debug_attestations_last for the calling thread's last lhb200_block_signatures_verify.  Both hooks
+ * read one per-thread record, so each reports the last batch check of either call on this thread. */
+LHB200_API int32_t lhb200_debug_block_signatures_last(uint8_t gt576[576], uint32_t* plan, uint32_t n_words);
+/* Test hook: the kernel launches the calling thread's last lhb200_block_signatures_verify made besides its batch
+ * check's (library-wide launch counter; other threads' launches meanwhile are counted too), and the host synchronises
+ * it made, the batch check's result included. */
+LHB200_API int32_t lhb200_debug_block_signatures_counts(uint64_t* launches, uint64_t* syncs);
 /* Test hook: final-exponentiated product of the last verify as 12 x 48-byte big-endian Fp (tower order
  * c0.c0.c0 .. c1.c2.c1).  NOTE: this is the cube of the canonical GT element (3 is coprime to r). */
 LHB200_API int32_t lhb200_bls_batch_gt(lhb200_bls_batch* b, uint8_t out576[576]);

@@ -162,6 +162,10 @@ _sig("lhb200_committee_cache_release", C.c_int32, vp)
 _sig("lhb200_attestations_verify", C.c_int32, vp, vp, C.c_uint32, C.c_int32, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp,
      vp, vp, C.c_uint64)
 _sig("lhb200_debug_attestations_last", C.c_int32, vp, vp, C.c_uint32)
+_sig("lhb200_block_signatures_verify", C.c_int32, vp, vp, C.c_uint32, C.c_int32, C.c_uint32, vp, vp, vp, C.c_uint32,
+     vp, vp, vp, C.c_uint64, vp, vp, vp, C.c_uint64, vp)
+_sig("lhb200_debug_block_signatures_last", C.c_int32, vp, vp, C.c_uint32)
+_sig("lhb200_debug_block_signatures_counts", C.c_int32, vp, vp)
 
 
 class ListEdit(C.Structure):
@@ -179,3 +183,14 @@ class CommitteeInfo(C.Structure):
 class Fork(C.Structure):
     """lhb200_fork"""
     _fields_ = [("previous_version", C.c_uint8 * 4), ("current_version", C.c_uint8 * 4), ("epoch", C.c_uint64)]
+
+
+class ChainVersions(C.Structure):
+    """lhb200_chain_versions"""
+    _fields_ = [("genesis_fork_version", C.c_uint8 * 4), ("capella_fork_version", C.c_uint8 * 4)]
+
+
+class BlockSet(C.Structure):
+    """lhb200_block_set"""
+    _fields_ = [("block", C.c_uint32), ("item", C.c_uint16), ("kind", C.c_uint8), ("status", C.c_uint8),
+                ("signing_root", C.c_uint8 * 32)]

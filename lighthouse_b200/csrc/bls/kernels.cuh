@@ -347,13 +347,17 @@ __global__ void __launch_bounds__(BLS_BLOCK) k_table_import(const uint8_t* __res
     out[i] = m;
 }
 
-__global__ void __launch_bounds__(BLS_BLOCK) k_pk_aggregate_indexed(const G1Mont* __restrict__ table, uint32_t table_len,
-                                                                     const uint32_t* __restrict__ indices,
-                                                                     const uint32_t* __restrict__ offsets,
-                                                                     const uint64_t* __restrict__ rands, uint32_t n,
-                                                                     G1Proj3* __restrict__ out_p,
-                                                                     uint8_t* __restrict__ pk_status,
-                                                                     uint32_t* __restrict__ fail) {
+// The body of k_pk_aggregate_indexed and k_pk_aggregate_indexed_local.  LOCAL: indices at or above table_len name
+// local[idx - table_len] (keys a call decoded for itself, lhb200_block_signatures_verify's BLS-to-execution changes);
+// without it the body is the table-only kernel every other caller launches.
+template <bool LOCAL>
+__device__ __forceinline__ void pk_aggregate_indexed_body(const G1Mont* __restrict__ table, uint32_t table_len,
+                                                          const G1Mont* __restrict__ local, uint32_t local_len,
+                                                          const uint32_t* __restrict__ indices,
+                                                          const uint32_t* __restrict__ offsets,
+                                                          const uint64_t* __restrict__ rands, uint32_t n,
+                                                          G1Proj3* __restrict__ out_p, uint8_t* __restrict__ pk_status,
+                                                          uint32_t* __restrict__ fail) {
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const uint32_t lo = offsets[i], hi = offsets[i + 1];
         uint8_t st = SET_OK;
@@ -362,9 +366,9 @@ __global__ void __launch_bounds__(BLS_BLOCK) k_pk_aggregate_indexed(const G1Mont
         if (hi <= lo) st = SET_NO_KEYS;
         for (uint32_t j = lo; j < hi && st == SET_OK; j++) {
             const uint32_t idx = __ldg(indices + j);
-            if (idx >= table_len) { st = SET_PK_DECODE; break; }
+            if (idx >= table_len && (!LOCAL || idx - table_len >= local_len)) { st = SET_PK_DECODE; break; }
             G1Affine a;
-            const G1Mont& m = table[idx];
+            const G1Mont& m = LOCAL && idx >= table_len ? local[idx - table_len] : table[idx];
             a.x = m.x; a.y = m.y; a.inf = 0;
             jac_add_affine(acc, acc, a);
         }
@@ -381,6 +385,23 @@ __global__ void __launch_bounds__(BLS_BLOCK) k_pk_aggregate_indexed(const G1Mont
         pk_status[i] = st;
         if (st != SET_OK) atomicOr(fail, 1u);
     }
+}
+
+__global__ void __launch_bounds__(BLS_BLOCK) k_pk_aggregate_indexed(const G1Mont* __restrict__ table, uint32_t table_len,
+                                                                     const uint32_t* __restrict__ indices,
+                                                                     const uint32_t* __restrict__ offsets,
+                                                                     const uint64_t* __restrict__ rands, uint32_t n,
+                                                                     G1Proj3* __restrict__ out_p,
+                                                                     uint8_t* __restrict__ pk_status,
+                                                                     uint32_t* __restrict__ fail) {
+    pk_aggregate_indexed_body<false>(table, table_len, nullptr, 0, indices, offsets, rands, n, out_p, pk_status, fail);
+}
+__global__ void __launch_bounds__(BLS_BLOCK) k_pk_aggregate_indexed_local(
+    const G1Mont* __restrict__ table, uint32_t table_len, const G1Mont* __restrict__ local, uint32_t local_len,
+    const uint32_t* __restrict__ indices, const uint32_t* __restrict__ offsets, const uint64_t* __restrict__ rands,
+    uint32_t n, G1Proj3* __restrict__ out_p, uint8_t* __restrict__ pk_status, uint32_t* __restrict__ fail) {
+    pk_aggregate_indexed_body<true>(table, table_len, local, local_len, indices, offsets, rands, n, out_p, pk_status,
+                                    fail);
 }
 
 __global__ void __launch_bounds__(BLS_BLOCK) k_hash_to_g2(const uint8_t* __restrict__ msgs, uint32_t n,

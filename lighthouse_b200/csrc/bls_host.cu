@@ -274,11 +274,18 @@ struct lhb200_bls_batch {
     size_t d_aux_bytes = 0;
     uint8_t* h_aux = nullptr;                // pinned
     size_t h_aux_bytes = 0;
+    // call-local keys (bls_batch_local_keys): key indices at or above table->len name d_local[idx - table->len]; only
+    // a borrowed handle sets them, and borrowing or returning it clears them
+    G1Mont* d_local = nullptr;
+    uint8_t* d_local96 = nullptr;            // their uncompressed form, then a u32 count of undecodable keys
+    uint32_t local_len = 0, local_cap = 0;
 };
 
 static void batch_free(lhb200_bls_batch* b) {
     if (!b) return;
     if (b->d_indices) cudaFree(b->d_indices);
+    if (b->d_local) cudaFree(b->d_local);
+    if (b->d_local96) cudaFree(b->d_local96);
     void* ptrs[] = {b->d_sigs, b->d_msgs, b->d_pks, b->d_offsets, b->d_rands, b->d_sigr, b->d_sig_tmp[0],
                     b->d_sig_tmp[1], b->d_p, b->d_h, b->d_f, b->d_f_tmp[0], b->d_f_tmp[1], b->d_flast, b->d_gt,
                     b->d_status, b->d_pk_status, b->d_fail, b->d_ok, b->d_mc_scratch, b->d_neg_g1, b->d_pk_part,
@@ -1096,6 +1103,13 @@ static int32_t launch_hash(lhb200_bls_batch* b, const Plan& p, uint64_t& launche
 // (high-priority) stream that copies the chunk, as soon as its keys have landed
 static int32_t launch_keys(lhb200_bls_batch* b, const Plan& p, cudaStream_t s, uint64_t& launches) {
     const uint32_t key = p.w[LHB200_PLAN_KEY], grid = p.w[LHB200_PLAN_LANE_GRID];
+    if (key == LHB200_K_PK_AGGREGATE_INDEXED && b->local_len) {
+        k_pk_aggregate_indexed_local<<<grid, BLS_BLOCK, 0, s>>>(b->table->d_keys, (uint32_t)b->table->len, b->d_local,
+                                                               b->local_len, b->d_indices, b->in_offsets, b->in_rands,
+                                                               b->n, b->d_p, b->d_pk_status, b->d_fail);
+        launches++;
+        return LHB200_OK;
+    }
     if (key == LHB200_K_PK_AGGREGATE_INDEXED) {
         k_pk_aggregate_indexed<<<grid, BLS_BLOCK, 0, s>>>(b->table->d_keys, (uint32_t)b->table->len, b->d_indices,
                                                          b->in_offsets, b->in_rands, b->n, b->d_p, b->d_pk_status, b->d_fail);
@@ -1951,13 +1965,16 @@ namespace {
 thread_local Fp12 t_last_gt;                          // the calling thread's last bls_batch_finish (test hook)
 thread_local uint32_t t_last_plan[LHB200_PLAN_WORDS];
 thread_local bool t_last_valid = false;
+thread_local uint64_t t_last_launches = 0;            // the launches of that batch check
 }  // namespace
 
 namespace lhb200 {
 lhb200_bls_batch* bls_pool_borrow(uint32_t n_sets) {
     t_last_valid = false;
+    t_last_launches = 0;
     lhb200_bls_batch* b = pool_acquire(n_sets, 0);
     if (!b) set_error("bls_pool_borrow: no batch handle for %u sets", n_sets);
+    else b->local_len = 0;
     return b;
 }
 
@@ -1965,7 +1982,36 @@ void bls_pool_return(lhb200_bls_batch* b) {
     cudaStreamSynchronize(b->s_main);
     cudaStreamSynchronize(b->s2);
     cudaStreamSynchronize(b->s3);
+    b->local_len = 0;
     pool_release(b);
+}
+
+// PublicKey::deserialize + key_validate of n compressed keys already on the device (d_pk48), queued on the handle's
+// stream: d_status[i] as lhb200_g1_decompress_validate reports it (0 ok, 1 infinity, 2 bad encoding or off the curve,
+// 3 outside the subgroup), and the keys imported like the pubkey table's, as the call-local keys the next
+// verify resolves key indices table->len + i into.  Two launches.
+int32_t bls_batch_local_keys(lhb200_bls_batch* b, const uint8_t* d_pk48, uint32_t n, uint8_t* d_status) {
+    b->local_len = 0;
+    if (n == 0) return LHB200_OK;
+    if (n > b->local_cap) {
+        LHB_CUDA(cudaStreamSynchronize(b->s_main));
+        if (b->d_local) cudaFree(b->d_local);
+        if (b->d_local96) cudaFree(b->d_local96);
+        b->d_local = nullptr;
+        b->d_local96 = nullptr;
+        b->local_cap = 0;
+        LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&b->d_local), (size_t)n * sizeof(G1Mont)));
+        LHB_CUDA(cudaMalloc(reinterpret_cast<void**>(&b->d_local96), (size_t)n * 96 + 16));
+        b->local_cap = n;
+    }
+    uint32_t* d_bad = reinterpret_cast<uint32_t*>(b->d_local96 + (size_t)n * 96);
+    LHB_CUDA(cudaMemsetAsync(d_bad, 0, 4, b->s_main));
+    k_g1_decompress_validate<<<cdiv(n, BLS_BLOCK), BLS_BLOCK, 0, b->s_main>>>(d_pk48, n, b->d_local96, d_status);
+    k_table_import<<<cdiv(n, BLS_BLOCK), BLS_BLOCK, 0, b->s_main>>>(b->d_local96, n, b->d_local, d_bad);
+    count_launch(2);
+    LHB_CUDA(cudaGetLastError());
+    b->local_len = n;
+    return LHB200_OK;
 }
 
 cudaStream_t bls_batch_stream(const lhb200_bls_batch* b) { return b->s_main; }
@@ -2026,6 +2072,7 @@ int32_t bls_batch_finish(lhb200_bls_batch* b, uint8_t* ok, uint8_t* set_status) 
     if (int32_t rc = lhb200_bls_batch_result(b, b->s_main, ok, set_status)) return rc;
     memcpy(&t_last_gt, h_gt, sizeof(Fp12));
     memcpy(t_last_plan, b->plan, sizeof t_last_plan);
+    t_last_launches = b->launches_last;
     t_last_valid = true;
     return LHB200_OK;
 }
@@ -2038,4 +2085,12 @@ extern "C" LHB200_API int32_t lhb200_debug_attestations_last(uint8_t gt576[576],
     if (gt576) gt_to_bytes(t_last_gt, gt576);
     if (plan) memcpy(plan, t_last_plan, sizeof(uint32_t) * std::min<uint32_t>(n_words, LHB200_PLAN_WORDS));
     return LHB200_OK;
+}
+// The same for lhb200_block_signatures_verify, which runs its batch check on a borrowed handle the same way (the two
+// hooks read one per-thread record: each reports the last call of either kind)
+extern "C" LHB200_API int32_t lhb200_debug_block_signatures_last(uint8_t gt576[576], uint32_t* plan, uint32_t n_words) {
+    return lhb200_debug_attestations_last(gt576, plan, n_words);
+}
+namespace lhb200 {
+uint64_t bls_last_batch_launches() { return t_last_launches; }
 }

@@ -65,5 +65,7 @@ int32_t bls_batch_stage_table(lhb200_bls_batch* b, const lhb200_pubkey_table* ta
                               const uint8_t* msgs, const uint32_t* pk_offsets, const uint64_t* rands, uint32_t n_sets,
                               uint32_t** d_key_indices);
 int32_t bls_batch_finish(lhb200_bls_batch* b, uint8_t* ok, uint8_t* set_status);
+int32_t bls_batch_local_keys(lhb200_bls_batch* b, const uint8_t* d_pk48, uint32_t n, uint8_t* d_status);
+uint64_t bls_last_batch_launches();   // launches of the calling thread's last bls_batch_finish (0: none)
 
 }  // namespace lhb200

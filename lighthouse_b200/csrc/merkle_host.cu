@@ -13,7 +13,7 @@
 #include <cub/device/device_segmented_sort.cuh>
 #include "ctx.h"
 #include "merkle.cuh"
-#include "attest.cuh"
+#include "block_sigs.cuh"
 
 namespace lhb200 {
 
@@ -3557,6 +3557,551 @@ int32_t lhb200_attestations_verify(const uint8_t* ssz, const uint64_t* offsets, 
                                        indices, indices_cap);
     bls_pool_return(b);
     return rc;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------
+// The signature sets of SignedBeaconBlocks against a resident state (block_sigs.cuh): BlockSignatureVerifier::
+// include_all_signatures (block_signature_verifier.rs:150-173) with the sets of signature_sets.rs.  The host walks the
+// SSZ offsets and copies the signed objects out; every hash runs on the device.
+namespace lhb200 {
+namespace {
+constexpr uint32_t DOMAIN_RANDAO = 2, DOMAIN_VOLUNTARY_EXIT = 4, DOMAIN_BLS_TO_EXECUTION_CHANGE = 0x0A,
+                   DOMAIN_CONSOLIDATION = 0x0B;
+constexpr uint32_t SIGNED_BLOCK_FIXED = 100, SYNC_BITS = 220, SYNC_SIG = 284;
+// KEY_LOCAL: a BLS-to-execution change's from_bls_pubkey, decoded on the device into the batch's call-local keys
+enum : uint8_t { KEY_PROPOSER, KEY_INDEX, KEY_INDEX_LIST, KEY_SYNC, KEY_PAIR, KEY_ATTESTATION, KEY_LOCAL };
+
+struct BlockSet {
+    uint32_t block;
+    uint16_t item;
+    uint8_t kind, status = 0;
+    uint8_t key_src;
+    uint64_t key_at = 0;   // offset in ssz of the index, the index pair, the index list or the sync bits
+    uint32_t key_n = 0;    // KEY_INDEX_LIST: how many indices; KEY_LOCAL: which call-local key
+    uint64_t sig_at = 0;   // offset in ssz of the signature
+    uint32_t ref = 0;      // its descriptor, or for KEY_ATTESTATION its attestation record
+    uint32_t key_lo = 0, key_cnt = 0;   // its keys in the host key list once constructed
+};
+
+// What the walk gathers: the sets in push order, the descriptors of the non-attestation sets and the objects they
+// root, and the attestation records re-laid out in lhb200_attestations_verify's order
+struct BlockWalk {
+    std::vector<BlockSet> sets;
+    std::vector<BlockSetDesc> desc;
+    std::vector<uint8_t> objects;
+    std::vector<uint8_t> atts;
+    std::vector<uint64_t> att_offs{0};
+    std::vector<uint64_t> att_sig;   // offset in ssz of each record's signature
+    std::vector<uint64_t> slot, proposer;   // per block
+    std::vector<uint8_t> local_pks;         // the changes' from_bls_pubkey, 48 bytes each
+};
+
+inline uint64_t rd64(const uint8_t* p) {
+    uint64_t v;
+    memcpy(&v, p, 8);
+    return v;
+}
+inline uint32_t be_word32(const uint8_t* q) {
+    return ((uint32_t)q[0] << 24) | ((uint32_t)q[1] << 16) | ((uint32_t)q[2] << 8) | (uint32_t)q[3];
+}
+
+// The offset table of a list of variable-size items at s[0, len): item k is [b[k], b[k + 1])
+bool item_bounds(const uint8_t* s, uint64_t len, uint64_t max_n, std::vector<uint64_t>& b) {
+    b.assign(1, 0);
+    if (len == 0) return true;
+    if (len < 4) return false;
+    const uint32_t first = rd32(s);
+    if (first % 4 || first == 0 || first > len || first / 4 > max_n) return false;
+    b.clear();
+    for (uint32_t i = 0; i < first / 4; i++) b.push_back(rd32(s + 4 * i));
+    b.push_back(len);
+    for (size_t i = 0; i + 1 < b.size(); i++)
+        if (b[i] > b[i + 1]) return false;
+    return true;
+}
+
+struct BlockWalker {
+    const uint8_t* ssz;
+    const ForkLayout& fl;
+    int32_t fork;
+    BlockWalk& w;
+
+    // a descriptor over the `n` bytes of its object at ssz + at (none for BSO_EPOCH)
+    uint32_t describe(uint32_t object, uint64_t at, uint32_t n, uint64_t epoch, uint32_t domain) {
+        BlockSetDesc d{w.objects.size(), epoch, object, domain, 0, 0};
+        w.objects.insert(w.objects.end(), ssz + at, ssz + at + n);
+        w.desc.push_back(d);
+        return (uint32_t)w.desc.size() - 1;
+    }
+    void push(uint32_t blk, uint16_t item, uint8_t kind, uint8_t key_src, uint64_t key_at, uint64_t sig_at, uint32_t ref,
+              uint32_t key_n = 0) {
+        BlockSet s{blk, item, kind};
+        s.key_src = key_src;
+        s.key_at = key_at;
+        s.key_n = key_n;
+        s.sig_at = sig_at;
+        s.ref = ref;
+        w.sets.push_back(s);
+    }
+    // the sets of block blk at ssz[off, off + len); false when its framing is malformed
+    bool block(uint32_t blk, uint64_t off, uint64_t len, bool skip_proposal) {
+        using namespace block_layout;
+        Span sb[1], v[1], bv[N_BODY_VAR];
+        if (!read_offsets(ssz + off, len, SIGNED_BLOCK_FIXED, FIRST_VAR_POS, sb)) return false;
+        const uint64_t m = off + SIGNED_BLOCK_FIXED, mlen = sb[0].len;
+        if (!read_offsets(ssz + m, mlen, BLOCK_FIXED, BLOCK_VAR_POS, v)) return false;
+        const uint64_t body = m + v[0].off, blen = v[0].len;
+        if (!read_offsets(ssz + body, blen, fl.body_fixed, BODY_VAR_POS, bv)) return false;
+        const uint64_t slot = rd64(ssz + m), epoch = slot / SLOTS_PER_EPOCH;
+        w.slot.push_back(slot);
+        w.proposer.push_back(rd64(ssz + m + 8));
+        // proposal: the caller's block root; randao: the epoch
+        if (!skip_proposal)
+            push(blk, 0, LHB200_BSET_PROPOSAL, KEY_PROPOSER, 0, off + 4,
+                 describe(BSO_ROOT, 0, 0, epoch, DOMAIN_BEACON_PROPOSER));
+        push(blk, 0, LHB200_BSET_RANDAO, KEY_PROPOSER, 0, body, describe(BSO_EPOCH, 0, 0, epoch, DOMAIN_RANDAO));
+        // ProposerSlashing: two SignedBeaconBlockHeaders of 208 bytes
+        const Span ps = bv[B_PROPOSER_SLASHINGS];
+        if (!ps.fits(416, 16)) return false;
+        for (uint64_t j = 0; j < ps.len / 416; j++)
+            for (uint32_t k = 0; k < 2; k++) {
+                const uint64_t h = body + ps.off + 416 * j + 208 * k;
+                push(blk, (uint16_t)(2 * j + k), LHB200_BSET_PROPOSER_SLASHING, KEY_INDEX, h + 8, h + 112,
+                     describe(BSO_HEADER, h, 112, rd64(ssz + h) / SLOTS_PER_EPOCH, DOMAIN_BEACON_PROPOSER));
+            }
+        // AttesterSlashing: two IndexedAttestations {attesting_indices offset, data, signature}
+        std::vector<uint64_t> b;
+        const Span as = bv[B_ATTESTER_SLASHINGS];
+        if (!item_bounds(ssz + body + as.off, as.len, fl.max_attester_slashings, b)) return false;
+        for (size_t j = 0; j + 1 < b.size(); j++) {
+            const uint64_t q = body + as.off + b[j];
+            Span a[2];
+            if (!read_offsets(ssz + q, b[j + 1] - b[j], 8, ATTESTER_SLASHING_VAR_POS, a)) return false;
+            for (uint32_t k = 0; k < 2; k++) {
+                const uint64_t ia = q + a[k].off;
+                Span x[1];
+                if (!read_offsets(ssz + ia, a[k].len, 228, FIRST_VAR_POS, x) || !x[0].fits(8, fl.max_attesting_indices))
+                    return false;
+                push(blk, (uint16_t)(2 * j + k), LHB200_BSET_ATTESTER_SLASHING, KEY_INDEX_LIST, ia + x[0].off, ia + 132,
+                     describe(BSO_ATT_DATA, ia + 4, 128, rd64(ssz + ia + 4 + 88), DOMAIN_BEACON_ATTESTER),
+                     (uint32_t)(x[0].len / 8));
+            }
+        }
+        // Attestations, framed as lhb200_beacon_block_roots frames them
+        const Span at = bv[B_ATTESTATIONS];
+        if (!item_bounds(ssz + body + at.off, at.len, fl.max_attestations, b)) return false;
+        const uint32_t fixed = fl.attestation_fixed;
+        for (size_t j = 0; j + 1 < b.size(); j++) {
+            const uint64_t r = body + at.off + b[j], rlen = b[j + 1] - b[j];
+            Span x[1];
+            if (!read_offsets(ssz + r, rlen, fixed, FIRST_VAR_POS, x) || x[0].len == 0 || ssz[r + rlen - 1] == 0) return false;
+            const uint64_t bitlen = 8 * (x[0].len - 1) + 31 - __builtin_clz(ssz[r + rlen - 1]);
+            if (bitlen > fl.max_aggregation_bits) return false;
+            const uint8_t* p = ssz + r;
+            if (fixed == ATT_FIXED_ELECTRA) {   // in a block: committee_bits at 132, signature at 140
+                w.atts.insert(w.atts.end(), p, p + 132);
+                w.atts.insert(w.atts.end(), p + 140, p + 236);
+                w.atts.insert(w.atts.end(), p + 132, p + 140);
+                w.atts.insert(w.atts.end(), p + 236, p + rlen);
+                w.att_sig.push_back(r + 140);
+            } else {
+                w.atts.insert(w.atts.end(), p, p + rlen);
+                w.att_sig.push_back(r + ATT_SIG);
+            }
+            w.att_offs.push_back(w.atts.size());
+            push(blk, (uint16_t)j, LHB200_BSET_ATTESTATION, KEY_ATTESTATION, 0, w.att_sig.back(),
+                 (uint32_t)w.att_sig.size() - 1);
+        }
+        // SignedVoluntaryExit {epoch, validator_index, signature}: EIP-7044 fixes the domain at Capella's from Deneb on
+        const Span ex = bv[B_EXITS];
+        if (!ex.fits(112, 16)) return false;
+        for (uint64_t j = 0; j < ex.len / 112; j++) {
+            const uint64_t e = body + ex.off + 112 * j;
+            push(blk, (uint16_t)j, LHB200_BSET_EXIT, KEY_INDEX, e + 8, e + 16,
+                 describe(BSO_EXIT, e, 16, rd64(ssz + e), DOMAIN_VOLUNTARY_EXIT));
+            if (fork >= LHB200_FORK_DENEB) w.desc.back().pad = 1;   // a fixed version, set from the chain versions
+        }
+        // SyncAggregate over the parent root at the previous slot's epoch; no set for zero bits with the infinity
+        // signature
+        if (fl.body_fields > 8) {
+            bool any = false, inf = ssz[body + SYNC_SIG] == 0xc0;
+            for (uint32_t k = 0; k < 64; k++) any |= ssz[body + SYNC_BITS + k] != 0;
+            for (uint32_t k = 1; k < 96; k++) inf &= ssz[body + SYNC_SIG + k] == 0;
+            if (any || !inf)
+                push(blk, 0, LHB200_BSET_SYNC_AGGREGATE, KEY_SYNC, body + SYNC_BITS, body + SYNC_SIG,
+                     describe(BSO_ROOT, m + 16, 32, (std::max<uint64_t>(slot, 1) - 1) / SLOTS_PER_EPOCH,
+                              DOMAIN_SYNC_COMMITTEE));
+        }
+        // SignedBLSToExecutionChange {validator_index, from_bls_pubkey, to_execution_address, signature}: the key is
+        // the message's own pubkey (no registry lookup) and the domain uses genesis_fork_version
+        if (fl.body_fields > 10) {
+            const Span bc = bv[B_BLS_CHANGES];
+            if (!bc.fits(172, 16)) return false;
+            for (uint64_t j = 0; j < bc.len / 172; j++) {
+                const uint64_t c = body + bc.off + 172 * j;
+                push(blk, (uint16_t)j, LHB200_BSET_BLS_CHANGE, KEY_LOCAL, c + 8, c + 76,
+                     describe(BSO_BLS_CHANGE, c, 76, 0, DOMAIN_BLS_TO_EXECUTION_CHANGE),
+                     (uint32_t)(w.local_pks.size() / 48));
+                w.desc.back().pad = 2;   // genesis_fork_version
+                w.local_pks.insert(w.local_pks.end(), ssz + c + 8, ssz + c + 56);
+            }
+        }
+        // SignedConsolidation {source_index, target_index, epoch, signature}: genesis_fork_version
+        if (fl.body_fields > 12) {
+            const Span cs = bv[B_CONSOLIDATIONS];
+            if (!cs.fits(120, 1)) return false;
+            for (uint64_t j = 0; j < cs.len / 120; j++) {
+                const uint64_t c = body + cs.off + 120 * j;
+                push(blk, (uint16_t)j, LHB200_BSET_CONSOLIDATION, KEY_PAIR, c, c + 24,
+                     describe(BSO_CONSOLIDATION, c, 24, 0, DOMAIN_CONSOLIDATION));
+                w.desc.back().pad = 2;   // genesis_fork_version
+            }
+        }
+        return true;
+    }
+};
+
+// A literal of the state's fixed part (the handle keeps the literal chunks current through patches)
+bool state_literal(const lhb200_state* st, uint64_t off, uint32_t n, uint8_t* out) {
+    for (const Plan::LitSrc& ls : st->plan.lit_src)
+        if (ls.src_off == off && ls.n == n) {
+            memcpy(out, &st->plan.lit[(size_t)ls.lit_index * 32], n);
+            return true;
+        }
+    return false;
+}
+
+}  // namespace
+}  // namespace lhb200
+
+namespace {
+// the calling thread's last lhb200_block_signatures_verify: its own launches (the batch check's excluded) and the host
+// synchronises it made, the batch check's included (lhb200_debug_block_signatures_counts)
+thread_local uint64_t t_block_launches = 0, t_block_syncs = 0;
+}
+
+extern "C" {
+
+int32_t lhb200_debug_block_signatures_counts(uint64_t* launches, uint64_t* syncs) {
+    if (launches) *launches = t_block_launches;
+    if (syncs) *syncs = t_block_syncs;
+    return LHB200_OK;
+}
+
+int32_t lhb200_block_signatures_verify(const uint8_t* ssz, const uint64_t* offsets, uint32_t n, int32_t fork,
+                                       uint32_t flags, const uint8_t* block_roots, lhb200_state* st,
+                                       const lhb200_committee_cache* const* caches, uint32_t n_caches,
+                                       const lhb200_pubkey_table* table, const lhb200_chain_versions* versions,
+                                       const uint64_t* rands, uint64_t n_rands, uint8_t* ok, uint8_t* block_status,
+                                       lhb200_block_set* sets, uint64_t sets_cap, uint64_t* n_sets) {
+    const char* fn = "block_signatures_verify";
+    LHB_REQUIRE_READY();
+    t_block_launches = t_block_syncs = 0;
+    const uint64_t launches0 = ctx().launches.load();
+    uint64_t syncs = 0;
+    if (!ssz || !offsets || !block_roots || !st || !caches || !table || !versions || !ok || !block_status || !sets ||
+        !n_sets) {
+        set_error("%s: null argument", fn);
+        return LHB200_EINVAL;
+    }
+    if (n == 0) { set_error("%s: no blocks", fn); return LHB200_EINVAL; }
+    const ForkLayout* fl = fork_layout(fork);
+    if (!fl) { set_error("%s: unknown fork %d", fn, fork); return LHB200_EINVAL; }
+    if (flags & ~(uint32_t)LHB200_BLOCK_SKIP_PROPOSAL) { set_error("%s: unknown flags 0x%x", fn, flags); return LHB200_EINVAL; }
+    if (n_caches == 0 || n_caches > ATT_MAX_CACHES) {
+        set_error("%s: %u committee caches (1 to %u)", fn, n_caches, ATT_MAX_CACHES);
+        return LHB200_EINVAL;
+    }
+    for (uint32_t k = 0; k < n_caches; k++) {
+        if (!caches[k]) { set_error("%s: null committee cache", fn); return LHB200_EINVAL; }
+        for (uint32_t j = 0; j < k; j++)
+            if (caches[j]->info.epoch == caches[k]->info.epoch) {
+                set_error("%s: two committee caches of epoch %llu", fn, (unsigned long long)caches[k]->info.epoch);
+                return LHB200_EINVAL;
+            }
+    }
+    for (uint32_t i = 0; i < n; i++)
+        if (offsets[i] > offsets[i + 1]) { set_error("%s: offsets not monotone", fn); return LHB200_EINVAL; }
+    Ctx& c = ctx();
+    // the state's inputs and literals
+    CommitteeInputs in;
+    uint8_t fork_lit[16], gvr[32];
+    {
+        std::lock_guard<std::recursive_mutex> g(c.mu);
+        if (int32_t rc = committee_inputs(st, fn, in)) return rc;
+        if (st->shard.fork != fork) {
+            set_error("%s: fork %d blocks against a fork %d state", fn, fork, st->shard.fork);
+            return LHB200_EINVAL;
+        }
+        using namespace state_layout;
+        if (!state_literal(st, O_FORK, 4, fork_lit) || !state_literal(st, O_FORK + 4, 4, fork_lit + 4) ||
+            !state_literal(st, O_FORK + 8, 8, fork_lit + 8) || !state_literal(st, O_GVR, 32, gvr)) {
+            set_error("%s: the handle has no fork or genesis_validators_root literal", fn);
+            return LHB200_EINVAL;
+        }
+    }
+    // 1. the host walk: sets, descriptors, objects and attestation records; every refusal comes before a launch
+    BlockWalk w;
+    BlockWalker walker{ssz, *fl, fork, w};
+    const bool skip = flags & LHB200_BLOCK_SKIP_PROPOSAL;
+    for (uint32_t i = 0; i < n; i++) {
+        const uint64_t len = offsets[i + 1] - offsets[i];
+        if (!walker.block(i, offsets[i], len, skip)) {
+            set_error("%s: block %u: malformed SignedBeaconBlock offsets or lengths for this fork", fn, i);
+            return LHB200_EINVAL;
+        }
+    }
+    const uint64_t total_sets = w.sets.size();
+    *n_sets = total_sets;
+    if (sets_cap < total_sets || (rands && n_rands < total_sets)) {
+        set_error("%s: room for %llu sets and %llu scalars, the blocks contribute %llu", fn, (unsigned long long)sets_cap,
+                  (unsigned long long)(rands ? n_rands : 0), (unsigned long long)total_sets);
+        return LHB200_EINVAL;
+    }
+    if (rands)
+        for (uint64_t j = 0; j < total_sets; j++)
+            if (rands[j] == 0) { set_error("%s: zero random scalar", fn); return LHB200_EINVAL; }
+    // the domains' versions: get_domain over the state's fork, or the fixed chain versions
+    const uint64_t fork_epoch = rd64(fork_lit + 8);
+    for (BlockSetDesc& d : w.desc) {
+        d.version = d.pad == 1 ? be_word32(versions->capella_fork_version)
+                  : d.pad == 2 ? be_word32(versions->genesis_fork_version)
+                               : be_word32(fork_lit + (d.epoch < fork_epoch ? 0 : 4));
+        d.domain <<= 24;
+        d.pad = 0;
+    }
+    const uint32_t n_desc = (uint32_t)w.desc.size(), n_att = (uint32_t)w.att_sig.size(),
+                   n_local = (uint32_t)(w.local_pks.size() / 48);
+    // proposal objects are the caller's block roots
+    for (const BlockSet& s : w.sets)
+        if (s.kind == LHB200_BSET_PROPOSAL) {
+            w.desc[s.ref].off = w.objects.size();
+            w.objects.insert(w.objects.end(), block_roots + 32ull * s.block, block_roots + 32ull * s.block + 32);
+        }
+    bool want_sync = false;
+    for (const BlockSet& s : w.sets)
+        if (s.key_src == KEY_SYNC)
+            for (uint32_t k = 0; k < 64; k++) want_sync |= ssz[s.key_at + k] != 0;
+
+    lhb200_bls_batch* b = bls_pool_borrow((uint32_t)std::max<uint64_t>(total_sets, 1));
+    if (!b) return LHB200_ENOMEM;
+    struct Return { lhb200_bls_batch* b; ~Return() { bls_pool_return(b); } } ret{b};
+    cudaStream_t s = bls_batch_stream(b);
+    const uint64_t att_bytes = w.atts.size();
+    const size_t b_obj = align_up(w.objects.size() + 16, 256), b_desc = align_up(n_desc * sizeof(BlockSetDesc) + 16, 256),
+                 b_roots = align_up(32ull * n_desc + 16, 256), b_sync = align_up(4 * SYNC_MEMBERS, 256),
+                 b_att = align_up(att_bytes + 16, 256), b_aoff = align_up(8ull * (n_att + 1), 256),
+                 b_arec = align_up(37ull * n_att + 16, 256), b_koff = align_up(4ull * n_att + 16, 256),
+                 b_local = align_up(49ull * n_local + 16, 256);
+    const size_t h_sync = align_up(4 * SYNC_MEMBERS, 64), h_roots = align_up(32ull * n_desc, 64),
+                 h_arec = align_up(37ull * n_att, 64);
+    uint8_t* h = nullptr;
+    uint8_t* d = static_cast<uint8_t*>(bls_batch_aux(b, b_obj + b_desc + b_roots + b_sync + b_att + b_aoff + b_arec + b_koff +
+                                                            b_local,
+                                                     &h, h_sync + h_roots + h_arec + n_local + 64));
+    if (!d) return LHB200_ENOMEM;
+    uint8_t* d_obj = d;
+    BlockSetDesc* d_desc = reinterpret_cast<BlockSetDesc*>(d += b_obj);
+    uint8_t* d_roots = (d += b_desc);
+    uint32_t* d_sync = reinterpret_cast<uint32_t*>(d += b_roots);
+    uint8_t* d_att = (d += b_sync);
+    uint64_t* d_aoff = reinterpret_cast<uint64_t*>(d += b_att);
+    uint8_t* d_arec = (d += b_aoff);
+    uint32_t* d_koff = reinterpret_cast<uint32_t*>(d += b_arec);
+    uint8_t* d_local = (d += b_koff);
+    uint8_t* d_lst = d_local + 48ull * n_local;
+    uint32_t* hs = reinterpret_cast<uint32_t*>(h);
+    uint8_t* hr = h + h_sync;
+    uint8_t* ha = hr + h_roots;
+    uint8_t* h_local = ha + h_arec;
+
+    // 2. the state front under the library mutex: the proposers of the current epoch and the sync committee's indices
+    uint64_t proposers[SLOTS_PER_EPOCH];
+    const uint64_t current = in.slot / SLOTS_PER_EPOCH;
+    {
+        std::lock_guard<std::recursive_mutex> g(c.mu);
+        // the handle as it is now: the record pointer and count may have moved, and the slot, fork and root the sets
+        // were described with must still hold
+        const uint64_t slot0 = in.slot;
+        uint8_t lit_now[48];
+        using namespace state_layout;
+        if (int32_t rc = committee_inputs(st, fn, in)) return rc;
+        if (in.slot != slot0 || !state_literal(st, O_FORK, 4, lit_now) || !state_literal(st, O_FORK + 4, 4, lit_now + 4) ||
+            !state_literal(st, O_FORK + 8, 8, lit_now + 8) || !state_literal(st, O_GVR, 32, lit_now + 16) ||
+            memcmp(lit_now, fork_lit, 16) || memcmp(lit_now + 16, gvr, 32)) {
+            set_error("%s: the state's slot, fork or genesis_validators_root changed during the call", fn);
+            return LHB200_EINVAL;
+        }
+        SeedTable tab{};
+        tab.n = SLOTS_PER_EPOCH;
+        for (uint32_t k = 0; k < SLOTS_PER_EPOCH; k++)
+            tab.r[k] = {current, current * SLOTS_PER_EPOCH + k, DOMAIN_BEACON_PROPOSER, 1};
+        if (int32_t rc = sample_validators(in, fn, current, tab, 1, proposers)) return rc;
+        syncs++;   // sample_validators' read-back
+        if (want_sync) {
+            const uint8_t* committee = st->copies[st->marks[22].copies].dst;
+            const uint32_t grid = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(ceil_div(in.n, SYNC_RESOLVE_THREADS), 1), 1024);
+            LHB_CUDA(cudaMemsetAsync(d_sync, 0xff, 4 * SYNC_MEMBERS, c.stream));
+            k_sync_committee_resolve<<<grid, SYNC_RESOLVE_THREADS, 0, c.stream>>>(in.vals, in.n, committee, d_sync);
+            count_launch();
+            LHB_CUDA(cudaGetLastError());
+            LHB_CUDA(cudaMemcpyAsync(hs, d_sync, 4 * SYNC_MEMBERS, cudaMemcpyDeviceToHost, c.stream));
+            LHB_CUDA(cudaStreamSynchronize(c.stream));
+            syncs++;
+        }
+    }
+
+    // 3. every signing root, the changes' keys and the attestations' indexing on the device, one read-back
+    const uint64_t table_len = lhb200_pubkey_table_len(table), limit = std::min<uint64_t>(table_len, in.n);
+    if (n_local) {
+        LHB_CUDA(cudaMemcpyAsync(d_local, w.local_pks.data(), 48ull * n_local, cudaMemcpyHostToDevice, s));
+        if (int32_t rc = bls_batch_local_keys(b, d_local, n_local, d_lst)) return rc;
+        LHB_CUDA(cudaMemcpyAsync(h_local, d_lst, n_local, cudaMemcpyDeviceToHost, s));
+    }
+    LHB_CUDA(cudaMemcpyAsync(d_obj, w.objects.data(), w.objects.size(), cudaMemcpyHostToDevice, s));
+    LHB_CUDA(cudaMemcpyAsync(d_desc, w.desc.data(), n_desc * sizeof(BlockSetDesc), cudaMemcpyHostToDevice, s));
+    BlockRootParams rp{d_obj, d_desc, n_desc, {}, d_roots};
+    for (int k = 0; k < 8; k++) rp.gvr[k] = be_word32(gvr + 4 * k);
+    k_block_set_roots<<<(unsigned)ceil_div(n_desc, BLOCK_ROOT_THREADS), BLOCK_ROOT_THREADS, 0, s>>>(rp);
+    count_launch();
+    AttParams ap{};
+    if (n_att) {
+        LHB_CUDA(cudaMemcpyAsync(d_att, w.atts.data(), att_bytes, cudaMemcpyHostToDevice, s));
+        LHB_CUDA(cudaMemcpyAsync(d_aoff, w.att_offs.data(), 8ull * (n_att + 1), cudaMemcpyHostToDevice, s));
+        ap.ssz = d_att;
+        ap.offs = d_aoff;
+        ap.n = n_att;
+        ap.electra = fork == LHB200_FORK_ELECTRA;
+        ap.n_caches = n_caches;
+        for (uint32_t k = 0; k < n_caches; k++)
+            ap.cache[k] = {caches[k]->d_shuffling, caches[k]->info.epoch, (uint32_t)caches[k]->info.n_active,
+                           (uint32_t)caches[k]->info.committees_per_slot};
+        ap.table_len = limit;
+        ap.fork_epoch = fork_epoch;
+        ap.version[0] = be_word32(fork_lit);
+        ap.version[1] = be_word32(fork_lit + 4);
+        for (int k = 0; k < 8; k++) ap.gvr[k] = rp.gvr[k];
+        ap.roots = d_arec;
+        ap.counts = reinterpret_cast<uint32_t*>(d_arec + 32ull * n_att);
+        ap.status = d_arec + 36ull * n_att;
+        k_attestation_index_count<<<(unsigned)ceil_div(n_att, ATT_COUNT_WARPS), 32 * ATT_COUNT_WARPS, 0, s>>>(ap);
+        count_launch();
+        LHB_CUDA(cudaMemcpyAsync(ha, d_arec, 37ull * n_att, cudaMemcpyDeviceToHost, s));
+    }
+    LHB_CUDA(cudaGetLastError());
+    LHB_CUDA(cudaMemcpyAsync(hr, d_roots, 32ull * n_desc, cudaMemcpyDeviceToHost, s));
+    LHB_CUDA(cudaStreamSynchronize(s));
+    syncs++;
+    const uint32_t* a_counts = reinterpret_cast<const uint32_t*>(ha + 32ull * n_att);
+    const uint8_t* a_st = ha + 36ull * n_att;
+
+    // 4. construction codes and the host-known keys
+    std::vector<uint32_t> hkeys;
+    for (BlockSet& x : w.sets) {
+        if (x.key_src == KEY_ATTESTATION) continue;
+        x.key_lo = (uint32_t)hkeys.size();
+        auto key = [&](uint64_t v) {
+            if (v >= limit) x.status = LHB200_ATT_UNKNOWN_VALIDATOR;
+            else hkeys.push_back((uint32_t)v);
+        };
+        const uint64_t slot = w.slot[x.block];
+        switch (x.key_src) {
+        case KEY_PROPOSER: {
+            const uint64_t p = proposers[slot % SLOTS_PER_EPOCH];
+            if (slot / SLOTS_PER_EPOCH != current) x.status = LHB200_BLOCK_SLOT_OUT_OF_BOUNDS;
+            else if (x.kind == LHB200_BSET_PROPOSAL && p != w.proposer[x.block]) x.status = LHB200_BLOCK_INCORRECT_PROPOSER;
+            else key(p);
+            break;
+        }
+        case KEY_INDEX: key(rd64(ssz + x.key_at)); break;
+        case KEY_PAIR: key(rd64(ssz + x.key_at)); if (!x.status) key(rd64(ssz + x.key_at + 8)); break;
+        case KEY_INDEX_LIST:
+            for (uint32_t k = 0; k < x.key_n && !x.status; k++) key(rd64(ssz + x.key_at + 8ull * k));
+            break;
+        case KEY_LOCAL:   // PublicKey::deserialize + key_validate on the device; the key follows the table's
+            if (h_local[x.key_n]) x.status = LHB200_BLOCK_PUBKEY_DECOMPRESSION;
+            else hkeys.push_back((uint32_t)(table_len + x.key_n));
+            break;
+        default:   // KEY_SYNC: the participants' resolved indices, in committee order
+            for (uint32_t m = 0; m < SYNC_MEMBERS && !x.status; m++)
+                if ((ssz[x.key_at + m / 8] >> (m % 8)) & 1) {
+                    if (hs[m] == UINT32_MAX || hs[m] >= limit) x.status = LHB200_BLOCK_PUBKEY_DECOMPRESSION;
+                    else hkeys.push_back(hs[m]);
+                }
+        }
+        if (x.status) hkeys.resize(x.key_lo);
+        x.key_cnt = (uint32_t)hkeys.size() - x.key_lo;
+    }
+
+
+    // 5. the batch: the constructed host-keyed sets, then the constructed attestations, each group in push order
+    std::vector<uint32_t> pk_off(1, 0), batch_set, hk(n_att, UINT32_MAX);
+    std::vector<uint8_t> sigs, msgs;
+    std::vector<uint64_t> r_sets;
+    auto add = [&](uint64_t j, uint32_t n_keys, const uint8_t* msg) {
+        pk_off.push_back(pk_off.back() + n_keys);
+        batch_set.push_back((uint32_t)j);
+        sigs.insert(sigs.end(), ssz + w.sets[j].sig_at, ssz + w.sets[j].sig_at + 96);
+        msgs.insert(msgs.end(), msg, msg + 32);
+        if (rands) r_sets.push_back(rands[j]);
+    };
+    for (uint64_t j = 0; j < total_sets; j++) {
+        const BlockSet& x = w.sets[j];
+        if (x.key_src == KEY_ATTESTATION || x.status) continue;
+        add(j, x.key_cnt, hr + 32ull * x.ref);
+    }
+    for (uint64_t j = 0; j < total_sets; j++) {
+        BlockSet& x = w.sets[j];
+        if (x.key_src != KEY_ATTESTATION) continue;
+        x.status = a_st[x.ref];
+        if (x.status) continue;
+        if ((uint64_t)pk_off.back() + a_counts[x.ref] >= UINT32_MAX) { set_error("%s: more than 2^32 keys", fn); return LHB200_EINVAL; }
+        hk[x.ref] = pk_off.back();
+        add(j, a_counts[x.ref], ha + 32ull * x.ref);
+    }
+    const uint32_t n_batch = (uint32_t)batch_set.size();
+    uint32_t* d_keys = nullptr;
+    std::vector<uint8_t> set_st(n_batch);
+    uint8_t verdict = 0;
+    if (n_batch) {
+        if (int32_t rc = bls_batch_stage_table(b, table, sigs.data(), msgs.data(), pk_off.data(),
+                                               rands ? r_sets.data() : nullptr, n_batch, &d_keys))
+            return rc;
+        if (!hkeys.empty())
+            LHB_CUDA(cudaMemcpyAsync(d_keys, hkeys.data(), 4 * hkeys.size(), cudaMemcpyHostToDevice, s));
+        if (n_att) {
+            LHB_CUDA(cudaMemcpyAsync(d_koff, hk.data(), 4ull * n_att, cudaMemcpyHostToDevice, s));
+            const AttWrite wr{d_koff, d_keys, nullptr, nullptr};
+            k_attestation_index_write<<<n_att, ATT_WRITE_THREADS, 0, s>>>(ap, wr);
+            count_launch();
+            LHB_CUDA(cudaGetLastError());
+        }
+        // 6. the batch check
+        if (int32_t rc = bls_batch_finish(b, &verdict, set_st.data())) return rc;
+        syncs++;   // the batch check's result
+    }
+
+    // the outputs
+    bool constructed = true;
+    for (uint64_t j = 0; j < total_sets; j++) constructed &= w.sets[j].status == 0;
+    for (uint32_t q = 0; q < n_batch; q++) w.sets[batch_set[q]].status = set_st[q];
+    memset(block_status, 0, n);
+    for (uint64_t j = 0; j < total_sets; j++) {
+        const BlockSet& x = w.sets[j];
+        lhb200_block_set& o = sets[j];
+        o.block = x.block;
+        o.item = x.item;
+        o.kind = x.kind;
+        o.status = x.status;
+        memcpy(o.signing_root, x.key_src == KEY_ATTESTATION ? ha + 32ull * x.ref : hr + 32ull * x.ref, 32);
+        if (x.status && !block_status[x.block]) block_status[x.block] = x.status;
+    }
+    *ok = constructed && n_batch && verdict == 1 ? 1 : 0;
+    t_block_launches = ctx().launches.load() - launches0 - bls_last_batch_launches();
+    t_block_syncs = syncs;
+    return LHB200_OK;
 }
 
 }  // extern "C"

@@ -531,3 +531,199 @@ def signed_attestations(cache, kind, n, sks, fork_info, gvr=MAINNET_GVR, seed=0,
     sigs = bls.sign(b"".join(a.to_bytes(32, "big") for a in agg), msgs)
     return [attestation_ssz(bits, data, sigs[96 * j:96 * j + 96], cbits)
             for j, (bits, data, cbits, _) in enumerate(records)]
+
+
+# ---------------------------------------------------------------------------------------------------------
+# Signed blocks over a resident world (lhb200_block_signatures_verify, lighthouse_b200.block_signatures).  Validator i
+# holds interop key i; every signature is (sum of its signers' secret keys mod r) . H(signing root) from `sign_fn`
+# (default: the CUDA library's lhb200_sign), which is the aggregate of the signers' own signatures.
+O_STATE_GVR, O_STATE_SLOT, O_STATE_FORK, O_STATE_VAL_OFF, O_STATE_CSC = 8, 40, 48, 524552, 2687381
+DOMAIN_PROPOSER, DOMAIN_ATTESTER, DOMAIN_RANDAO, DOMAIN_EXIT, DOMAIN_SYNC = 0, 1, 2, 4, 7
+DOMAIN_BLS_TO_EXECUTION_CHANGE, DOMAIN_CONSOLIDATION = 0x0A, 0x0B
+INFINITY_SIGNATURE = b"\xc0" + bytes(95)
+
+
+def compute_domain(domain_type, version, gvr):
+    return domain_type.to_bytes(4, "little") + _sha(bytes(version) + bytes(28) + bytes(gvr))[:28]
+
+
+def _chunk(v):
+    return struct.pack("<Q", v) + bytes(24)
+
+
+def header_root(slot, proposer_index, parent_root, state_root, body_root):
+    z = bytes(32)
+    return _sha(_sha(_sha(_chunk(slot) + _chunk(proposer_index)) + _sha(parent_root + state_root))
+                + _sha(_sha(body_root + z) + _sha(z + z)))
+
+
+def g1_compress(pk96):
+    """48-byte compressed form of a 96-byte uncompressed G1 point (x || y, big-endian; not infinity)."""
+    p = 0x1A0111EA397FE69A4B1BA7B6434BACD764774B84F38512BF6730D2A0F6B0F6241EABFFFEB153FFFFB9FEFFFFFFFFAAAB
+    y = int.from_bytes(pk96[48:], "big")
+    out = bytearray(pk96[:48])
+    out[0] |= 0x80 | (0x20 if y > (p - 1) // 2 else 0)
+    return bytes(out)
+
+
+def block_signature_state(n, fork, slot, fork_versions, pubkeys48, sync_members=None, seed=5):
+    """SSZ of a BeaconState<fork> of n validators at `slot` whose records carry `pubkeys48` (n x 48 bytes, validator i's
+    compressed key), whose fork is fork_versions = (previous_version, current_version, epoch), and whose
+    current_sync_committee names `sync_members` (512 validator indices; default 7919 i mod n)."""
+    ssz = bytearray(beacon_state_deneb_ssz(n, seed=seed, fork=fork, n_votes=3, n_hist_roots=5, n_summaries=2))
+    struct.pack_into("<Q", ssz, O_STATE_SLOT, slot)
+    prev, cur, epoch = fork_versions
+    ssz[O_STATE_FORK:O_STATE_FORK + 16] = bytes(prev) + bytes(cur) + struct.pack("<Q", epoch)
+    lo = struct.unpack_from("<I", ssz, O_STATE_VAL_OFF)[0]
+    v = np.frombuffer(ssz, dtype=np.uint8, count=121 * n, offset=lo).reshape(n, 121)
+    v[:, :48] = np.frombuffer(bytes(pubkeys48), dtype=np.uint8).reshape(n, 48)
+    if fork != "base":
+        if sync_members is None:
+            sync_members = [(7919 * i) % n for i in range(512)]
+        pk = np.frombuffer(bytes(pubkeys48), dtype=np.uint8).reshape(n, 48)
+        ssz[O_STATE_CSC:O_STATE_CSC + 512 * 48] = pk[np.asarray(sync_members, dtype=np.int64)].tobytes()
+    return bytes(ssz)
+
+
+def _attestation_value(ssz, electra):
+    """Attestation SSZ in lhb200_attestations_verify's layout -> the block body's value"""
+    data = ssz[4:132]
+    fixed = 236 if electra else 228
+    raw = np.frombuffer(ssz[fixed:], dtype=np.uint8)
+    bits = np.unpackbits(raw, bitorder="little")[:8 * (len(raw) - 1) + int(raw[-1]).bit_length() - 1]
+    s, i, bbr, se, sr, te, tr = struct.unpack_from("<QQ32sQ32sQ32s", data)
+    v = {"aggregation_bits": [bool(b) for b in bits], "signature": ssz[132:228],
+         "data": {"slot": s, "index": i, "beacon_block_root": bbr, "source": {"epoch": se, "root": sr},
+                  "target": {"epoch": te, "root": tr}}}
+    if electra:
+        cb = struct.unpack_from("<Q", ssz, 228)[0]
+        v["committee_bits"] = [bool((cb >> k) & 1) for k in range(64)]
+    return v
+
+
+def signed_beacon_block(fork, slot, proposer, sks, state_fork, gvr, versions, block_root_fn, sign_fn=None, seed=0,
+                        attestations=(), n_proposer_slashings=1, n_attester_slashings=1, slashing_size=3,
+                        n_exits=2, sync_committee=None, sync_participation=0.9, n_consolidations=None,
+                        n_validators=None, n_bls_changes=None, bls_change_pubkeys=None, pk_fn=None):
+    """-> (SignedBeaconBlock SSZ, block root) of a BeaconBlock<fork> at `slot` by `proposer`, every set signed with the
+    interop keys `sks`: the proposal (over block_root_fn(BeaconBlock SSZ)), the RANDAO reveal, n proposer and attester
+    slashings (slashing_size signers each), `attestations` (SSZ in lhb200_attestations_verify's layout, e.g.
+    signed_attestations), n exits, the sync aggregate over `sync_committee` (its 512 validator indices) with
+    `sync_participation` of the bits set (0: all zero, with the infinity signature), from Capella n BLS-to-execution
+    changes (2 by default) signed by keys outside the registry (`bls_change_pubkeys` replaces their from_bls_pubkey
+    bytes, for keys that must fail to decode; pk_fn(sk bytes) -> compressed keys, default the CUDA library's
+    lhb200_sk_to_pk), and Electra's consolidations (1 by default).  state_fork = (previous_version, current_version, epoch); versions = (genesis_fork_version,
+    capella_fork_version).  Deposits (2) carry no set.  Bellatrix on, the payload has 4 small transactions."""
+    from . import ssz_schema as S
+    if sign_fn is None:
+        from . import bls
+        sign_fn = bls.sign
+    rng = np.random.default_rng([seed, slot, 11])
+    n_val = n_validators or len(sks)
+    electra, epoch = fork == "electra", slot // 32
+    prev, cur, fork_epoch = state_fork
+
+    def domain(dtype, e):
+        return compute_domain(dtype, prev if e < fork_epoch else cur, gvr)
+
+    def rb(n):
+        return rng.integers(0, 256, size=n, dtype=np.uint8).tobytes()
+
+    def pick(k):
+        return sorted(int(x) for x in rng.choice(n_val, size=k, replace=False))
+
+    todo = []   # (signers, signing root, setter)
+
+    def signed(signers, root, setter):
+        todo.append((signers, root, setter))
+
+    if electra:
+        block, _ = beacon_block_electra(seed=seed + 1, n_attestations=0, n_attester_slashings=0, n_consolidations=0,
+                                        n_deposit_requests=1, n_withdrawal_requests=1, n_transactions=4, n_exits=0,
+                                        n_bls_changes=0, n_proposer_slashings=0, n_deposits=2)
+    else:
+        block, _ = beacon_block_deneb(seed=seed + 1, n_attestations=0, n_transactions=4, n_proposer_slashings=0,
+                                      n_attester_slashings=0, n_deposits=2, n_exits=0, n_bls_changes=0, fork=fork)
+    body = block["body"]
+    block.update(slot=slot, proposer_index=proposer, parent_root=_sha(b"parent" + struct.pack("<QQ", seed, slot)))
+    signed([proposer], _sha(_chunk(epoch) + domain(DOMAIN_RANDAO, epoch)), lambda s: body.update(randao_reveal=s))
+    body["proposer_slashings"] = []
+    for j in range(n_proposer_slashings):
+        v, hs = pick(1)[0], int(rng.integers(0, slot + 1))
+        ps = {}
+        for k in (1, 2):
+            h = {"slot": hs, "proposer_index": v, "parent_root": rb(32), "state_root": rb(32), "body_root": rb(32)}
+            root = header_root(hs, v, h["parent_root"], h["state_root"], h["body_root"])
+            ps["signed_header_%d" % k] = {"message": h, "signature": None}
+            signed([v], _sha(root + domain(DOMAIN_PROPOSER, hs // 32)),
+                   lambda s, d=ps["signed_header_%d" % k]: d.update(signature=s))
+        body["proposer_slashings"].append(ps)
+    body["attester_slashings"] = []
+    for j in range(n_attester_slashings):
+        sl = {}
+        for k in (1, 2):
+            idx = pick(slashing_size)
+            data = attestation_data_ssz(max(slot - 1, 0), 0, rb(32), (max(epoch - 1, 0), rb(32)), (epoch, rb(32)))
+            s_, i_, bbr, se, sr, te, tr = struct.unpack_from("<QQ32sQ32sQ32s", data)
+            sl["attestation_%d" % k] = {"attesting_indices": idx, "signature": None, "data": {
+                "slot": s_, "index": i_, "beacon_block_root": bbr, "source": {"epoch": se, "root": sr},
+                "target": {"epoch": te, "root": tr}}}
+            signed(idx, _sha(attestation_data_root(data) + domain(DOMAIN_ATTESTER, te)),
+                   lambda s, d=sl["attestation_%d" % k]: d.update(signature=s))
+        body["attester_slashings"].append(sl)
+    body["attestations"] = [_attestation_value(a, electra) for a in attestations]
+    body["voluntary_exits"] = []
+    for j in range(n_exits):
+        v, e = pick(1)[0], int(rng.integers(0, epoch + 1))
+        ex = {"message": {"epoch": e, "validator_index": v}, "signature": None}
+        d = compute_domain(DOMAIN_EXIT, versions[1], gvr) if fork in ("deneb", "electra") else domain(DOMAIN_EXIT, e)
+        signed([v], _sha(_sha(_chunk(e) + _chunk(v)) + d), lambda s, x=ex: x.update(signature=s))
+        body["voluntary_exits"].append(ex)
+    if fork != "base":
+        bits = [False] * 512
+        if sync_participation > 0:
+            bits = [bool(b) for b in rng.random(512) < sync_participation]
+        body["sync_aggregate"] = {"sync_committee_bits": bits, "sync_committee_signature": INFINITY_SIGNATURE}
+        if any(bits):
+            prev_slot = max(slot, 1) - 1
+            signers = [int(sync_committee[m]) for m in range(512) if bits[m]]
+            signed(signers, _sha(block["parent_root"] + domain(DOMAIN_SYNC, prev_slot // 32)),
+                   lambda s: body["sync_aggregate"].update(sync_committee_signature=s))
+    if fork in ("capella", "deneb", "electra"):
+        if pk_fn is None:
+            from . import bls
+            pk_fn = lambda b: bls.sk_to_pk(b)[0]
+        n_ch = 2 if n_bls_changes is None else n_bls_changes
+        csks = [int.from_bytes(_sha(b"bls-change" + struct.pack("<QQQ", seed, slot, j)), "little") % CURVE_ORDER
+                for j in range(n_ch)]
+        pks = pk_fn(b"".join(k.to_bytes(32, "big") for k in csks)) if n_ch else b""
+        body["bls_to_execution_changes"] = []
+        for j in range(n_ch):
+            pk = pks[48 * j:48 * j + 48] if bls_change_pubkeys is None else bls_change_pubkeys[j]
+            v, addr = pick(1)[0], rb(20)
+            ch = {"message": {"validator_index": v, "from_bls_pubkey": pk, "to_execution_address": addr},
+                  "signature": None}
+            root = _sha(_sha(_chunk(v) + _sha(pk[:32] + pk[32:] + bytes(16))) + _sha(addr + bytes(12) + bytes(32)))
+            todo.append((None, _sha(root + compute_domain(DOMAIN_BLS_TO_EXECUTION_CHANGE, versions[0], gvr)),
+                         lambda s, x=ch: x.update(signature=s), csks[j]))
+            body["bls_to_execution_changes"].append(ch)
+    if electra:
+        body["consolidations"] = []
+        for j in range(1 if n_consolidations is None else n_consolidations):
+            src, tgt = pick(2)
+            e = int(rng.integers(0, epoch + 1))
+            c = {"message": {"source_index": src, "target_index": tgt, "epoch": e}, "signature": None}
+            root = _sha(_sha(_chunk(src) + _chunk(tgt)) + _sha(_chunk(e) + bytes(32)))
+            signed([src, tgt], _sha(root + compute_domain(DOMAIN_CONSOLIDATION, versions[0], gvr)),
+                   lambda s, x=c: x.update(signature=s))
+            body["consolidations"].append(c)
+    def secret(t):   # (signers, root, setter) over registry keys, or (None, root, setter, sk) for an outside key
+        return t[3] if t[0] is None else sum(sks[v] for v in t[0]) % CURVE_ORDER or 1
+    sk_bytes = b"".join(secret(t).to_bytes(32, "big") for t in todo)
+    sigs = sign_fn(sk_bytes, b"".join(t[1] for t in todo))
+    for k, t in enumerate(todo):
+        t[2](sigs[96 * k:96 * k + 96])
+    msg = S.serialize(S.BEACON_BLOCK_BY_FORK[fork], block)
+    root = block_root_fn(msg)
+    sig = sign_fn(sks[proposer].to_bytes(32, "big"), _sha(root + domain(DOMAIN_PROPOSER, epoch)))
+    return struct.pack("<I", 100) + sig + msg, root
